@@ -61,8 +61,9 @@ def test_bn_prelu_fwd_bwd_vs_autograd(c, h, w, b, res, up):
     invstd = torch.rsqrt(var + 1e-5)
     scale = (gamma * invstd).contiguous()
     shift = (beta - mean * scale).contiguous()
-    # statistics + finalisation in ONE call (last CTA of the statistics kernel finalises) == nn.BatchNorm2d's bookkeeping
-    f_sums = torch.full((2 * c + 1,), 3.0, device=dev)       # the call zeroes it (sums + ticket)
+    # statistics + finalisation in ONE call (the reduction of the per-CTA partial rows finalises each channel) ==
+    # nn.BatchNorm2d's bookkeeping
+    f_sums = torch.full((2 * c + 1,), 3.0, device=dev)       # sums[0, 2c) are overwritten, whatever they held
     f_mean, f_inv, f_sc, f_sh = (torch.empty(c, device=dev) for _ in range(4))
     rm, rv = torch.full((c,), 0.25, device=dev), torch.full((c,), 2.0, device=dev)
     assert lib.ryolo_bn_stats_finalize(pt(zb), cs, b, h, w, c, pt(f_sums), 1e-5, 0.1, pt(gamma), pt(beta), pt(f_mean), pt(f_inv),

@@ -146,8 +146,10 @@ def test_first_layer_tensor_core_conv(cout, cs, shape):
     dict(batch=2, h=10, w=12, cin=160, cout=96, k=1, narrow=True),   # strides 160 / 96 (not tile multiples)
 ])
 def test_conv_wgrad_vs_torch(cfg):
-    """wgmma wgrad (K = pixels, MN-major operands, split-K atomics) vs torch.nn.grad.conv2d_weight in fp32 on the
-    same bf16-representable operands; tolerance 2e-3 of the gradient scale (fp32 atomics reorder the split-K sum)."""
+    """wgmma wgrad (K = pixels, MN-major operands, split-K partials added in split order) vs
+    torch.nn.grad.conv2d_weight in fp32 on the same bf16-representable operands; tolerance 2e-3 of the gradient scale
+    (the fp32 reference adds in yet another order).  The element-wise float64 bounds, the ksize 2 (space-to-depth) path
+    and uneven split counts are in tests/test_wgrad_gpu.py."""
     import ctypes
     import rotate_yolov3_b200 as pkg
     from rotate_yolov3_b200 import layout as L

@@ -68,8 +68,9 @@ def test_train_forward_backward_vs_reference_autograd():
     assert np.all(np.abs(ratio_all[big] - 1) <= 0.15), ratio_all[big]
     assert np.median(np.abs(ratio_all[big] - 1)) <= 0.02
     bnp = np.array([("BatchNorm2d" in n) or n.endswith("Conv2d.bias") for n in names])
-    # BN vectors of the stem layers are the noisiest quantities of the whole graph (few elements, deepest back-propagation
-    # path): single entries move by > 20 % between identical runs, the bulk stays within a few percent
+    # BN vectors of the stem layers are the noisiest quantities of the whole graph against the fp32 reference (few
+    # elements, deepest back-propagation path): bf16 rounding moves single entries by > 20 %, the bulk stays within a few
+    # percent.  Between identical runs they do not move at all (tests/test_determinism_gpu.py).
     assert np.median(cos_all[bnp]) >= 0.75 and np.all(np.abs(ratio_all[bnp] - 1) <= 0.35)
     assert np.median(np.abs(ratio_all[bnp] - 1)) <= 0.05
     # running statistics followed nn.BatchNorm2d (momentum 0.1, unbiased variance)

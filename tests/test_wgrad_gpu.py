@@ -1,0 +1,390 @@
+"""wgmma weight gradient (csrc/wgrad.cu) against float64, element by element, on the paths the training step takes.
+
+For bf16-exact x and dz the exact gradient is want = conv2d_weight(x, dz) in float64, and every fp32 addition the kernel
+makes can be off by at most half an ulp of the running sum, which is bounded by A = conv2d_weight(|x|, |dz|).  With random
+signs the rounding errors add like a random walk, so every entry must satisfy
+
+    |got - want| <= KAPPA * sqrt(n_add) * 2^-24 * A + TINY,     n_add = ceil(K / 16) + ksplit
+
+where K is the padded pixel count (the GEMM's K dimension, whole 64-pixel k-steps), K / 16 the sequential wgmma
+accumulations and ksplit the split-K partial sums that the last split adds in split order.  KAPPA = 1 for every shape,
+chosen from the first run on an H100 SXM (132 SMs, 700 W): the worst |got - want| / bound over all cases was 0.143
+(ksize 2, cin_pad 256, ksplit 4), 0.012-0.064 on the long-K cases.  A k-step of 64 pixels that is lost, or a split that
+is added twice, moves entries by O(sqrt(64)) products -- three orders of magnitude above the bound (ratio 1131 in
+test_bound_rejects_a_lost_k_step).
+
+wgrad_plan() mirrors the host heuristic of ryolo_conv_wgrad (tile width BN, taps per CTA TG, split count), so that each
+case can assert the path it covers and a change to the heuristic cannot silently drop coverage."""
+import ctypes
+import math
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+pytestmark = pytest.mark.gpu
+
+KAPPA = 1.0
+U = 2.0 ** -24
+TINY = 1e-30
+H100_SXM_SMS = 132
+
+
+def wgrad_plan(ksize, cin_pad, cout_pad, batch, h, w, sms):
+    """Python mirror of the launch heuristic in ryolo_conv_wgrad (csrc/wgrad.cu)"""
+    np_ = batch * (h + 2) * (w + 2)
+    taps = ksize * ksize
+    bn = 256 if cin_pad >= 192 else cin_pad
+    m_tiles = -(-cout_pad // 128)
+    n_tiles = -(-cin_pad // bn)
+    ksteps = -(-np_ // 64)
+    tg = 1
+    if bn <= 128:
+        tg = 3 if taps == 9 else (2 if taps == 4 else 1)
+    if tg * bn > 256:
+        tg = 1
+    tiles = (taps // tg) * m_tiles * n_tiles
+    ksplit, best = 1, 0.0
+    for waves in range(1, 5):
+        ks = max(1, waves * sms // tiles)
+        ctas = tiles * ks
+        eff = ctas / (-(-ctas // sms) * sms)
+        if eff > best + 1e-9:
+            best, ksplit = eff, ks
+        if eff >= 0.9:
+            break
+    max_split = -(-ksteps // 16)
+    ksplit = max(1, min(ksplit, max_split))
+    per_split = -(-ksteps // ksplit)
+    ksplit = -(-ksteps // per_split)
+    last = ksteps - (ksplit - 1) * per_split
+    return dict(bn=bn, tg=tg, tiles=tiles, ksteps=ksteps, ksplit=ksplit, per_split=per_split, last=last,
+                short_last=last < per_split, n_add=-(-ksteps * 64 // 16) + ksplit)
+
+
+def gemm_sms(reserved=0):
+    n = torch.cuda.get_device_properties(0).multi_processor_count
+    return n - reserved if n - reserved > 8 else n
+
+
+def _bf(t):
+    return t.to(torch.bfloat16).float()
+
+
+def _lib():
+    import rotate_yolov3_b200 as pkg
+    return pkg._lib
+
+
+def wgrad(dzb, zcs, cout_pad, xb, xcs, cin_pad, b, h, w, k, dw, stream=None):
+    L = _lib()
+    sp = ctypes.c_void_p(stream.cuda_stream) if stream is not None else L.stream_ptr(dw.device)
+    st = L.lib.ryolo_conv_wgrad(L.ptr(dzb), zcs, cout_pad, L.ptr(xb), xcs, cin_pad, b, h, w, k, L.ptr(dw), sp)
+    assert st == 0, L.last_error()
+
+
+def ref_wgrad(x, dz, k, stride=1):
+    """float64 weight gradient of the k x k conv (k = 2: taps at offsets -1..0, the space-to-depth form) and its magnitude"""
+    x64, dz64 = x.double(), dz.double()
+    if k == 2:
+        shape = (dz.shape[1], x.shape[1], 2, 2)
+        f = lambda a, d: torch.nn.grad.conv2d_weight(F.pad(a, (1, 0, 1, 0)), shape, d, stride=1, padding=0)
+    else:
+        shape = (dz.shape[1], x.shape[1], k, k)
+        f = lambda a, d: torch.nn.grad.conv2d_weight(a, shape, d, stride=stride, padding=(k - 1) // 2)
+    return f(x64, dz64), f(x64.abs(), dz64.abs())
+
+
+def worst_ratio(got, want, mag, n_add, extra=None):
+    """max over entries of |got - want| / bound; <= 1 everywhere means the kernel is within the float64 bound"""
+    bound = KAPPA * math.sqrt(n_add) * U * mag + TINY
+    if extra is not None:
+        bound = bound + extra
+    return float(((got.double() - want).abs() / bound).max())
+
+
+def unpacked(dw, k, cout_pad, cin_pad, cout, cin):
+    return dw.view(k, k, cout_pad, cin_pad)[:, :, :cout, :cin].permute(2, 3, 0, 1)
+
+
+def s2d_nchw(x):
+    """space-to-depth of an NCHW tensor: channel (py * 2 + px) * C + c holds pixel (2Y + py, 2X + px)"""
+    return torch.cat([x[:, :, py::2, px::2] for py in range(2) for px in range(2)], 1)
+
+
+class Case:
+    """one wgrad launch: operands in padded NHWC, their float64 reference and the mirrored launch plan"""
+
+    def __init__(self, batch, h, w, cout, ksize, cin=None, s2d_c=None, narrow=False, seed=0):
+        from rotate_yolov3_b200 import layout as L
+        dev = torch.device("cuda")
+        g = torch.Generator().manual_seed(seed)
+        self.b, self.k = batch, ksize
+        if s2d_c is not None:        # 3x3/stride-2 layer on a [b, C, 2h, 2w] input, in its space-to-depth form
+            self.x_full = _bf(torch.randn(batch, s2d_c, 2 * h, 2 * w, generator=g)).to(dev)
+            self.x = s2d_nchw(self.x_full)
+            cin = 4 * s2d_c
+        else:
+            self.x = _bf(torch.randn(batch, cin, h, w, generator=g)).to(dev)
+        self.h, self.w, self.cin, self.cout = h, w, cin, cout
+        self.dz = _bf(torch.randn(batch, cout, h, w, generator=g)).to(dev)
+        self.cin_pad = L.round_up(cin, 64)
+        self.cout_pad = L.round_up(cout, 64 if cout <= 64 else (128 if cout <= 128 else 256))
+        self.xcs = L.round_up(cin, 32) if narrow else self.cin_pad
+        self.zcs = L.round_up(cout, 32) if narrow else self.cout_pad
+        if s2d_c is not None:        # built by the library's own space-to-depth kernel, as the training step does
+            xf = L.to_padded_nhwc(self.x_full, L.round_up(s2d_c, 64))
+            self.xb = L.alloc_padded(batch, h, w, self.xcs, dev)
+            st = _lib().lib.ryolo_space_to_depth(_lib().ptr(xf), xf.shape[-1], batch, 2 * h, 2 * w, s2d_c,
+                                                 _lib().ptr(self.xb), self.xcs, _lib().stream_ptr(dev))
+            assert st == 0, _lib().last_error()
+        else:
+            self.xb = L.to_padded_nhwc(self.x, self.xcs)
+        self.dzb = L.to_padded_nhwc(self.dz, self.zcs)
+        self._ref = None
+
+    def plan(self, reserved=0):
+        return wgrad_plan(self.k, self.cin_pad, self.cout_pad, self.b, self.h, self.w, gemm_sms(reserved))
+
+    def ref(self):
+        if self._ref is None:
+            self._ref = ref_wgrad(self.x, self.dz, self.k)
+        return self._ref
+
+    def new_dw(self, fill=None):
+        shape = (self.k * self.k, self.cout_pad, self.cin_pad)
+        if fill is None:
+            return torch.zeros(shape, dtype=torch.float32, device="cuda")
+        return fill.clone()
+
+    def run(self, dw, stream=None):
+        wgrad(self.dzb, self.zcs, self.cout_pad, self.xb, self.xcs, self.cin_pad, self.b, self.h, self.w, self.k, dw, stream)
+        return dw
+
+    def got(self, dw):
+        return unpacked(dw, self.k, self.cout_pad, self.cin_pad, self.cout, self.cin)
+
+
+# (case kwargs, expected plan: bn, tg always; ksplit and a short last split on a 132-SM H100 SXM)
+CASES = {
+    "k3_c64_tg3": (dict(batch=4, h=76, w=76, cin=64, cout=64, ksize=3), dict(bn=64, tg=3, ksplit=24, short_last=True, last=13)),
+    "k3_c128_tg1": (dict(batch=2, h=76, w=76, cin=128, cout=64, ksize=3), dict(bn=128, tg=1, ksplit=12, short_last=True)),
+    "s2d_c32_tg2": (dict(batch=4, h=38, w=38, s2d_c=32, cout=64, ksize=2), dict(bn=128, tg=2, ksplit=7, short_last=True)),
+    "s2d_c16_tg2": (dict(batch=4, h=38, w=38, s2d_c=16, cout=64, ksize=2), dict(bn=64, tg=2, ksplit=7)),
+    "s2d_c64_bn256": (dict(batch=2, h=38, w=38, s2d_c=64, cout=128, ksize=2), dict(bn=256, tg=1, ksplit=4, short_last=True)),
+    "k1_c768_3n2m": (dict(batch=2, h=38, w=38, cin=768, cout=256, ksize=1), dict(bn=256, tg=1, ksplit=4, tiles=6)),
+    "k3_narrow32": (dict(batch=2, h=40, w=40, cin=32, cout=32, ksize=3, narrow=True), dict(bn=64, tg=3, ksplit=4)),
+}
+
+
+def check_plan(plan, want):
+    assert plan["bn"] == want["bn"] and plan["tg"] == want["tg"], (plan, want)
+    assert plan["ksplit"] > 1, plan                   # every case covers the split-K path on any card
+    if gemm_sms() == H100_SXM_SMS:
+        for key in ("ksplit", "short_last", "last", "tiles"):
+            if key in want:
+                assert plan[key] == want[key], (key, plan, want)
+
+
+@pytest.mark.parametrize("name", list(CASES))
+def test_wgrad_vs_float64(name):
+    kw, want_plan = CASES[name]
+    c = Case(**kw)
+    plan = c.plan()
+    check_plan(plan, want_plan)
+    dw = c.run(c.new_dw())
+    torch.cuda.synchronize()
+    want, mag = c.ref()
+    r = worst_ratio(c.got(dw), want, mag, plan["n_add"])
+    print("[wgrad] %s: bn %d tg %d ksplit %d (k-steps %d, %d per split, last %d) n_add %d worst |got-want|/bound %.4f"
+          % (name, plan["bn"], plan["tg"], plan["ksplit"], plan["ksteps"], plan["per_split"], plan["last"], plan["n_add"], r))
+    assert r <= 1.0, (name, r)
+    # padding filters / channels: nothing but zeros was added to them
+    full = dw.view(c.k * c.k, c.cout_pad, c.cin_pad)
+    assert float(full[:, c.cout:].abs().max() if c.cout_pad > c.cout else 0.0) == 0.0
+    assert float(full[:, :, c.cin:].abs().max() if c.cin_pad > c.cin else 0.0) == 0.0
+
+
+def test_bound_rejects_a_lost_k_step():
+    """The same bound, applied to a reference that misses ONE 64-pixel k-step (the last one of split 0), must fail on
+    the kernel's output: the bound is tight enough to see a dropped or doubled k-step."""
+    kw, _ = CASES["k3_c64_tg3"]
+    c = Case(**kw)
+    plan = c.plan()
+    dw = c.run(c.new_dw())
+    torch.cuda.synchronize()
+    want, mag = c.ref()
+    assert worst_ratio(c.got(dw), want, mag, plan["n_add"]) <= 1.0
+    j = plan["per_split"] - 1
+    hp, wp = c.h + 2, c.w + 2
+    flat = torch.zeros(c.b * hp * wp, dtype=torch.float64, device="cuda")
+    flat[64 * j:64 * (j + 1)] = 1.0
+    mask = flat.view(c.b, 1, hp, wp)[:, :, 1:-1, 1:-1]
+    assert float(mask.sum()) >= 32                    # the k-step lies on interior pixels
+    lost, _ = ref_wgrad(c.x, c.dz * mask, c.k)
+    r = worst_ratio(c.got(dw), want - lost, mag, plan["n_add"])
+    print("[wgrad] reference without k-step %d: worst ratio %.1f" % (j, r))
+    assert r > 1.0, r
+
+
+def test_wgrad_accumulates_into_dw():
+    """dw += gradient: a random prefill survives (padding entries bit-exactly), the interior is prefill + gradient"""
+    kw, _ = CASES["s2d_c32_tg2"]
+    kw = dict(kw, cout=48)                            # cout_pad 64 > cout: padding filters exist
+    c = Case(**kw)
+    plan = c.plan()
+    assert plan["ksplit"] > 1
+    pre = torch.randn(c.k * c.k, c.cout_pad, c.cin_pad, generator=torch.Generator().manual_seed(9)).cuda() * 50.0
+    dw = c.run(c.new_dw(pre))
+    torch.cuda.synchronize()
+    want, mag = c.ref()
+    pre_u = c.got(pre).double()
+    # the final fp32 add of the prefill rounds once more: half an ulp of |prefill + gradient|
+    r = worst_ratio(c.got(dw), pre_u + want, mag, plan["n_add"], extra=U * (pre_u + want).abs())
+    assert r <= 1.0, r
+    full, pfull = dw.view(c.k * c.k, c.cout_pad, c.cin_pad), pre.view(c.k * c.k, c.cout_pad, c.cin_pad)
+    assert torch.equal(full[:, c.cout:], pfull[:, c.cout:])
+    # s2d: cin = 4 * 32 = 128 = cin_pad, so the channel padding is covered by a 40 -> 64 channel case
+    c2 = Case(batch=2, h=40, w=40, cin=40, cout=40, ksize=3, narrow=True, seed=3)
+    assert c2.plan()["ksplit"] > 1
+    pre2 = torch.randn(9, c2.cout_pad, c2.cin_pad, generator=torch.Generator().manual_seed(10)).cuda()
+    dw2 = c2.run(c2.new_dw(pre2))
+    torch.cuda.synchronize()
+    want2, mag2 = c2.ref()
+    p2 = c2.got(pre2).double()
+    assert worst_ratio(c2.got(dw2), p2 + want2, mag2, c2.plan()["n_add"], extra=U * (p2 + want2).abs()) <= 1.0
+    assert torch.equal(dw2[:, c2.cout:], pre2[:, c2.cout:]) and torch.equal(dw2[:, :, c2.cin:], pre2[:, :, c2.cin:])
+
+
+def test_wgrad_split_counts_via_reserved_sms():
+    """ryolo_set_reserved_sms shrinks the GEMM grid and with it the split count: every split count stays within the
+    float64 bound, and repeated launches at one setting are bitwise equal.  The setting is process-global: restored."""
+    L = _lib()
+    c = Case(batch=8, h=76, w=76, cin=64, cout=64, ksize=3, seed=4)
+    want, mag = c.ref()
+    seen = {}
+    try:
+        for r in (0, 32, 60, 64):
+            assert L.lib.ryolo_set_reserved_sms(r) == 0
+            plan = c.plan(r)
+            assert plan["tg"] == 3 and plan["ksplit"] > 1
+            outs = [c.run(c.new_dw()) for _ in range(2)]
+            torch.cuda.synchronize()
+            assert torch.equal(outs[0], outs[1]), r
+            ratio = worst_ratio(c.got(outs[0]), want, mag, plan["n_add"])
+            print("[wgrad] reserved %d: %d SMs, ksplit %d, worst ratio %.4f" % (r, gemm_sms(r), plan["ksplit"], ratio))
+            assert ratio <= 1.0, (r, ratio)
+            seen[plan["ksplit"]] = outs[0]
+        assert L.lib.ryolo_set_reserved_sms(100) != 0     # outside the documented 0..64
+    finally:
+        L.lib.ryolo_set_reserved_sms(0)
+    if gemm_sms() == H100_SXM_SMS:
+        assert sorted(seen) == [22, 24, 32, 43], sorted(seen)
+    assert len(seen) >= 2
+
+
+def test_wgrad_scratch_growth_and_concurrent_streams():
+    """The split-K scratch is per stream and grows on demand.  small -> large (grows it) -> small on one stream without
+    synchronising in between; then the same launches on two streams at once.  All results correct, and the streams'
+    results bitwise equal.  High-priority streams: a pool the rest of the suite does not draw from, so the scratch of
+    the first stream starts at its initial 4 MB."""
+    small = Case(batch=2, h=40, w=40, cin=32, cout=32, ksize=3, narrow=True, seed=5)
+    large = Case(batch=4, h=76, w=76, cin=256, cout=128, ksize=3, seed=6)     # 9 taps x 14 splits, 128 KB per CTA
+    for cs in (small, large):
+        assert cs.plan()["ksplit"] > 1
+    sp, lp = small.plan(), large.plan()
+    per_cta = lambda p: (p["tg"] * p["bn"] // 2) * 256 * 4
+    assert sp["tiles"] * sp["ksplit"] * per_cta(sp) < (4 << 20) < lp["tiles"] * lp["ksplit"] * per_cta(lp)
+    cur = torch.cuda.current_stream()
+    s1, s2 = torch.cuda.Stream(priority=-1), torch.cuda.Stream(priority=-1)
+    seq = [small, large, small]
+    out1 = [cs.new_dw() for cs in seq]
+    s1.wait_stream(cur)
+    with torch.cuda.stream(s1):
+        for cs, dw in zip(seq, out1):
+            cs.run(dw, s1)
+    s1.synchronize()
+    s3 = torch.cuda.Stream(priority=-1)
+    out_a, out_b = [cs.new_dw() for cs in seq], [cs.new_dw() for cs in seq]
+    s2.wait_stream(cur)
+    s3.wait_stream(cur)
+    for cs, da, db in zip(seq, out_a, out_b):
+        cs.run(da, s2)
+        cs.run(db, s3)
+    torch.cuda.synchronize()
+    for cs, d1, da, db in zip(seq, out1, out_a, out_b):
+        want, mag = cs.ref()
+        assert worst_ratio(cs.got(d1), want, mag, cs.plan()["n_add"]) <= 1.0
+        assert torch.equal(d1, da) and torch.equal(da, db)
+
+
+@pytest.mark.parametrize("c_in,cout", [(32, 64), (16, 64), (64, 128)])
+def test_stride2_wgrad_space_to_depth_end_to_end(c_in, cout):
+    """space_to_depth(x) -> 2x2-tap wgrad at h/2 x w/2 -> unpack mode 2 == float64 gradient of the 3x3/stride-2/pad-1
+    conv; the multi-tensor unpack (one job table, as the training step builds it) writes the same bits"""
+    L = _lib()
+    from rotate_yolov3_b200 import _lib as lm
+    c = Case(batch=4 if c_in < 64 else 2, h=38, w=38, s2d_c=c_in, cout=cout, ksize=2, seed=c_in)
+    plan = c.plan()
+    assert plan["ksplit"] > 1
+    dw = c.run(c.new_dw())
+    grad = torch.full((cout, c_in, 3, 3), float("nan"), device="cuda")
+    st = L.lib.ryolo_conv_unpack_wgrad(L.ptr(dw), c.cout_pad, c.cin_pad, 2, cout, c_in, 3, L.ptr(grad), L.stream_ptr())
+    assert st == 0, L.last_error()
+    # the multi form with a second (plain 1x1) job in the same table
+    other = torch.randn(1, 64, 64, generator=torch.Generator().manual_seed(1)).cuda()
+    g_multi = torch.full_like(grad, float("nan"))
+    g_other = torch.full((40, 24, 1, 1), float("nan"), device="cuda")
+    jobs = [lm.UnpackJob(dw.data_ptr(), g_multi.data_ptr(), c.cout_pad, c.cin_pad, 2, cout, c_in, 3),
+            lm.UnpackJob(other.data_ptr(), g_other.data_ptr(), 64, 64, 0, 40, 24, 1)]
+    arr = (lm.UnpackJob * 2)(*jobs)
+    raw = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).cuda()
+    sizes = [cout * c_in * 9, 40 * 24]
+    prefix = torch.tensor([0, sizes[0], sizes[0] + sizes[1]], dtype=torch.int64).cuda()
+    st = L.lib.ryolo_conv_unpack_wgrad_multi(L.ptr(raw), 2, L.ptr(prefix), sum(sizes), L.stream_ptr())
+    assert st == 0, L.last_error()
+    torch.cuda.synchronize()
+    want, mag = ref_wgrad(c.x_full, c.dz, 3, stride=2)
+    r = worst_ratio(grad, want, mag, plan["n_add"])
+    print("[wgrad] s2d end to end C=%d cout=%d: ksplit %d worst ratio %.4f" % (c_in, cout, plan["ksplit"], r))
+    assert r <= 1.0, r
+    assert torch.equal(g_multi, grad)
+    assert torch.equal(g_other.view(40, 24), other[0, :40, :24])
+
+
+def test_stride2_wgrad_zero_insert_end_to_end():
+    """zero_insert2x(dz) -> 3x3 wgrad at input resolution == float64 gradient of the 3x3/stride-2/pad-1 conv"""
+    from rotate_yolov3_b200 import layout as Lo
+    L = _lib()
+    dev = torch.device("cuda")
+    g = torch.Generator().manual_seed(12)
+    b, cin, cout, h, w = 4, 64, 128, 76, 76
+    x = _bf(torch.randn(b, cin, h, w, generator=g)).to(dev)
+    dz = _bf(torch.randn(b, cout, h // 2, w // 2, generator=g)).to(dev)
+    cin_pad, cout_pad = 64, 128
+    xb = Lo.to_padded_nhwc(x, cin_pad)
+    dzb = Lo.to_padded_nhwc(dz, cout_pad)
+    up = Lo.alloc_padded(b, h, w, cout_pad, dev)
+    st = L.lib.ryolo_zero_insert2x(L.ptr(dzb), cout_pad, b, h // 2, w // 2, cout_pad, L.ptr(up), cout_pad, h, w, L.stream_ptr())
+    assert st == 0, L.last_error()
+    plan = wgrad_plan(3, cin_pad, cout_pad, b, h, w, gemm_sms())
+    assert plan["tg"] == 3 and plan["ksplit"] > 1
+    dw = torch.zeros(9, cout_pad, cin_pad, device=dev)
+    wgrad(up, cout_pad, cout_pad, xb, cin_pad, cin_pad, b, h, w, 3, dw)
+    torch.cuda.synchronize()
+    want, mag = ref_wgrad(x, dz, 3, stride=2)
+    r = worst_ratio(unpacked(dw, 3, cout_pad, cin_pad, cout, cin), want, mag, plan["n_add"])
+    print("[wgrad] zero-insert stride 2: ksplit %d worst ratio %.4f" % (plan["ksplit"], r))
+    assert r <= 1.0, r
+
+
+def test_wgrad_plan_mirror_is_self_consistent():
+    """the mirror's split arithmetic: every split non-empty, the splits cover the k-steps exactly"""
+    for ks, cin_pad, cout_pad, b, h, w in [(3, 64, 64, 4, 76, 76), (2, 256, 128, 2, 38, 38), (1, 768, 256, 2, 38, 38),
+                                           (3, 512, 1024, 1, 19, 19), (3, 64, 64, 1, 8, 8)]:
+        for sms in (132, 114, 72, 16):
+            p = wgrad_plan(ks, cin_pad, cout_pad, b, h, w, sms)
+            assert 1 <= p["last"] <= p["per_split"]
+            assert (p["ksplit"] - 1) * p["per_split"] + p["last"] == p["ksteps"]
+            # max_split = ceil(k-steps / 16) rounds up: a split gets at least 8 k-steps (13 in the 50-k-step cases)
+            assert p["ksplit"] == 1 or p["per_split"] >= 8

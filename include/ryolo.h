@@ -417,11 +417,16 @@ int ryolo_px_conv(const void* x_base, int x_cstride, int x_ch_off, int plane_str
                   const void* packed_w, int nterms, int a_plane_code, int batch, int in_h, int in_w,
                   int ksize, int cout, float* out, int out_cstride, int out_cols, int accumulate,
                   void* stream);
-/* wgrad of split operands = ryolo_conv_wgrad over all planes of dz and x ([taps][np*plane_out][np*plane_in]);
+/* wgrad of split operands = ryolo_px_wgrad over all planes of dz and x ([taps][np*plane_out][np*plane_in]);
  * this sums the nplanes^2 plane blocks into nn.Conv2d layout (mode 0 / 2 as ryolo_conv_unpack_wgrad); cin_off:
  * first channel of x's view inside its plane (a conv reading a slice of a concat buffer). */
 int ryolo_px_unpack_wgrad(const float* dw, int plane_out, int plane_in, int nplanes, int mode, int cout,
                           int cin, int ksize, int cin_off, float* grad, void* stream);
+/* ryolo_conv_wgrad with the accumulation of ryolo_px_conv: the wgmma accumulator is restarted every 8
+ * k-steps and folded into round-to-nearest fp32 register sums, so the dW of a long pixel range carries no
+ * truncation bias.  Same arguments and dW layout; the parity path runs it over all planes of dz and x. */
+int ryolo_px_wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x, int x_cstride,
+                   int cin_pad, int batch, int in_h, int in_w, int ksize, float* dw, void* stream);
 /* batch statistics of fp32 z: sums[0..c) = sum, [c..2c) = sum of squares (fp64, zeroed inside) */
 int ryolo_px_bn_stats(const float* z, int z_cstride, int batch, int h, int w, int c, double* sums,
                       void* stream);

@@ -103,6 +103,7 @@ SIGNATURES = {
     "ryolo_px_pack_weights": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_px_conv": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "ryolo_px_unpack_wgrad": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "ryolo_px_wgrad": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_px_bn_stats": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_px_bn_finalize": (_i, [_vp, _i, _d, _f, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_px_bn_act_fwd": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _vp]),

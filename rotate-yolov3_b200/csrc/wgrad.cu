@@ -9,6 +9,11 @@
 // to scratch and the LAST split of a tile to finish (ticket per tile) adds the splits in split order and adds the sum to
 // dW -- a fixed order, so the weight gradient is the same every run (float atomics would add in arrival order).
 // Stride-2 layers pass the zero-inserted dz at input resolution.
+//
+// SEG variant (ryolo_px_wgrad, the parity-precision path): the tensor pipe's fp32 accumulator does not round to nearest,
+// and over the thousands of updates of one pixel range its error is biased towards zero.  As in conv_parity.cu, the MMA
+// warp groups then restart the accumulator every WG_SEG k-steps (32 MMA updates) and fold it into a second register set
+// with round-to-nearest fp32 adds; the split-K reduction and the store are unchanged.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -19,6 +24,7 @@ namespace ryolo {
 constexpr int WG_BM = 128;   // filters per tile (two m64 warp groups)
 constexpr int WG_BK = 64;    // pixels per k-step
 constexpr int WG_THREADS = 384;   // warp group 0: TMA; warp groups 1-2: MMA + reduction
+constexpr int WG_SEG = 8;         // SEG variant: k-steps per accumulator segment
 
 struct WgradParams {
   int np, wp, taps;   // taps: 1, 4 (2x2, offsets -1..0) or 9 (3x3, offsets -1..1)
@@ -42,13 +48,13 @@ struct WgradCfg {
   static constexpr int kSmem = kStages * kStageBytes + 2 * kStages * 8 + 1024;
 };
 
-template <int BN, int TG>
+template <int BN, int TG, bool SEG>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_constant__ CUtensorMap map_x, const WgradParams p) {
   using C = WgradCfg<BN, TG>;
   constexpr int kABytes = C::kABytes, kBBytes = C::kBBytes, kStageBytes = C::kStageBytes, WG_STAGES = C::kStages;
   constexpr int NS = BN / 64;
-  static_assert(TG * BN <= 256, "accumulators must fit the registers");
+  static_assert(TG * BN <= (SEG ? 128 : 256), "accumulators (and the SEG sums) must fit the registers");
   extern __shared__ unsigned char smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + WG_STAGES * kStageBytes;
@@ -116,11 +122,21 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
   const int half = wg - 1;
   const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
   float acc[TG][NS][32];
+  float sum[SEG ? TG : 1][SEG ? NS : 1][32];   // SEG: round-to-nearest running sum of the closed segments
+  if constexpr (SEG) {
+#pragma unroll
+    for (int j = 0; j < TG; j++)
+#pragma unroll
+      for (int n = 0; n < NS; n++)
+#pragma unroll
+        for (int v = 0; v < 32; v++) sum[j][n][v] = 0.f;
+  }
   int stage = 0, prev = -1;
   uint32_t phase = 0;
   for (int kk = 0; kk < k_iters; kk++) {
     mbar_wait(full_bar(stage), phase);
     const uint32_t sa = smem_base + stage * kStageBytes;
+    const bool seg_start = SEG ? kk % WG_SEG == 0 : kk == 0;
     wg_fence();
 #pragma unroll
     for (int k = 0; k < WG_BK / 16; k++) {
@@ -131,19 +147,46 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
 #pragma unroll
         for (int n = 0; n < NS; n++)
           wgmma_n64<1, 1>(acc[j][n], adesc, make_smem_desc_mn(sa + kABytes + j * kBBytes + n * 8192 + k * 2048, 8192),
-                          (kk | k) != 0);
+                          (!seg_start || k > 0) ? 1u : 0u);
     }
     wg_commit();
-    wg_wait<1>();
-    if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
-    prev = stage;
+    bool seg_end = false;
+    if constexpr (SEG) {
+      seg_end = kk % WG_SEG == WG_SEG - 1 || kk == k_iters - 1;
+      if (seg_end) {
+        // close the segment: fold it into the round-to-nearest running sum
+        wg_wait<0>();
+#pragma unroll
+        for (int j = 0; j < TG; j++)
+#pragma unroll
+          for (int n = 0; n < NS; n++) {
+            wg_fence_regs(acc[j][n]);
+#pragma unroll
+            for (int v = 0; v < 32; v++) sum[j][n][v] = __fadd_rn(sum[j][n][v], acc[j][n][v]);
+          }
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        if (lane == 0) mbar_arrive(empty_bar(stage));
+        prev = -1;
+      }
+    }
+    if (!seg_end) {
+      wg_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+      prev = stage;
+    }
     if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
   }
   wg_wait<0>();
 #pragma unroll
   for (int j = 0; j < TG; j++)
 #pragma unroll
-    for (int n = 0; n < NS; n++) wg_fence_regs(acc[j][n]);
+    for (int n = 0; n < NS; n++) {
+      wg_fence_regs(acc[j][n]);
+      if constexpr (SEG) {
+#pragma unroll
+        for (int v = 0; v < 32; v++) acc[j][n][v] = sum[j][n][v];
+      }
+    }
 
   if (p.ksplit > 1) {
     // split-K in a fixed order: store my fragment, take a ticket; the last split of the tile adds splits 0, 1, ...
@@ -208,23 +251,18 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
   }
 }
 
-template <int BN, int TG>
+template <int BN, int TG, bool SEG>
 static int launch_wgrad(const CUtensorMap& mdz, const CUtensorMap& mx, const WgradParams& p, cudaStream_t stream) {
   using C = WgradCfg<BN, TG>;
-  RYOLO_SMEM_OPT_IN((conv_wgrad_kernel<BN, TG>), C::kSmem);
+  RYOLO_SMEM_OPT_IN((conv_wgrad_kernel<BN, TG, SEG>), C::kSmem);
   const int grid = p.tap_groups * p.m_tiles * p.n_tiles * p.ksplit;
-  conv_wgrad_kernel<BN, TG><<<grid, WG_THREADS, C::kSmem, stream>>>(mdz, mx, p);
+  conv_wgrad_kernel<BN, TG, SEG><<<grid, WG_THREADS, C::kSmem, stream>>>(mdz, mx, p);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }
 
-}  // namespace ryolo
-
-using namespace ryolo;
-
-extern "C" int ryolo_conv_wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x, int x_cstride, int cin_pad,
-                                int batch, int in_h, int in_w, int ksize, float* dw, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+static int wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x, int x_cstride, int cin_pad, int batch,
+                 int in_h, int in_w, int ksize, float* dw, bool seg, cudaStream_t stream) {
   RYOLO_ARG_CHECK(dz && x && dw && batch > 0 && in_h > 0 && in_w > 0);
   RYOLO_ARG_CHECK(ksize == 1 || ksize == 3 || ksize == 2);
   RYOLO_ARG_CHECK(cout_pad > 0 && cout_pad % 64 == 0 && cin_pad > 0 && cin_pad % 64 == 0);
@@ -238,7 +276,8 @@ extern "C" int ryolo_conv_wgrad(const void* dz, int dz_cstride, int cout_pad, co
   p.taps = ksize * ksize;
   p.cout_pad = cout_pad;
   p.cin_pad = cin_pad;
-  const int bn = cin_pad >= 192 ? 256 : cin_pad;   // 64, 128 or 256
+  // 64, 128 or 256 channels per tile; SEG keeps a second register set, so TG * bn <= 128 there
+  const int bn = seg ? (cin_pad % 128 == 0 ? 128 : 64) : (cin_pad >= 192 ? 256 : cin_pad);
   p.m_tiles = (cout_pad + WG_BM - 1) / WG_BM;
   p.n_tiles = (cin_pad + bn - 1) / bn;
   p.ksteps_total = (p.np + WG_BK - 1) / WG_BK;
@@ -252,7 +291,7 @@ extern "C" int ryolo_conv_wgrad(const void* dz, int dz_cstride, int cout_pad, co
   }
   int tg = 1;
   if (bn <= 128 && force_tg != 1) tg = p.taps == 9 ? 3 : (p.taps == 4 ? 2 : 1);
-  if (tg * bn > 256) tg = 1;
+  if (tg * bn > (seg ? 128 : 256)) tg = 1;
   p.tap_groups = p.taps / tg;
   const int tiles = p.tap_groups * p.m_tiles * p.n_tiles;
   // split-K: every (tile, split) CTA ends with tile-size fp32 reductions into dW and cannot overlap them with its
@@ -299,12 +338,33 @@ extern "C" int ryolo_conv_wgrad(const void* dz, int dz_cstride, int cout_pad, co
   if (st != RYOLO_OK) return st;
   st = encode_map_2d(&mx, x, (uint64_t)x_cstride, (uint64_t)p.np, (uint64_t)x_cstride * 2, 64, WG_BK);
   if (st != RYOLO_OK) return st;
-  if (bn == 256) return launch_wgrad<256, 1>(mdz, mx, p, stream);
-  if (bn == 128) {
-    if (tg == 2) return launch_wgrad<128, 2>(mdz, mx, p, stream);
-    return launch_wgrad<128, 1>(mdz, mx, p, stream);
+  if (seg) {
+    if (bn == 128) return launch_wgrad<128, 1, true>(mdz, mx, p, stream);
+    if (tg == 2) return launch_wgrad<64, 2, true>(mdz, mx, p, stream);
+    return launch_wgrad<64, 1, true>(mdz, mx, p, stream);
   }
-  if (tg == 3) return launch_wgrad<64, 3>(mdz, mx, p, stream);
-  if (tg == 2) return launch_wgrad<64, 2>(mdz, mx, p, stream);
-  return launch_wgrad<64, 1>(mdz, mx, p, stream);
+  if (bn == 256) return launch_wgrad<256, 1, false>(mdz, mx, p, stream);
+  if (bn == 128) {
+    if (tg == 2) return launch_wgrad<128, 2, false>(mdz, mx, p, stream);
+    return launch_wgrad<128, 1, false>(mdz, mx, p, stream);
+  }
+  if (tg == 3) return launch_wgrad<64, 3, false>(mdz, mx, p, stream);
+  if (tg == 2) return launch_wgrad<64, 2, false>(mdz, mx, p, stream);
+  return launch_wgrad<64, 1, false>(mdz, mx, p, stream);
+}
+
+}  // namespace ryolo
+
+using namespace ryolo;
+
+extern "C" int ryolo_conv_wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x, int x_cstride, int cin_pad,
+                                int batch, int in_h, int in_w, int ksize, float* dw, void* stream_) {
+  return wgrad(dz, dz_cstride, cout_pad, x, x_cstride, cin_pad, batch, in_h, in_w, ksize, dw, false,
+               static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ryolo_px_wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x, int x_cstride, int cin_pad,
+                              int batch, int in_h, int in_w, int ksize, float* dw, void* stream_) {
+  return wgrad(dz, dz_cstride, cout_pad, x, x_cstride, cin_pad, batch, in_h, in_w, ksize, dw, true,
+               static_cast<cudaStream_t>(stream_));
 }

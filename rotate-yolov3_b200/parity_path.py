@@ -9,8 +9,8 @@ number bench.py prints says which precision produced it.
 
 Per conv block, forward:  [space-to-depth of both planes] -> px_conv -> z (fp32) -> batch or running statistics ->
 y = prelu(z*scale + shift) [+ shortcut] [2x2 replicated], re-split.  Backward: px_bn_act_bwd (fp32 dy, z -> d gamma,
-d beta, d slope, split dz, shortcut gradient) -> wgrad (the bf16 wgmma wgrad GEMM over all planes of dz and x: nine
-plane blocks, summed by px_unpack_wgrad) -> dgrad (px_conv with mirrored / transposed split weights, fp32 accumulate
+d beta, d slope, split dz, shortcut gradient) -> wgrad (px_wgrad: the wgmma wgrad GEMM with segment sums, over all
+planes of dz and x: nine plane blocks, summed by px_unpack_wgrad) -> dgrad (px_conv with mirrored / transposed split weights, fp32 accumulate
 into the source's gradient buffer)."""
 import ctypes
 
@@ -330,10 +330,10 @@ class ParityPlan:
                 pg[(b.i, "BatchNorm2d.weight")] = f[b.cout:2 * b.cout]
                 if b.has_act:
                     pg[(b.i, "activation.weight")] = f[2 * b.cout:]
-            # ---- weight gradient: bf16 wgrad GEMM over both planes of dz and of the source buffer ----
+            # ---- weight gradient: segmented wgrad GEMM over all planes of dz and of the source buffer ----
             b.dw.zero_()
             xcs = b.xw_buf.shape[-1]
-            _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(b.dz), NP * b.po, NP * b.po, _lib.ptr(b.xw_buf), xcs, xcs, B, b.gh, b.gw_,
+            _lib.check(lib.ryolo_px_wgrad(_lib.ptr(b.dz), NP * b.po, NP * b.po, _lib.ptr(b.xw_buf), xcs, xcs, B, b.gh, b.gw_,
                                             b.k_eff, _lib.ptr(b.dw), st), "wgrad")
             w = seq.Conv2d.weight
             gw = torch.empty(tuple(w.shape), dtype=torch.float32, device=self.device)

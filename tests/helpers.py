@@ -160,3 +160,41 @@ def mini_cfg(width=64, height=48):
     s += "[route]\nlayers = -3\n\n" + conv(32, 1) + "[upsample]\nstride=2\n\n[route]\nlayers = -1, 4\n\n"
     s += conv(64, 3) + conv(21, 1, bn=0, act="linear") + yolo(0, 2)
     return s
+
+
+def wgrad_plan(ksize, cin_pad, cout_pad, batch, h, w, sms, segmented=False):
+    """Python mirror of the launch heuristic of ryolo_conv_wgrad and (segmented=True) ryolo_px_wgrad (csrc/wgrad.cu):
+    tile width bn, taps per CTA tg, split count; `updates` = wgmma k16 accumulations per split, the length of one
+    accumulator chain of ryolo_conv_wgrad (ryolo_px_wgrad restarts it every 32)"""
+    np_ = batch * (h + 2) * (w + 2)
+    taps = ksize * ksize
+    regs = 128 if segmented else 256
+    if segmented:
+        bn = 128 if cin_pad % 128 == 0 else 64
+    else:
+        bn = 256 if cin_pad >= 192 else cin_pad
+    m_tiles = -(-cout_pad // 128)
+    n_tiles = -(-cin_pad // bn)
+    ksteps = -(-np_ // 64)
+    tg = 1
+    if bn <= 128:
+        tg = 3 if taps == 9 else (2 if taps == 4 else 1)
+    if tg * bn > regs:
+        tg = 1
+    tiles = (taps // tg) * m_tiles * n_tiles
+    ksplit, best = 1, 0.0
+    for waves in range(1, 5):
+        ks = max(1, waves * sms // tiles)
+        ctas = tiles * ks
+        eff = ctas / (-(-ctas // sms) * sms)
+        if eff > best + 1e-9:
+            best, ksplit = eff, ks
+        if eff >= 0.9:
+            break
+    max_split = -(-ksteps // 16)
+    ksplit = max(1, min(ksplit, max_split))
+    per_split = -(-ksteps // ksplit)
+    ksplit = -(-ksteps // per_split)
+    last = ksteps - (ksplit - 1) * per_split
+    return dict(bn=bn, tg=tg, tiles=tiles, ksteps=ksteps, ksplit=ksplit, per_split=per_split, last=last,
+                short_last=last < per_split, n_add=-(-ksteps * 64 // 16) + ksplit, updates=4 * per_split)

@@ -22,44 +22,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from helpers import wgrad_plan
+
 pytestmark = pytest.mark.gpu
 
 KAPPA = 1.0
 U = 2.0 ** -24
 TINY = 1e-30
 H100_SXM_SMS = 132
-
-
-def wgrad_plan(ksize, cin_pad, cout_pad, batch, h, w, sms):
-    """Python mirror of the launch heuristic in ryolo_conv_wgrad (csrc/wgrad.cu)"""
-    np_ = batch * (h + 2) * (w + 2)
-    taps = ksize * ksize
-    bn = 256 if cin_pad >= 192 else cin_pad
-    m_tiles = -(-cout_pad // 128)
-    n_tiles = -(-cin_pad // bn)
-    ksteps = -(-np_ // 64)
-    tg = 1
-    if bn <= 128:
-        tg = 3 if taps == 9 else (2 if taps == 4 else 1)
-    if tg * bn > 256:
-        tg = 1
-    tiles = (taps // tg) * m_tiles * n_tiles
-    ksplit, best = 1, 0.0
-    for waves in range(1, 5):
-        ks = max(1, waves * sms // tiles)
-        ctas = tiles * ks
-        eff = ctas / (-(-ctas // sms) * sms)
-        if eff > best + 1e-9:
-            best, ksplit = eff, ks
-        if eff >= 0.9:
-            break
-    max_split = -(-ksteps // 16)
-    ksplit = max(1, min(ksplit, max_split))
-    per_split = -(-ksteps // ksplit)
-    ksplit = -(-ksteps // per_split)
-    last = ksteps - (ksplit - 1) * per_split
-    return dict(bn=bn, tg=tg, tiles=tiles, ksteps=ksteps, ksplit=ksplit, per_split=per_split, last=last,
-                short_last=last < per_split, n_add=-(-ksteps * 64 // 16) + ksplit)
 
 
 def gemm_sms(reserved=0):

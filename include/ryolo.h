@@ -88,11 +88,11 @@ int ryolo_rnms_batched(const float* dets, int segments, int cap, const int32_t* 
                        void* stream);
 
 /* Batched candidate selection in front of it (reference: utils/nms/nms.py:34-40 per image; detect.py:204-213).
- * io [batch, p, 6+nc] fp32 decoded predictions (NOT modified).  Per image: rows passing the reference's filter
- * (conf = obj * max class conf > conf_thres, w and h > min_wh, all values finite) whose conf lies in or above the
- * histogram bin (4096 linear bins on [0,1]) of the limit-th largest conf are written IN INPUT ORDER to
- * dets_out [batch, cap, 6] = (x, y, w, h, theta, conf); n_out [batch] int32 = their number (<= cap; cap >= limit,
- * the surplus over limit is at most one bin's population and is cut by ryolo_rnms_batched's `limit`). */
+ * io [batch, p, 6+nc] fp32 decoded predictions (NOT modified).  Per image: of the rows passing the reference's filter
+ * (conf = obj * max class conf > conf_thres, w and h > min_wh, all values finite), exactly the `limit` with the largest
+ * conf -- ties resolved by lowest row index -- are written IN INPUT ORDER to dets_out [batch, cap, 6] =
+ * (x, y, w, h, theta, conf); n_out [batch] int32 = min(limit, rows passing).  cap >= limit is the row stride of
+ * dets_out.  conf_thres must be >= 0 (RYOLO_E_ARG otherwise, NaN included). */
 size_t ryolo_detect_select_workspace_bytes(int batch, int p);
 int ryolo_detect_select(const float* io, int batch, int p, int nc, float conf_thres, float min_wh, int limit,
                         float* dets_out, int cap, int32_t* n_out, void* workspace, size_t workspace_bytes,

@@ -5,13 +5,17 @@
 //
 // The reference has no cap (trained weights leave a few hundred candidates); a random-init network puts ~half of the
 // 545 832 proposals above any threshold, and RNMS is quadratic, so detect caps the candidates per image (SURVEY.md 8d
-// config 5).  torch.topk + gather cost 8 ms per 32 images in round 1; here:
-//   1. histogram of conf over 4096 linear bins per image (shared-memory atomics, one flush per CTA);
-//   2. per image: the bin that holds the limit-th largest conf -> selection threshold t (its lower edge; everything >= t
-//      is at most `limit` + one bin's population);
-//   3. ordered two-pass compaction (block counts -> scan -> write) of the rows with conf >= t: deterministic, input order.
-// The batched RNMS sorts the candidates by score (stable) and keeps the first `limit`: exactly the top-`limit` set
-// with ties resolved by row index.
+// config 5).  The selection is exact: the top-`limit` rows by conf, ties resolved by lowest row index, for every
+// distribution of conf (no histogram-bin surplus, whatever the number of rows sharing a value).
+//   1. conf_thres >= 0, so every passing conf is a positive finite float and its fp32 bit pattern orders like the value.
+//      One pass over io stores key = bits(conf) per row (0 = filtered out) and histograms bits 30..19 of the keys.
+//   2. Radix select in three digits (bits 30..19, 18..7, 6..0), one 4096-bin histogram pass over the keys per digit,
+//      each restricted to the keys that share the digits found so far -> v = the limit-th largest key, `above` = the
+//      number of keys > v (< limit) and need = limit - above.  At most `limit` passing rows: v = 0, need = 0.
+//   3. Ordered two-pass compaction (block counts -> scan -> write) of the rows with key > v and of the first `need`
+//      rows with key == v: two block counts per 256 rows (above / tied), both scanned, so the output position of a row
+//      is above_before + min(tied_before, need).  Deterministic, input order, exactly min(limit, #passing) rows.
+// The batched RNMS then sorts the candidates by score (stable): the same order as a stable top-`limit` sort.
 #include "common.cuh"
 #include "filter.cuh"
 
@@ -20,21 +24,41 @@ namespace ryolo {
 constexpr int SEL_BINS = 4096;
 constexpr int SEL_T = 256;
 constexpr int SEL_ROWS_PER_CTA = 8192;
+constexpr int SEL_PASSES = 3;
+__constant__ int c_sel_shift[SEL_PASSES] = {19, 7, 0};   // digit of pass d: bits [shift, shift + bits) of the key
+__constant__ int c_sel_bits[SEL_PASSES] = {12, 12, 7};
 
-__device__ __forceinline__ bool sel_row(const float* __restrict__ row, int nc, float conf_thres, float min_wh, float* conf_out) {
+struct SelState {
+  unsigned prefix;   // the key digits found so far; after the last pass: v, the limit-th largest key
+  int k;             // rank (1-based, from the top) of the wanted key among the keys that share `prefix`; after the
+                     // last pass: need, the number of rows with key == v to take
+  int done;          // at most `limit` rows pass: all of them are selected (v = 0, need = 0)
+};
+
+__device__ __forceinline__ unsigned sel_key(const float* __restrict__ row, int nc, float conf_thres, float min_wh) {
   float best; int bi; bool fin;
   class_max(row, nc, &best, &bi, &fin);
   const float conf = row[5] * best;
-  *conf_out = conf;
-  return keep_row(row, conf, fin, conf_thres, min_wh);
-}
-__device__ __forceinline__ int sel_bin(float conf) {
-  int b = (int)(conf * (float)SEL_BINS);
-  return b < 0 ? 0 : (b >= SEL_BINS ? SEL_BINS - 1 : b);
+  return keep_row(row, conf, fin, conf_thres, min_wh) ? __float_as_uint(conf) : 0u;
 }
 
-__global__ void __launch_bounds__(SEL_T) sel_hist_kernel(const float* __restrict__ io, int p, int nc, float conf_thres,
-                                                         float min_wh, int* __restrict__ hist /*[B][SEL_BINS]*/) {
+// warp-aggregated shared-memory histogram update (many rows share one bin: dense or quantised confidences)
+__device__ __forceinline__ void sel_hist_add(int* s_h, bool valid, int bin) {
+  const unsigned same = __match_any_sync(0xffffffffu, valid ? bin : -1);
+  if (valid && (threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&s_h[bin], __popc(same));
+}
+
+__device__ __forceinline__ void sel_hist_flush(const int* s_h, int* __restrict__ hist) {
+  __syncthreads();
+  for (int i = threadIdx.x; i < SEL_BINS; i += SEL_T)
+    if (s_h[i]) atomicAdd(&hist[i], s_h[i]);
+}
+
+// pass 0: keys of all rows + histogram of their top digit
+__global__ void __launch_bounds__(SEL_T) sel_key_hist_kernel(const float* __restrict__ io, int p, int nc,
+                                                             float conf_thres, float min_wh,
+                                                             unsigned* __restrict__ keys /*[B][p]*/,
+                                                             int* __restrict__ hist /*[B][SEL_BINS]*/) {
   __shared__ int s_h[SEL_BINS];
   for (int i = threadIdx.x; i < SEL_BINS; i += SEL_T) s_h[i] = 0;
   __syncthreads();
@@ -42,28 +66,56 @@ __global__ void __launch_bounds__(SEL_T) sel_hist_kernel(const float* __restrict
   const int r0 = blockIdx.x * SEL_ROWS_PER_CTA;
   const int r1 = min(p, r0 + SEL_ROWS_PER_CTA);
   const float* base = io + (size_t)b * p * (6 + nc);
-  for (int r = r0 + threadIdx.x; r < r1; r += SEL_T) {
-    float conf;
-    if (sel_row(base + (size_t)r * (6 + nc), nc, conf_thres, min_wh, &conf)) atomicAdd(&s_h[sel_bin(conf)], 1);
+  for (int r = r0 + (int)threadIdx.x; r - (int)threadIdx.x < r1; r += SEL_T) {   // warp-uniform trip count
+    unsigned key = 0;
+    if (r < r1) {
+      key = sel_key(base + (size_t)r * (6 + nc), nc, conf_thres, min_wh);
+      keys[(size_t)b * p + r] = key;
+    }
+    sel_hist_add(s_h, key != 0, (int)(key >> 19));
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < SEL_BINS; i += SEL_T)
-    if (s_h[i]) atomicAdd(&hist[b * SEL_BINS + i], s_h[i]);
+  sel_hist_flush(s_h, hist + (size_t)b * SEL_BINS);
 }
 
-// one CTA per image: suffix sums over the bins from the top; t_bin = the highest bin whose suffix count reaches limit
-// (0 if fewer than `limit` rows pass the filter at all)
-__global__ void __launch_bounds__(1024) sel_thresh_kernel(const int* __restrict__ hist, int limit, int* __restrict__ t_bin) {
+// passes 1, 2: histogram of the next digit over the keys that share the digits found so far
+__global__ void __launch_bounds__(SEL_T) sel_digit_hist_kernel(const unsigned* __restrict__ keys, int p, int pass,
+                                                               const SelState* __restrict__ st,
+                                                               int* __restrict__ hist) {
+  __shared__ int s_h[SEL_BINS];
+  const int b = blockIdx.y;
+  if (st[b].done) return;
+  const unsigned prefix = st[b].prefix;
+  const int shift = c_sel_shift[pass], top = shift + c_sel_bits[pass];
+  const unsigned dmask = (1u << c_sel_bits[pass]) - 1u;
+  for (int i = threadIdx.x; i < SEL_BINS; i += SEL_T) s_h[i] = 0;
+  __syncthreads();
+  const int r0 = blockIdx.x * SEL_ROWS_PER_CTA;
+  const int r1 = min(p, r0 + SEL_ROWS_PER_CTA);
+  const unsigned* kb = keys + (size_t)b * p;
+  for (int r = r0 + (int)threadIdx.x; r - (int)threadIdx.x < r1; r += SEL_T) {
+    const unsigned key = r < r1 ? kb[r] : 0u;
+    sel_hist_add(s_h, key != 0 && (key >> top) == prefix, (int)((key >> shift) & dmask));
+  }
+  sel_hist_flush(s_h, hist + (size_t)b * SEL_BINS);
+}
+
+// one CTA per image: suffix sums over the bins from the top; the bin whose suffix count first reaches k holds the wanted
+// key -> append its digit to the prefix; its rank within that bin = k - (keys in the bins above it)
+__global__ void __launch_bounds__(1024) sel_radix_kernel(const int* __restrict__ hist, int pass, int limit,
+                                                         SelState* __restrict__ st) {
   __shared__ int s_part[1024];
   const int b = blockIdx.x, tid = threadIdx.x;
+  if (pass > 0 && st[b].done) return;
+  const unsigned prefix = pass ? st[b].prefix : 0u;
+  const int k = pass ? st[b].k : limit;
   constexpr int PER = SEL_BINS / 1024;
-  const int* h = hist + b * SEL_BINS;
+  const int* h = hist + (size_t)b * SEL_BINS;
   int loc[PER];
   int sum = 0;
 #pragma unroll
-  for (int k = 0; k < PER; k++) {      // thread tid owns bins [tid*PER, tid*PER + PER)
-    loc[k] = h[tid * PER + k];
-    sum += loc[k];
+  for (int j = 0; j < PER; j++) {      // thread tid owns bins [tid*PER, tid*PER + PER)
+    loc[j] = h[tid * PER + j];
+    sum += loc[j];
   }
   s_part[tid] = sum;
   __syncthreads();
@@ -74,42 +126,39 @@ __global__ void __launch_bounds__(1024) sel_thresh_kernel(const int* __restrict_
     s_part[tid] += v;
     __syncthreads();
   }
-  int above = tid + 1 < 1024 ? s_part[tid + 1] : 0;   // rows in bins above this thread's range
-  if (tid == 0) t_bin[b] = 0;
-  __syncthreads();
+  if (pass == 0 && s_part[0] <= limit) {   // at most `limit` rows pass the filter: take them all
+    if (tid == 0) st[b] = SelState{0u, 0, 1};
+    return;
+  }
+  int above = tid + 1 < 1024 ? s_part[tid + 1] : 0;   // keys in bins above this thread's range
 #pragma unroll
-  for (int k = PER - 1; k >= 0; k--) {
-    const int incl = above + loc[k];
-    if (above < limit && incl >= limit) t_bin[b] = tid * PER + k;   // exactly one (thread, k) satisfies this
+  for (int j = PER - 1; j >= 0; j--) {
+    const int incl = above + loc[j];
+    if (above < k && incl >= k)                        // exactly one (thread, j) satisfies this
+      st[b] = SelState{(prefix << c_sel_bits[pass]) | (unsigned)(tid * PER + j), k - above, 0};
     above = incl;
   }
 }
 
-__device__ __forceinline__ bool sel_take(const float* __restrict__ row, int nc, float conf_thres, float min_wh, int tb,
-                                         float* conf_out) {
-  float conf;
-  const bool ok = sel_row(row, nc, conf_thres, min_wh, &conf);
-  *conf_out = conf;
-  return ok && sel_bin(conf) >= tb;
-}
-
-__global__ void __launch_bounds__(SEL_T) sel_count_kernel(const float* __restrict__ io, int p, int nc, float conf_thres,
-                                                          float min_wh, const int* __restrict__ t_bin,
+// per 256-row block: number of keys > v and number of keys == v, at [b][0][blk] and [b][1][blk]
+__global__ void __launch_bounds__(SEL_T) sel_count_kernel(const unsigned* __restrict__ keys, int p,
+                                                          const SelState* __restrict__ st,
                                                           int* __restrict__ block_counts, int nblocks) {
   const int b = blockIdx.y;
   const int i = blockIdx.x * SEL_T + threadIdx.x;
-  bool keep = false;
-  if (i < p) {
-    float conf;
-    keep = sel_take(io + ((size_t)b * p + i) * (6 + nc), nc, conf_thres, min_wh, t_bin[b], &conf);
+  const unsigned v = st[b].prefix;
+  const unsigned key = i < p ? keys[(size_t)b * p + i] : 0u;
+  const int n_above = __syncthreads_count(i < p && key > v);
+  const int n_tied = __syncthreads_count(i < p && key == v);
+  if (threadIdx.x == 0) {
+    block_counts[((size_t)b * 2 + 0) * nblocks + blockIdx.x] = n_above;
+    block_counts[((size_t)b * 2 + 1) * nblocks + blockIdx.x] = n_tied;
   }
-  const int cnt = __syncthreads_count(keep);
-  if (threadIdx.x == 0) block_counts[b * nblocks + blockIdx.x] = cnt;
 }
 
-// exclusive scan of one image's block counts (one CTA per image), total (clipped to cap) -> n_out
-__global__ void __launch_bounds__(1024) sel_scan_kernel(int* __restrict__ block_counts, int nblocks, int cap,
-                                                        int* __restrict__ n_out) {
+// exclusive scan of one row of block counts (one CTA per row), its total -> totals[row]
+__global__ void __launch_bounds__(1024) sel_scan_kernel(int* __restrict__ block_counts, int nblocks,
+                                                        int* __restrict__ totals) {
   __shared__ int s_warp[32];
   __shared__ int s_carry;
   int* bc = block_counts + (size_t)blockIdx.x * nblocks;
@@ -144,33 +193,43 @@ __global__ void __launch_bounds__(1024) sel_scan_kernel(int* __restrict__ block_
     if (tid == 1023) s_carry = incl;
     __syncthreads();
   }
-  if (tid == 0) n_out[blockIdx.x] = s_carry < cap ? s_carry : cap;
+  if (tid == 0) totals[blockIdx.x] = s_carry;
 }
 
-__global__ void __launch_bounds__(SEL_T) sel_write_kernel(const float* __restrict__ io, int p, int nc, float conf_thres,
-                                                          float min_wh, const int* __restrict__ t_bin,
-                                                          const int* __restrict__ block_offsets, int nblocks,
-                                                          float* __restrict__ dets, int cap) {
-  __shared__ int s_warp[SEL_T / 32];
-  const int b = blockIdx.y;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int i = blockIdx.x * SEL_T + tid;
-  bool keep = false;
-  float conf = 0.f;
-  const float* row = io + ((size_t)b * p + i) * (6 + nc);
-  if (i < p) keep = sel_take(row, nc, conf_thres, min_wh, t_bin[b], &conf);
-  const unsigned bal = __ballot_sync(0xffffffffu, keep);
+// rows of this block before this thread's row that satisfy pred
+__device__ __forceinline__ int sel_block_prefix(int* s_warp, bool pred) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned bal = __ballot_sync(0xffffffffu, pred);
   if (lane == 0) s_warp[warp] = __popc(bal);
   __syncthreads();
   int prefix = 0;
   for (int w = 0; w < warp; w++) prefix += s_warp[w];
-  if (keep) {
-    const int dst = block_offsets[b * nblocks + blockIdx.x] + prefix + __popc(bal & ((1u << lane) - 1u));
-    if (dst < cap) {
-      float* o = dets + ((size_t)b * cap + dst) * 6;
-      o[0] = row[0]; o[1] = row[1]; o[2] = row[2]; o[3] = row[3]; o[4] = row[4]; o[5] = conf;
-    }
+  return prefix + __popc(bal & ((1u << lane) - 1u));
+}
+
+__global__ void __launch_bounds__(SEL_T) sel_write_kernel(const float* __restrict__ io, int p, int nc,
+                                                          const unsigned* __restrict__ keys,
+                                                          const SelState* __restrict__ st,
+                                                          const int* __restrict__ block_offsets,
+                                                          const int* __restrict__ totals, int nblocks,
+                                                          float* __restrict__ dets, int cap, int* __restrict__ n_out) {
+  __shared__ int s_warp[2][SEL_T / 32];
+  const int b = blockIdx.y;
+  const int i = blockIdx.x * SEL_T + threadIdx.x;
+  const unsigned v = st[b].prefix;
+  const int need = st[b].done ? 0 : st[b].k;
+  const unsigned key = i < p ? keys[(size_t)b * p + i] : 0u;
+  const bool is_above = i < p && key > v, is_tied = i < p && key == v;
+  const int above_before = block_offsets[((size_t)b * 2 + 0) * nblocks + blockIdx.x] +
+                           sel_block_prefix(s_warp[0], is_above);
+  const int tied_before = block_offsets[((size_t)b * 2 + 1) * nblocks + blockIdx.x] +
+                          sel_block_prefix(s_warp[1], is_tied);
+  if (is_above || (is_tied && tied_before < need)) {
+    const float* row = io + ((size_t)b * p + i) * (6 + nc);
+    float* o = dets + ((size_t)b * cap + above_before + min(tied_before, need)) * 6;
+    o[0] = row[0]; o[1] = row[1]; o[2] = row[2]; o[3] = row[3]; o[4] = row[4]; o[5] = __uint_as_float(key);
   }
+  if (blockIdx.x == 0 && threadIdx.x == 0) n_out[b] = totals[b * 2 + 0] + min(totals[b * 2 + 1], need);
 }
 
 }  // namespace ryolo
@@ -180,8 +239,10 @@ using namespace ryolo;
 extern "C" size_t ryolo_detect_select_workspace_bytes(int batch, int p) {
   if (batch <= 0 || p <= 0) return 256;
   const size_t nblocks = (size_t)(p + SEL_T - 1) / SEL_T;
-  return align_up((size_t)batch * SEL_BINS * sizeof(int), 256) + align_up((size_t)batch * sizeof(int), 256) +
-         align_up((size_t)batch * nblocks * sizeof(int), 256) + 256;
+  return SEL_PASSES * align_up((size_t)batch * SEL_BINS * sizeof(int), 256) +
+         align_up((size_t)batch * sizeof(SelState), 256) + align_up((size_t)batch * p * sizeof(unsigned), 256) +
+         align_up((size_t)batch * 2 * nblocks * sizeof(int), 256) + align_up((size_t)batch * 2 * sizeof(int), 256) +
+         256;
 }
 
 extern "C" int ryolo_detect_select(const float* io, int batch, int p, int nc, float conf_thres, float min_wh, int limit,
@@ -190,27 +251,37 @@ extern "C" int ryolo_detect_select(const float* io, int batch, int p, int nc, fl
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RYOLO_ARG_CHECK(io && dets_out && n_out && workspace && batch > 0 && p > 0 && nc >= 1 && limit > 0 && cap >= limit);
   RYOLO_ARG_CHECK(batch <= 65535);
+  RYOLO_ARG_CHECK(conf_thres >= 0.f);   // also rejects NaN; a positive conf's bit pattern orders like its value
   if (workspace_bytes < ryolo_detect_select_workspace_bytes(batch, p)) {
     set_err("ryolo_detect_select: workspace too small");
     return RYOLO_E_WORKSPACE;
   }
   const int nblocks = (p + SEL_T - 1) / SEL_T;
   Carver c(workspace);
-  int* hist = c.take<int>((size_t)batch * SEL_BINS);
-  int* t_bin = c.take<int>(batch);
-  int* counts = c.take<int>((size_t)batch * nblocks);
-  RYOLO_CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)batch * SEL_BINS * sizeof(int), stream));
+  int* hist = c.take<int>((size_t)SEL_PASSES * batch * SEL_BINS);
+  SelState* st = c.take<SelState>(batch);
+  unsigned* keys = c.take<unsigned>((size_t)batch * p);
+  int* counts = c.take<int>((size_t)batch * 2 * nblocks);
+  int* totals = c.take<int>((size_t)batch * 2);
+  RYOLO_CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)SEL_PASSES * batch * SEL_BINS * sizeof(int), stream));
   dim3 gh((p + SEL_ROWS_PER_CTA - 1) / SEL_ROWS_PER_CTA, batch);
-  sel_hist_kernel<<<gh, SEL_T, 0, stream>>>(io, p, nc, conf_thres, min_wh, hist);
+  sel_key_hist_kernel<<<gh, SEL_T, 0, stream>>>(io, p, nc, conf_thres, min_wh, keys, hist);
   RYOLO_LAUNCH_CHECK();
-  sel_thresh_kernel<<<batch, 1024, 0, stream>>>(hist, limit, t_bin);
+  sel_radix_kernel<<<batch, 1024, 0, stream>>>(hist, 0, limit, st);
   RYOLO_LAUNCH_CHECK();
+  for (int pass = 1; pass < SEL_PASSES; pass++) {
+    int* h = hist + (size_t)pass * batch * SEL_BINS;
+    sel_digit_hist_kernel<<<gh, SEL_T, 0, stream>>>(keys, p, pass, st, h);
+    RYOLO_LAUNCH_CHECK();
+    sel_radix_kernel<<<batch, 1024, 0, stream>>>(h, pass, limit, st);
+    RYOLO_LAUNCH_CHECK();
+  }
   dim3 gc(nblocks, batch);
-  sel_count_kernel<<<gc, SEL_T, 0, stream>>>(io, p, nc, conf_thres, min_wh, t_bin, counts, nblocks);
+  sel_count_kernel<<<gc, SEL_T, 0, stream>>>(keys, p, st, counts, nblocks);
   RYOLO_LAUNCH_CHECK();
-  sel_scan_kernel<<<batch, 1024, 0, stream>>>(counts, nblocks, cap, n_out);
+  sel_scan_kernel<<<batch * 2, 1024, 0, stream>>>(counts, nblocks, totals);
   RYOLO_LAUNCH_CHECK();
-  sel_write_kernel<<<gc, SEL_T, 0, stream>>>(io, p, nc, conf_thres, min_wh, t_bin, counts, nblocks, dets_out, cap);
+  sel_write_kernel<<<gc, SEL_T, 0, stream>>>(io, p, nc, keys, st, counts, totals, nblocks, dets_out, cap, n_out);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }

@@ -167,11 +167,12 @@ def r_nms_batched(dets, counts, threshold, limit=None):
     return keep, num
 
 
-def detect_select(io, conf_thres, limit, min_wh=2.0, slack=2048):
+def detect_select(io, conf_thres, limit, min_wh=2.0):
     """Candidate selection of a whole decoded batch on the device: per image the `limit` most confident rows that pass
-    the reference's filter (utils/nms/nms.py:34-40).  Returns (dets [B, limit+slack, 6], counts [B] int32)."""
+    the reference's filter (utils/nms/nms.py:34-40), ties resolved by lowest row index, in input order.
+    conf_thres must be >= 0.  Returns (dets [B, limit, 6], counts [B] int32 = min(limit, rows passing the filter))."""
     bsz, p, no = io.shape
-    cap = int(limit) + int(slack)
+    cap = int(limit)
     with torch.cuda.device(io.device):
         dets = torch.empty((bsz, cap, 6), dtype=torch.float32, device=io.device)
         counts = torch.empty((bsz,), dtype=torch.int32, device=io.device)
@@ -187,14 +188,17 @@ def detect_select(io, conf_thres, limit, min_wh=2.0, slack=2048):
 def detect_postprocess(io, conf_thres, nms_thres, cap, filter_done_event=None):
     """detect.py:204-213 after the forward, for a whole batch WITHOUT host round trips: device-side candidate selection
     (filter + top-`cap` by confidence; the reference has no cap and relies on trained weights, a random-init network puts
-    ~half of the 545 832 proposals above any threshold) and ONE segmented rotated NMS over all images (single-class
-    configs: one segment per image).  io [B, P, 6+nc] float32 CUDA contiguous.
-    Returns dict(dets [B, cap+slack, 6], counts [B], keep [B, cap+slack] int64, num_keep [B] int32): image b keeps rows
+    ~half of the 545 832 proposals above any threshold) and ONE segmented rotated NMS over all images, one segment per
+    image.  Single-class configs only: io [B, P, 7] float32 CUDA contiguous.
+    Returns dict(dets [B, cap, 6], counts [B], keep [B, cap] int64, num_keep [B] int32): image b keeps rows
     dets[b, keep[b, :num_keep[b]]]."""
+    if io.dim() != 3 or io.shape[-1] != 7:
+        raise ValueError("detect_postprocess runs class-agnostic NMS and takes single-class io [B, P, 7], got %s; "
+                         "use non_max_suppression for multi-class configs (NMS per class)" % (tuple(io.shape),))
     if not io.is_contiguous():
         io = io.contiguous()
     dets, counts = detect_select(io, conf_thres, cap)
     if filter_done_event is not None:
         filter_done_event.record()
-    keep, num = r_nms_batched(dets, counts, nms_thres, limit=cap)
+    keep, num = r_nms_batched(dets, counts, nms_thres)
     return {"dets": dets, "counts": counts, "keep": keep, "num_keep": num}

@@ -109,6 +109,83 @@ def adversarial_dets(seed=7):
     return torch.cat([b, tie_free_scores(len(b), seed + 1)[:, None]], 1).contiguous()
 
 
+def filter_edge_rows(nc, conf_thres, min_wh, seed):
+    """Decoded rows [n, 6+nc] at the edges of the non_max_suppression candidate filter (utils/nms/nms.py:34-40) and of
+    a 4096-bin confidence histogram: conf exactly on bin edges k/4096, one float below and above each; conf == 1.0 in
+    many rows; conf == conf_thres and w or h == min_wh (all excluded: strict comparisons) next to the first float above
+    each (included); NaN / +inf / -inf in every column in turn, class columns included; tied class maxima (nc > 1)."""
+    g = torch.Generator().manual_seed(seed)
+    f32 = torch.float32
+
+    def boxes(n):
+        b = gen_boxes(n, seed + n, 608.0)
+        b[:, 2:4] = min_wh + 1.0 + 60.0 * torch.rand(n, 2, generator=g)
+        return b
+
+    def rows(conf):
+        """rows whose obj * max(cls) is conf exactly: the maximum class score is 1.0 (twice when nc > 1)"""
+        n = len(conf)
+        cls = 0.999 * torch.rand(n, nc, generator=g)
+        cls[:, 0] = 1.0
+        if nc > 1:
+            cls[:, nc - 1] = 1.0
+        return torch.cat([boxes(n), conf[:, None], cls], 1).to(f32)
+
+    edges = torch.arange(1, 4097, dtype=torch.float64).div(4096).to(f32)
+    edges = edges[edges >= conf_thres]
+    up = torch.nextafter(edges, torch.full_like(edges, 2.0))
+    down = torch.nextafter(edges, torch.zeros_like(edges))
+    parts = [rows(edges), rows(up[up <= 1.0]), rows(down), rows(torch.ones(700))]
+    thr = torch.tensor([conf_thres], dtype=f32)
+    above_thr = torch.nextafter(thr, torch.tensor([2.0]))
+    at = rows(thr.repeat(40))
+    at[20:, 5] = above_thr                                     # first float above the threshold: included
+    parts.append(at)
+    wh = rows(torch.full((60,), 0.8))
+    wh[:20, 2] = min_wh                                        # w == min_wh: excluded
+    wh[20:40, 3] = min_wh                                      # h == min_wh: excluded
+    wh[40:50, 2] = torch.nextafter(torch.tensor(float(min_wh)), torch.tensor(1e9))
+    wh[50:60, 3] = torch.nextafter(torch.tensor(float(min_wh)), torch.tensor(1e9))
+    parts.append(wh)
+    for col in range(6 + nc):
+        for bad in (float("nan"), float("inf"), -float("inf")):
+            r = rows(torch.full((3,), 0.9))
+            r[:, col] = bad
+            parts.append(r)
+    if nc > 1:                                                 # class scores: max below 1, tied, product rounds
+        r = rows(0.5 + 0.5 * torch.rand(300, generator=g))
+        r[:, 6:] = torch.rand(300, nc, generator=g)
+        r[:150, 6] = r[:150, 6 + nc - 1] = r[:150, 6:].max(1).values
+        parts.append(r)
+    out = torch.cat(parts, 0)
+    return out[torch.randperm(len(out), generator=g)].contiguous()
+
+
+def check_postprocess_equals_per_image(io, conf_thres, nms_thres, cap, min_wh=2.0):
+    """nms.detect_postprocess (device-side selection + segmented NMS) == the per-image pipeline (nms_filter -> stable
+    top-cap by confidence -> rows back in input order -> r_nms), image by image, bit for bit: the selection is exactly
+    the top-cap candidates and the kept boxes are identical.  io [B, P, 7] CUDA.  Returns each image's candidate
+    confidences (the filter's survivors, input order)."""
+    import rotate_yolov3_b200 as pkg
+    from rotate_yolov3_b200.nms import detect_postprocess, nms_filter
+    res = detect_postprocess(io, conf_thres, nms_thres, cap)
+    confs = []
+    for b in range(io.shape[0]):
+        cand = nms_filter(io[b].clone(), conf_thres, min_wh)             # [n, 8] in input order
+        confs.append(cand[:, 5])
+        top = torch.sort(torch.argsort(cand[:, 5], descending=True, stable=True)[:cap]).values
+        want_sel = cand[top][:, :6].contiguous()
+        n = int(res["counts"][b])
+        assert n == len(want_sel), (b, n, len(want_sel))
+        assert torch.equal(res["dets"][b, :n], want_sel), b
+        want = want_sel[pkg.r_nms(want_sel, nms_thres)] if len(want_sel) else want_sel
+        got = res["dets"][b][res["keep"][b, :int(res["num_keep"][b])]]
+        assert got.shape == want.shape, (b, got.shape, want.shape)
+        assert torch.equal(got, want), b
+    assert res["dets"].shape == (io.shape[0], cap, 6) and res["keep"].shape == (io.shape[0], cap)
+    return confs
+
+
 def init_darknet_weights(model, seed=0):
     """Deterministic non-trivial parameters for a (reference or our) Darknet: He-scaled conv weights, randomised BN
     affine + running statistics and PReLU slopes (defaults mu=0, var=1, slope=0.1 would hide folding bugs,

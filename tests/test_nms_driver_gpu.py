@@ -31,21 +31,32 @@ def test_non_max_suppression_vs_reference_driver():
         assert np.array_equal(out1[i].cpu().numpy(), g["out1_%d" % i])
 
 
+def _same_bits(a, b):
+    """bit-identical, except that any NaN equals any NaN (payloads are not part of IEEE arithmetic's result)"""
+    nan = torch.isnan(a)
+    return torch.equal(nan, torch.isnan(b)) and torch.equal(a.view(torch.int32)[~nan], b.view(torch.int32)[~nan])
+
+
 def test_filter_large_and_empty():
+    import helpers
     import rotate_yolov3_b200 as pkg
     g = torch.Generator().manual_seed(0)
     p = torch.rand(100003, 7, generator=g)
     p[:, 2:4] *= 10
     p[::7, 5] = 0.0
-    ref = p.clone()
-    cc, ci = ref[:, 6:].max(1)
-    ref[:, 5] *= cc
-    keep = (ref[:, 5] > 0.25) & (ref[:, 2:4] > 2).all(1) & torch.isfinite(ref).all(1)
-    want = torch.cat([ref[keep][:, :6], cc[keep, None], ci[keep, None].float()], 1)
-    pc = p.cuda()
-    got = pkg.nms_filter(pc, 0.25, 2.0)
-    assert torch.equal(got.cpu(), want)
-    assert torch.equal(pc.cpu(), ref)
+    # the uniform rows above, then rows at the filter's edges: conf on and next to 4096-bin edges and the threshold,
+    # w / h == min_wh, NaN / +-inf in every column in turn, tied class maxima
+    inputs = [(p, 0.25)] + [(helpers.filter_edge_rows(nc, 0.5, 2.0, seed=11), 0.5) for nc in (1, 3)]
+    for p, conf_thres in inputs:
+        ref = p.clone()
+        cc, ci = ref[:, 6:].max(1)
+        ref[:, 5] *= cc
+        keep = (ref[:, 5] > conf_thres) & (ref[:, 2:4] > 2).all(1) & torch.isfinite(ref).all(1)
+        want = torch.cat([ref[keep][:, :6], cc[keep, None], ci[keep, None].float()], 1)
+        pc = p.cuda()
+        got = pkg.nms_filter(pc, conf_thres, 2.0)
+        assert _same_bits(got.cpu(), want)
+        assert _same_bits(pc.cpu(), ref)
     none = pkg.non_max_suppression(torch.zeros(2, 10, 7, device="cuda"), 0.5, 0.5)
     assert none == [None, None]
 

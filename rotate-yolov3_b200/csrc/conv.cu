@@ -20,10 +20,12 @@
 //   warp group 0   TMA producer (one thread): per k-step one A box (shifted by the tap offset) + one B box into a
 //                  128B-swizzled shared-memory stage, completion on an mbarrier (expect_tx); gives its registers to
 //                  the MMA warp groups (setmaxnreg);
-//   warp groups 1, 2   64 pixel rows each: wgmma m64n64k16 per 64 filters of the tile, fp32 accumulators in
-//                  registers, one k-step kept in flight (the stage of the previous one is released when it retires);
-//                  then the epilogue straight from the accumulator fragments: +bias -> PReLU -> +residual -> bf16
-//                  (or fp32 NCHW for the heads, or the nearest x2 up-sampled grid).  The producer keeps filling the
+//   warp groups 1, 2   64 pixel rows each: one wgmma m64n{BN}k16 per 16 channels (the A slice is read from shared
+//                  memory once for the whole tile width), fp32 accumulators in registers, one k-step kept in flight
+//                  (the stage of the previous one is released when it retires); then the epilogue: +bias -> PReLU ->
+//                  +residual -> bf16.  Same-grid outputs are staged in shared memory and leave through TMA bulk
+//                  stores that drain while the next tile's MMAs run; fp32 NCHW heads, the nearest x2 up-sampled grid
+//                  and the strided fallback are stored straight from the fragments.  The producer keeps filling the
 //                  ring with the next tile's operands while the epilogue runs.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -67,14 +69,18 @@ struct ConvSmem {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = BN == 256 ? 4 : (BN == 128 ? 6 : 8);   // 192 KB of operand ring
-  static constexpr int kBarOffset = kStages * kStageBytes;
+  // operand ring + the output staging tile; 144 / 192 / 192 KB of ring
+  static constexpr int kStages = BN == 256 ? 3 : (BN == 128 ? 6 : 8);
+  static constexpr int kStagingOffset = kStages * kStageBytes;
+  static constexpr int kStagingBytes = BM * BN * 2;   // per warp group and 64 filters: one [64 px x 64 ch] box, 8 KB
+  static constexpr int kBarOffset = kStagingOffset + kStagingBytes;
   static constexpr int kTotal = kBarOffset + 2 * kStages * 8 + 1024 /*alignment slack*/;
 };
 
 template <int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const ConvParams p) {
+conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                  const __grid_constant__ CUtensorMap map_out, const ConvParams p) {
   using S = ConvSmem<BN>;
   constexpr int NS = BN / 64;   // m64n64 sub-tiles per warp group
   extern __shared__ unsigned char smem_raw[];
@@ -128,7 +134,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   const int half = wg - 1;
   const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
   const int quad = lane & 3;
-  float acc[NS][32];
+  float acc[BN / 2];   // m64n{BN} fragment: [32 n + i] is entry i of the 64-filter sub-tile n
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -139,15 +145,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       mbar_wait(full_bar(stage), phase);
       const uint32_t sa = smem_base + stage * S::kStageBytes;
       const uint64_t adesc = make_smem_desc(sa + half * 64 * 128);
+      // the B box is BN consecutive 128-byte rows: one descriptor covers the whole tile
+      const uint64_t bdesc = make_smem_desc(sa + S::kABytes);
       wg_fence();
 #pragma unroll
       for (int k = 0; k < BK / 16; k++) {
-#pragma unroll
-        for (int n = 0; n < NS; n++) {
-          // +32 bytes (16 bf16) along K inside the swizzle atom: start-address field += 2
-          const uint64_t bdesc = make_smem_desc(sa + S::kABytes + n * 64 * 128);
-          wgmma_n64<0, 0>(acc[n], adesc + 2 * k, bdesc + 2 * k, (kk | k) != 0);
-        }
+        // +32 bytes (16 bf16) along K inside the swizzle atom: start-address field += 2
+        wgmma_bf16<BN, 0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (kk | k) != 0);
       }
       wg_commit();
       // the previous k-step has retired: its stage may be refilled
@@ -157,11 +161,67 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       if (++stage == S::kStages) { stage = 0; phase ^= 1; }
     }
     wg_wait<0>();
-#pragma unroll
-    for (int n = 0; n < NS; n++) wg_fence_regs(acc[n]);
+    wg_fence_regs(acc);
     if (lane == 0) mbar_arrive(empty_bar(prev));
 
     // ---- epilogue: this thread holds rows r0 and r0 + 8, columns 8 j + 2 quad + {0, 1} of every 64-filter sub-tile
+    if (p.same_grid) {
+      // The tile's rows ARE output rows: the warp group converts its 64 x BN fragment into its half of the staging tile
+      // (one 128B-swizzled [64 px x 64 ch] TMA box per 64 filters: a warp's 8 rows x 16 bytes land in 8 distinct 16-byte
+      // chunks, no bank conflicts) and one thread stores it with TMA.  The output map's extents (store_cols channels, np
+      // rows) clip what lies beyond them; the MMAs of the next tile start while the store drains.
+      const uint32_t stg = smem_base + S::kStagingOffset + half * NS * 8192;
+      if (t == 0) bulk_wait_read();   // the previous tile's stores have read the staging tile
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
+#pragma unroll
+      for (int i = 0; i < 2; i++) {
+        const int row = warp * 16 + (lane >> 2) + 8 * i;
+        const int pix = mt * BM + half * 64 + row;   // flat padded pixel; >= np is clipped by the store
+        int b, yp, xp, tt;
+        fast_divmod(pix, p.d_wp, tt, xp);
+        fast_divmod(tt, p.d_hp, b, yp);
+        // halo rows are stored as zeros: the halo stays zero
+        const bool valid = pix < p.np && xp >= 1 && xp <= p.wp - 2 && yp >= 1 && yp <= p.hp - 2;
+#pragma unroll
+        for (int n = 0; n < NS; n++) {
+#pragma unroll
+          for (int j = 0; j < 8; j++) {
+            const int col = nt * BN + n * 64 + 8 * j + 2 * quad;   // even filter index of this thread's pair
+            uint32_t hw = 0u;
+            if (valid) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              float x0 = acc[32 * n + 4 * j + 2 * i] + bb.x, x1 = acc[32 * n + 4 * j + 2 * i + 1] + bb.y;
+              if (p.has_act) {
+                x0 = x0 > 0.f ? x0 : p.slope * x0;
+                x1 = x1 > 0.f ? x1 : p.slope * x1;
+              }
+              if (p.has_res && col < p.cout) {
+                // filters >= cout read as zero; a residual that is the output itself is read before the tile is stored
+                const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(p.residual + (size_t)pix * p.res_cs + col));
+                x0 += __uint_as_float(rw << 16);
+                if (col + 1 < p.cout) x1 += __uint_as_float(rw & 0xffff0000u);
+              }
+              const __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
+              hw = *reinterpret_cast<const uint32_t*>(&h);
+            }
+            st_shared_u32(stg + n * 8192 + row * 128 + ((j ^ (row & 7)) << 4) + quad * 4, hw);
+          }
+        }
+      }
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
+      if (t == 0) {
+        const int row0 = mt * BM + half * 64;
+        if (row0 < p.np) {
+#pragma unroll
+          for (int n = 0; n < NS; n++)
+            if (nt * BN + n * 64 < p.store_cols) tma_store_2d(&map_out, stg + n * 8192, nt * BN + n * 64, row0);
+        }
+        bulk_commit();
+      }
+      continue;
+    }
+    // up-sampled, strided or fp32 NCHW outputs: stored straight from the fragments
 #pragma unroll
     for (int i = 0; i < 2; i++) {
       const int pix = mt * BM + half * 64 + warp * 16 + (lane >> 2) + 8 * i;   // flat padded input-grid pixel
@@ -177,19 +237,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         ox >>= 1;
       }
       valid = valid && oy < p.oh && ox < p.ow;
-      if (!valid && !p.same_grid) continue;
+      if (!valid) continue;
 #pragma unroll
       for (int n = 0; n < NS; n++) {
 #pragma unroll
         for (int j = 0; j < 8; j++) {
           const int col = nt * BN + n * 64 + 8 * j + 2 * quad;   // even filter index of this thread's pair
           if (!p.out_f32_nchw && col >= p.store_cols) continue;
-          if (!valid) {   // halo row of a same-grid output: keep the halo zero
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)pix * p.out_cs + col) = 0u;
-            continue;
-          }
           const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-          float x0 = acc[n][4 * j + 2 * i] + bb.x, x1 = acc[n][4 * j + 2 * i + 1] + bb.y;
+          float x0 = acc[32 * n + 4 * j + 2 * i] + bb.x, x1 = acc[32 * n + 4 * j + 2 * i + 1] + bb.y;
           if (p.has_act) {
             x0 = x0 > 0.f ? x0 : p.slope * x0;
             x1 = x1 > 0.f ? x1 : p.slope * x1;
@@ -203,19 +259,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             if (col + 1 < p.cout) o[base + (size_t)(col + 1) * plane] = x1;
             continue;
           }
-          if (p.has_res && col < p.cout) {
-            // residual on the same padded grid (stride 1, no up-sampling); filters >= cout read as zero
-            const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(p.residual + (size_t)pix * p.res_cs + col));
-            x0 += __uint_as_float(rw << 16);
-            if (col + 1 < p.cout) x1 += __uint_as_float(rw & 0xffff0000u);
-          }
           const __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
           const uint32_t hw = *reinterpret_cast<const uint32_t*>(&h);
           __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out);
-          if (p.same_grid) {
-            *reinterpret_cast<uint32_t*>(o + (size_t)pix * p.out_cs + col) = hw;
-            continue;
-          }
           const int ohp = (p.upsample2x ? 2 * p.oh : p.oh) + 2, owp = (p.upsample2x ? 2 * p.ow : p.ow) + 2;
           const int reps = p.upsample2x ? 2 : 1;
           for (int ry = 0; ry < reps; ry++)
@@ -227,6 +273,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       }
     }
   }
+  if (p.same_grid && t == 0) bulk_wait();   // the CTA's last stores are complete before it exits
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -325,14 +372,15 @@ int encode_map_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t row
 }
 
 template <int BN>
-static int launch_conv(const CUtensorMap& ma, const CUtensorMap& mb, const ConvParams& p, cudaStream_t stream) {
+static int launch_conv(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const ConvParams& p,
+                       cudaStream_t stream) {
   using S = ConvSmem<BN>;
   static_assert(S::kTotal <= 227 * 1024, "shared memory budget");
   RYOLO_SMEM_OPT_IN(conv_igemm_kernel<BN>, S::kTotal);
   const int num_sms = gemm_sm_count();
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < num_sms ? total : num_sms;
-  conv_igemm_kernel<BN><<<grid, CONV_THREADS, S::kTotal, stream>>>(ma, mb, p);
+  conv_igemm_kernel<BN><<<grid, CONV_THREADS, S::kTotal, stream>>>(ma, mb, mo, p);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }
@@ -447,7 +495,15 @@ extern "C" int ryolo_conv_bn_act_fwd(const ryolo_conv_desc* d, const void* x, co
   st = encode_map_2d(&mb, packed_w, (uint64_t)g.cin_pad, (uint64_t)g.taps * g.cout_pad, (uint64_t)g.cin_pad * 2, BK,
                      (uint32_t)g.bn);
   if (st != RYOLO_OK) return st;
-  if (g.bn == 256) return launch_conv<256>(ma, mb, p, stream);
-  if (g.bn == 128) return launch_conv<128>(ma, mb, p, stream);
-  return launch_conv<64>(ma, mb, p, stream);
+  // same-grid output: the epilogue's TMA store map.  Base = the output view, inner extent = store_cols: channels at or
+  // beyond it (a concat neighbour, the rest of a wider buffer) are never written.  Other outputs leave it unused.
+  CUtensorMap mo;
+  memset(&mo, 0, sizeof(mo));
+  if (p.same_grid) {
+    st = encode_map_2d(&mo, y, (uint64_t)p.store_cols, (uint64_t)p.np, (uint64_t)p.out_cs * 2, 64, BM / 2);
+    if (st != RYOLO_OK) return st;
+  }
+  if (g.bn == 256) return launch_conv<256>(ma, mb, mo, p, stream);
+  if (g.bn == 128) return launch_conv<128>(ma, mb, mo, p, stream);
+  return launch_conv<64>(ma, mb, mo, p, stream);
 }

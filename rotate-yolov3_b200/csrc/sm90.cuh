@@ -40,6 +40,24 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 
+// TMA store of a shared-memory box; the parts of the box outside the tensor map's extents are not written.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the committed bulk stores have finished READING shared memory (the source may be overwritten)
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the committed bulk stores are complete
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy writes to shared memory become visible to the async proxy (TMA) of this CTA
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
 // Register budget of a warp-specialised CTA: the TMA warp group gives registers back, the MMA warp groups take them.
 template <int N>
 __device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
@@ -89,6 +107,55 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64
         "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
         "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+}
+// The full-width forms: one instruction reads its A slice once for all NN columns (NN / 64 m64n64k16 would read it
+// NN / 64 times).  The fragment is the NN / 64 fragments of m64n64k16 side by side: d[32 n + i] of m64n{NN}k16 is d[i]
+// of the m64n64k16 over columns [64 n, 64 n + 64).  B covers NN rows (K-major, SBO apart per 8) or NN / 64 groups of
+// 64 columns (MN-major, LBO apart).
+#define RYOLO_WG_F8(i)                                                                                              \
+  "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), \
+      "+f"(d[i + 7])
+#define RYOLO_WG_F32(i) RYOLO_WG_F8(i), RYOLO_WG_F8(i + 8), RYOLO_WG_F8(i + 16), RYOLO_WG_F8(i + 24)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : RYOLO_WG_F32(0), RYOLO_WG_F32(32)
+      : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, %131, %132;\n\t}"
+      : RYOLO_WG_F32(0), RYOLO_WG_F32(32), RYOLO_WG_F32(64), RYOLO_WG_F32(96)
+      : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+}
+#undef RYOLO_WG_F32
+#undef RYOLO_WG_F8
+// m64n{NN}k16 for NN = 64, 128, 256
+template <int NN, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[NN / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (NN == 256) wgmma_n256<TA, TB>(d, adesc, bdesc, acc);
+  else if constexpr (NN == 128) wgmma_n128<TA, TB>(d, adesc, bdesc, acc);
+  else wgmma_n64<TA, TB>(d, adesc, bdesc, acc);
 }
 __device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
   asm volatile(

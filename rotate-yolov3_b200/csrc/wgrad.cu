@@ -121,15 +121,13 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
   regs_alloc<232>();
   const int half = wg - 1;
   const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
-  float acc[TG][NS][32];
-  float sum[SEG ? TG : 1][SEG ? NS : 1][32];   // SEG: round-to-nearest running sum of the closed segments
+  float acc[TG][BN / 2];   // m64n{BN} fragment per tap: [32 n + v] is entry v of the 64-channel sub-tile n
+  float sum[SEG ? TG : 1][SEG ? BN / 2 : 1];   // SEG: round-to-nearest running sum of the closed segments
   if constexpr (SEG) {
 #pragma unroll
     for (int j = 0; j < TG; j++)
 #pragma unroll
-      for (int n = 0; n < NS; n++)
-#pragma unroll
-        for (int v = 0; v < 32; v++) sum[j][n][v] = 0.f;
+      for (int v = 0; v < BN / 2; v++) sum[j][v] = 0.f;
   }
   int stage = 0, prev = -1;
   uint32_t phase = 0;
@@ -143,11 +141,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
       // 16 pixels = two 8-row groups = 2048 bytes along K; this warp group's 64 filters are the box at half * 8192
       const uint64_t adesc = make_smem_desc_mn(sa + half * 8192 + k * 2048, 8192);
 #pragma unroll
-      for (int j = 0; j < TG; j++)
-#pragma unroll
-        for (int n = 0; n < NS; n++)
-          wgmma_n64<1, 1>(acc[j][n], adesc, make_smem_desc_mn(sa + kABytes + j * kBBytes + n * 8192 + k * 2048, 8192),
-                          (!seg_start || k > 0) ? 1u : 0u);
+      for (int j = 0; j < TG; j++)   // the tap's BN / 64 channel boxes are 8192 bytes (LBO) apart
+        wgmma_bf16<BN, 1, 1>(acc[j], adesc, make_smem_desc_mn(sa + kABytes + j * kBBytes + k * 2048, 8192),
+                             (!seg_start || k > 0) ? 1u : 0u);
     }
     wg_commit();
     bool seg_end = false;
@@ -157,13 +153,11 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
         // close the segment: fold it into the round-to-nearest running sum
         wg_wait<0>();
 #pragma unroll
-        for (int j = 0; j < TG; j++)
+        for (int j = 0; j < TG; j++) {
+          wg_fence_regs(acc[j]);
 #pragma unroll
-          for (int n = 0; n < NS; n++) {
-            wg_fence_regs(acc[j][n]);
-#pragma unroll
-            for (int v = 0; v < 32; v++) sum[j][n][v] = __fadd_rn(sum[j][n][v], acc[j][n][v]);
-          }
+          for (int v = 0; v < BN / 2; v++) sum[j][v] = __fadd_rn(sum[j][v], acc[j][v]);
+        }
         if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         if (lane == 0) mbar_arrive(empty_bar(stage));
         prev = -1;
@@ -178,19 +172,17 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
   }
   wg_wait<0>();
 #pragma unroll
-  for (int j = 0; j < TG; j++)
+  for (int j = 0; j < TG; j++) {
+    wg_fence_regs(acc[j]);
+    if constexpr (SEG) {
 #pragma unroll
-    for (int n = 0; n < NS; n++) {
-      wg_fence_regs(acc[j][n]);
-      if constexpr (SEG) {
-#pragma unroll
-        for (int v = 0; v < 32; v++) acc[j][n][v] = sum[j][n][v];
-      }
+      for (int v = 0; v < BN / 2; v++) acc[j][v] = sum[j][v];
     }
+  }
 
   if (p.ksplit > 1) {
     // split-K in a fixed order: store my fragment, take a ticket; the last split of the tile adds splits 0, 1, ...
-    constexpr int V = TG * NS * 32;
+    constexpr int V = TG * BN / 2;
     const int me = threadIdx.x - 128;                    // 0..255 over the two MMA warp groups
     const int tiles = p.tap_groups * p.n_tiles * p.m_tiles;
     const int tile = blockIdx.x - split * tiles;
@@ -198,9 +190,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
 #pragma unroll
     for (int j = 0; j < TG; j++)
 #pragma unroll
-      for (int n = 0; n < NS; n++)
-#pragma unroll
-        for (int v = 0; v < 32; v++) __stcg(mine + (size_t)((j * NS + n) * 32 + v) * 256, acc[j][n][v]);
+      for (int v = 0; v < BN / 2; v++) __stcg(mine + (size_t)(j * BN / 2 + v) * 256, acc[j][v]);
     __shared__ int s_last;
     __threadfence();
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -211,17 +201,13 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
 #pragma unroll
     for (int j = 0; j < TG; j++)
 #pragma unroll
-      for (int n = 0; n < NS; n++)
-#pragma unroll
-        for (int v = 0; v < 32; v++) acc[j][n][v] = 0.f;
+      for (int v = 0; v < BN / 2; v++) acc[j][v] = 0.f;
     for (int s = 0; s < p.ksplit; s++) {
       const float* src = p.partials + (size_t)(s * tiles + tile) * V * 256 + me;
 #pragma unroll
       for (int j = 0; j < TG; j++)
 #pragma unroll
-        for (int n = 0; n < NS; n++)
-#pragma unroll
-          for (int v = 0; v < 32; v++) acc[j][n][v] += __ldcg(src + (size_t)((j * NS + n) * 32 + v) * 256);
+        for (int v = 0; v < BN / 2; v++) acc[j][v] += __ldcg(src + (size_t)(j * BN / 2 + v) * 256);
     }
   }
 
@@ -242,8 +228,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_const
           const int ci = nt * BN + n * 64 + 8 * c + 2 * (lane & 3);
           // the only writer of these dW entries in this launch
           float2 d = *reinterpret_cast<float2*>(drow + ci);
-          d.x += acc[j][n][4 * c + 2 * i];
-          d.y += acc[j][n][4 * c + 2 * i + 1];
+          d.x += acc[j][32 * n + 4 * c + 2 * i];
+          d.y += acc[j][32 * n + 4 * c + 2 * i + 1];
           *reinterpret_cast<float2*>(drow + ci) = d;
         }
       }

@@ -24,8 +24,9 @@
 //                  memory once for the whole tile width), fp32 accumulators in registers, one k-step kept in flight
 //                  (the stage of the previous one is released when it retires); then the epilogue: +bias -> PReLU ->
 //                  +residual -> bf16.  Same-grid outputs are staged in shared memory and leave through TMA bulk
-//                  stores that drain while the next tile's MMAs run; fp32 NCHW heads, the nearest x2 up-sampled grid
-//                  and the strided fallback are stored straight from the fragments.  The producer keeps filling the
+//                  stores that drain while the next tile's MMAs run; fp32 NCHW heads are transposed through the same
+//                  staging area and stored as per-channel pixel runs; the nearest x2 up-sampled grid and the strided
+//                  fallback are stored straight from the fragments.  The producer keeps filling the
 //                  ring with the next tile's operands while the epilogue runs.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -221,7 +222,63 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       }
       continue;
     }
-    // up-sampled, strided or fp32 NCHW outputs: stored straight from the fragments
+    if (p.out_f32_nchw && p.stride == 1 && !p.upsample2x) {
+      // Heads, fp32 [B, cout, oh, ow]: the fragment is transposed through the warp group's staging area 32 filters at a
+      // time ([32 ch][64 px] fp32, 8 KB; a pixel's column is XOR-swizzled by (ch / 2) % 4 so that the fragment writes
+      // and the row reads are conflict-free), then thread t stores pixel t % 64 of channels t / 64, t / 64 + 2, ..: a
+      // warp writes 32 consecutive pixels of one channel, contiguous in the output up to an image-row or halo boundary.
+      float* const stg = reinterpret_cast<float*>(smem_raw + (smem_base + S::kStagingOffset - smem_u32(smem_raw))) +
+                         half * NS * 2048;
+      const int spx = t & 63, sch = t >> 6;
+      size_t obase = 0;
+      bool ovalid;
+      {
+        const int pix = mt * BM + half * 64 + spx;
+        int b, yp, xp, tt;
+        fast_divmod(pix, p.d_wp, tt, xp);
+        fast_divmod(tt, p.d_hp, b, yp);
+        ovalid = pix < p.np && xp >= 1 && xp <= p.wp - 2 && yp >= 1 && yp <= p.hp - 2 && yp - 1 < p.oh && xp - 1 < p.ow;
+        obase = (size_t)b * p.cout * p.oh * p.ow + (size_t)(yp - 1) * p.ow + (xp - 1);
+      }
+      const size_t plane = (size_t)p.oh * p.ow;
+      float* const o = reinterpret_cast<float*>(p.out);
+#pragma unroll
+      for (int n = 0; n < NS; n++) {
+#pragma unroll
+        for (int hc = 0; hc < 2; hc++) {
+#pragma unroll
+          for (int i = 0; i < 2; i++) {
+            const int row = warp * 16 + (lane >> 2) + 8 * i;
+#pragma unroll
+            for (int jj = 0; jj < 4; jj++) {
+              const int j = 4 * hc + jj;
+              const int col = nt * BN + n * 64 + 8 * j + 2 * quad;   // even filter index of this thread's pair
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+              float x0 = acc[32 * n + 4 * j + 2 * i] + bb.x, x1 = acc[32 * n + 4 * j + 2 * i + 1] + bb.y;
+              if (p.has_act) {
+                x0 = x0 > 0.f ? x0 : p.slope * x0;
+                x1 = x1 > 0.f ? x1 : p.slope * x1;
+              }
+              const int ch = 8 * jj + 2 * quad;                       // (ch / 2) % 4 == quad
+              stg[ch * 64 + (row ^ (quad << 3))] = x0;
+              stg[(ch + 1) * 64 + (row ^ (quad << 3))] = x1;
+            }
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
+          if (ovalid) {
+#pragma unroll
+            for (int s = 0; s < 16; s++) {
+              const int ch = sch + 2 * s;
+              const int col = nt * BN + n * 64 + hc * 32 + ch;
+              if (col < p.cout) o[obase + (size_t)col * plane] = stg[ch * 64 + (spx ^ (((ch >> 1) & 3) << 3))];
+            }
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");   // the area is free for the next 32 filters
+        }
+      }
+      continue;
+    }
+    // up-sampled or strided outputs: stored straight from the fragments
 #pragma unroll
     for (int i = 0; i < 2; i++) {
       const int pix = mt * BM + half * 64 + warp * 16 + (lane >> 2) + 8 * i;   // flat padded input-grid pixel

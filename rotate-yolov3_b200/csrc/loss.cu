@@ -1,7 +1,9 @@
 // Dense part of compute_loss (SURVEY.md 8 row a6, reference model/loss.py:340-348): the objectness term
 // BCEWithLogitsLoss(pos_weight)(pi[..., 5], tobj) runs over EVERY cell of the three head maps (64 x 72 x (19^2 + 38^2 +
 // 76^2) = 35 M cells per step).  Written as framework element-wise ops it costs ~20 passes over strided views of the head
-// tensors (forward + autograd) plus a permute copy each way -- ~4 ms of a 66 ms step.  Here: one kernel for the loss sum,
+// tensors (forward + autograd) plus a permute copy each way; its HBM bound at batch 64 is ~0.5 ms (8 B read per cell
+// forward, 8 B read + the 7-channel fp32 cotangent written backward; DESIGN.md section 8 has the measured kernel times).
+// Here: one kernel for the loss sum,
 // one kernel that writes the WHOLE head cotangent (objectness channel = d(loss)/dx, every other channel zero; the few
 // matched rows are scattered on top by the caller), both reading the head tensor through its strides so that the NCHW
 // buffer the head convolution wrote is consumed in place (no permute().contiguous() copy), and a transposing
@@ -18,9 +20,18 @@ namespace ryolo {
 struct HeadView {            // logical [B, na, ny, nx, no] tensor with arbitrary element strides
   long long sb, sa, sy, sx, sc;
   int B, na, ny, nx, no;
+  int cells32;                 // B * na * ny * nx < 2^31: cell_offset divides by multiply + shift
+  FastDiv fx, fy, fa;
 };
 
 __device__ __forceinline__ size_t cell_offset(const HeadView& v, size_t cell) {
+  if (v.cells32) {
+    int r, x, y, a, b;
+    fast_divmod((int)cell, v.fx, r, x);
+    fast_divmod(r, v.fy, r, y);
+    fast_divmod(r, v.fa, b, a);
+    return (size_t)(b * v.sb + a * v.sa + y * v.sy + x * v.sx);
+  }
   const int x = (int)(cell % v.nx);
   size_t r = cell / v.nx;
   const int y = (int)(r % v.ny);
@@ -207,29 +218,65 @@ __global__ void rows_gather_kernel(const float* __restrict__ x, HeadView v, RowI
 }
 // Several rows may name the same cell (targets sharing a grid cell and anchor).  Their gradients are added in ROW order
 // by the first row of the cell, so that the sum is the same every run: keys[i] = the cell of row i (~0 for rows that
-// write nothing), then one thread per row that owns its cell adds all rows of that cell in order.
+// write nothing), then one WARP per row: a live row looks for an earlier row of its cell, 128 keys per step (four
+// independent coalesced loads, one ballot each); the row that finds none owns the cell and walks the keys from itself to
+// the end the same way, and for every row j of the cell, in increasing j, lane k adds vals[j, k] * scale to channel k:
+//   g[cell, k] = fmaf(vals[jn, k], scale, ... fmaf(vals[j1, k], scale, g[cell, k]))
+// A live row reads at most R keys wherever it sits; all `no` channels ride on one walk (one walk per 32 channels).
+constexpr int SCATTER_UNROLL = 4;
 __global__ void rows_key_kernel(HeadView v, RowIdx r, unsigned long long* __restrict__ keys) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= r.rows) return;
   size_t off, cell;
   keys[i] = row_cell(r, v, i, &off, &cell) ? (unsigned long long)cell : ~0ull;
 }
-__global__ void rows_scatter_add_kernel(float* __restrict__ g, HeadView v, RowIdx r, const unsigned long long* __restrict__ keys,
-                                        const float* __restrict__ vals, const float* __restrict__ scale_dev) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+// bit u * 32 + l of the result: keys[j0 + u * 32 + l] == key and j0 + u * 32 + l < end (lanes agree on the result)
+__device__ __forceinline__ void match_keys(const unsigned long long* __restrict__ keys, int j0, int end,
+                                           unsigned long long key, int lane, unsigned (&m)[SCATTER_UNROLL]) {
+  unsigned long long k[SCATTER_UNROLL];
+#pragma unroll
+  for (int u = 0; u < SCATTER_UNROLL; u++) {
+    const int j = j0 + u * 32 + lane;
+    k[u] = j < end ? __ldg(keys + j) : ~0ull;
+  }
+#pragma unroll
+  for (int u = 0; u < SCATTER_UNROLL; u++) m[u] = __ballot_sync(0xffffffffu, k[u] == key);
+}
+__global__ void __launch_bounds__(256) rows_scatter_add_kernel(float* __restrict__ g, HeadView v, RowIdx r,
+                                                               const unsigned long long* __restrict__ keys,
+                                                               const float* __restrict__ vals,
+                                                               const float* __restrict__ scale_dev) {
+  const int i = (int)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
   if (i >= r.rows) return;
-  const unsigned long long key = keys[i];
+  const unsigned long long key = __ldg(keys + i);
   if (key == ~0ull) return;
-  for (int j = 0; j < i; j++)
-    if (__ldg(keys + j) == key) return;             // an earlier row owns this cell
+  unsigned m[SCATTER_UNROLL];
+  for (int j0 = 0; j0 < i; j0 += 32 * SCATTER_UNROLL) {
+    match_keys(keys, j0, i, key, lane, m);
+    unsigned any = 0u;
+#pragma unroll
+    for (int u = 0; u < SCATTER_UNROLL; u++) any |= m[u];
+    if (any) return;                                  // an earlier row owns this cell
+  }
   size_t off, cell;
   row_cell(r, v, i, &off, &cell);
   const float scale = __ldg(scale_dev);
-  for (int k = 0; k < v.no; k++) {
-    float acc = g[off + (size_t)k * v.sc];
-    for (int j = i; j < r.rows; j++)
-      if (__ldg(keys + j) == key) acc += vals[(size_t)j * v.no + k] * scale;
-    g[off + (size_t)k * v.sc] = acc;
+  for (int k0 = 0; k0 < v.no; k0 += 32) {
+    const int k = k0 + lane;
+    float* const gk = g + off + (size_t)k * v.sc;
+    float acc = k < v.no ? *gk : 0.f;
+    for (int j0 = i; j0 < r.rows; j0 += 32 * SCATTER_UNROLL) {
+      match_keys(keys, j0, r.rows, key, lane, m);
+#pragma unroll
+      for (int u = 0; u < SCATTER_UNROLL; u++) {
+        for (unsigned bits = m[u]; bits; bits &= bits - 1) {
+          const int j = j0 + u * 32 + __ffs(bits) - 1;
+          if (k < v.no) acc = fmaf(__ldg(vals + (size_t)j * v.no + k), scale, acc);
+        }
+      }
+    }
+    if (k < v.no) *gk = acc;
   }
 }
 __global__ void rows_set_tobj_kernel(float* __restrict__ tobj, HeadView v, RowIdx r) {
@@ -255,6 +302,8 @@ static inline bool mk_view(const long long* strides, int batch, int na, int ny, 
     if (strides[i] < 0) return false;
   v->sb = strides[0]; v->sa = strides[1]; v->sy = strides[2]; v->sx = strides[3]; v->sc = strides[4];
   v->B = batch; v->na = na; v->ny = ny; v->nx = nx; v->no = no;
+  v->cells32 = (long long)batch * na * ny * nx < (1ll << 31);
+  v->fx = make_fastdiv(nx); v->fy = make_fastdiv(ny); v->fa = make_fastdiv(na);
   return true;
 }
 
@@ -349,7 +398,7 @@ extern "C" int ryolo_loss_rows_scatter_add(float* grad, const long long* strides
   const RowIdx ri = mk_rows(b, a, gj, gi, mask, rows);
   rows_key_kernel<<<(rows + 255) / 256, 256, 0, stream>>>(v, ri, keys);
   RYOLO_LAUNCH_CHECK();
-  rows_scatter_add_kernel<<<(rows + 127) / 128, 128, 0, stream>>>(grad, v, ri, keys, vals, scale_dev);
+  rows_scatter_add_kernel<<<(unsigned)(((size_t)rows * 32 + 255) / 256), 256, 0, stream>>>(grad, v, ri, keys, vals, scale_dev);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }
@@ -364,6 +413,8 @@ extern "C" int ryolo_loss_rows_set_tobj(float* tobj, int batch, int na, int ny, 
   HeadView v;
   v.sb = v.sa = v.sy = v.sx = v.sc = 0;
   v.B = batch; v.na = na; v.ny = ny; v.nx = nx; v.no = 1;
+  v.cells32 = 0;
+  v.fx = v.fy = v.fa = make_fastdiv(1);
   rows_set_tobj_kernel<<<(rows + 255) / 256, 256, 0, stream>>>(tobj, v, mk_rows(b, a, gj, gi, mask, rows));
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;

@@ -1,7 +1,7 @@
 """Where the bf16 training step's time goes: per conv shape, the forward (conv_igemm_kernel), weight-gradient
 (conv_wgrad_kernel) and data-gradient (conv_igemm_kernel with the dgrad descriptor) launches of the batch-64 608x608
 Darknet-53 step, each timed with CUDA events and set next to a torch.matmul bf16 GEMM of the same M x N x K on the same
-card; then a torch.profiler breakdown of one eager step by kernel family.
+card; then a torch.profiler breakdown of one eager step by kernel family and by kernel name.
 
     python tools/conv_layer_times.py OUT_DIR [--batch 64] [--iters 20]
 
@@ -83,6 +83,20 @@ def family(name):
     if "ryolo" in name:
         return "other ryolo"
     return "framework"
+
+
+def kernel_name(name):
+    """the kernel's qualified name without the return type and the parameter list, at most 70 characters"""
+    if name.startswith("void "):
+        name = name[5:]
+    depth = 0
+    for i, ch in enumerate(name):         # cut at the parameter list, not at a '(' inside template arguments
+        depth += ch == "<"
+        depth -= ch == ">"
+        if ch == "(" and depth == 0 and i > 0:
+            name = name[:i]
+            break
+    return name if len(name) <= 70 else name[:67] + "..."
 
 
 def main():
@@ -214,7 +228,7 @@ def main():
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         train_step()
         torch.cuda.synchronize()
-    fam = {}
+    fam, kern = {}, {}
     for ev in prof.key_averages():
         t = getattr(ev, "device_time_total", None)
         if t is None:
@@ -223,11 +237,19 @@ def main():
             continue
         f = family(ev.key)
         fam[f] = fam.get(f, 0.0) + t / 1e3
+        name = kernel_name(ev.key)
+        k = kern.setdefault(name, {"family": f, "calls": 0, "ms": 0.0})
+        k["calls"] += ev.count
+        k["ms"] += t / 1e3
     kernel_ms = sum(fam.values())
+    # per kernel name: every kernel of the loss family and every ryolo kernel, plus the largest framework ones
+    shown = [(n, k) for n, k in sorted(kern.items(), key=lambda kv: -kv[1]["ms"])
+             if k["family"] != "framework" or k["ms"] >= 0.01 * kernel_ms]
 
     totals = {k: sum(r.get(k + "_us", 0.0) * r["count"] for r in rows.values()) / 1e3 for k in ("fwd", "wgrad", "dgrad")}
     res = {"gpu": clocks, "batch": B, "iters": args.iters, "rows": list(rows.values()),
-           "gemm_ms_from_rows": totals, "profile_ms_by_family": fam, "profile_kernel_ms": kernel_ms}
+           "gemm_ms_from_rows": totals, "profile_ms_by_family": fam, "profile_ms_by_kernel": kern,
+           "profile_kernel_ms": kernel_ms}
     with open(os.path.join(args.out_dir, "conv_layer_times.json"), "w") as f:
         json.dump(res, f, indent=1)
 
@@ -254,6 +276,10 @@ def main():
     lines.append("one eager step under torch.profiler, device time %.1f ms:" % kernel_ms)
     for k, v in sorted(fam.items(), key=lambda kv: -kv[1]):
         lines.append("  %-12s %8.1f ms  %5.1f %%" % (k, v, 100 * v / kernel_ms))
+    lines.append("by kernel (every ryolo kernel; framework kernels from 1 %% of the step):")
+    lines.append("  %-70s %-12s %6s %9s %9s" % ("kernel", "family", "calls", "ms", "us/call"))
+    for n, k in shown:
+        lines.append("  %-70s %-12s %6d %9.3f %9.1f" % (n, k["family"], k["calls"], k["ms"], 1e3 * k["ms"] / max(k["calls"], 1)))
     txt = "\n".join(lines)
     with open(os.path.join(args.out_dir, "conv_layer_times.txt"), "w") as f:
         f.write(txt + "\n")

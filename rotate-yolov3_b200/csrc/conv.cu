@@ -20,14 +20,17 @@
 //   warp group 0   TMA producer (one thread): per k-step one A box (shifted by the tap offset) + one B box into a
 //                  128B-swizzled shared-memory stage, completion on an mbarrier (expect_tx); gives its registers to
 //                  the MMA warp groups (setmaxnreg);
+//                  A second warp of warp group 0 is the epilogue DMA of same-grid outputs: it stores each filled
+//                  staging tile with TMA and, once the store has read it, refills the tile with a later tile's
+//                  residual (TMA, completion on an mbarrier) and its BN bias values;
 //   warp groups 1, 2   64 pixel rows each: one wgmma m64n{BN}k16 per 16 channels (the A slice is read from shared
 //                  memory once for the whole tile width), fp32 accumulators in registers, one k-step kept in flight
 //                  (the stage of the previous one is released when it retires); then the epilogue: +bias -> PReLU ->
-//                  +residual -> bf16.  Same-grid outputs are staged in shared memory and leave through TMA bulk
-//                  stores that drain while the next tile's MMAs run; fp32 NCHW heads are transposed through the same
-//                  staging area and stored as per-channel pixel runs; the nearest x2 up-sampled grid and the strided
-//                  fallback are stored straight from the fragments.  The producer keeps filling the
-//                  ring with the next tile's operands while the epilogue runs.
+//                  +residual -> bf16.  Same-grid outputs are written over the residual in the staging tile and leave
+//                  through the DMA warp's TMA stores, which drain while the next tile's MMAs run; fp32 NCHW heads are
+//                  transposed through the same staging area and stored as per-channel pixel runs; the nearest x2
+//                  up-sampled grid and the strided fallback are stored straight from the fragments.  The producer
+//                  keeps filling the ring with the next tile's operands while the epilogue runs.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -55,41 +58,53 @@ struct ConvParams {
   int oh, ow;         // output spatial size (unpadded)
   int out_cs;         // channel stride of the output buffer
   int store_cols;     // bf16 output: columns [0, store_cols) of the padded filter range are stored
-  int res_cs;         // channel stride of the residual buffer
-  int has_act, has_res, upsample2x, out_f32_nchw;
+  int has_act, upsample2x, out_f32_nchw;
   int same_grid;      // bf16 stride-1 non-upsampled output: the tile's rows ARE output rows, halo rows are stored as 0
   float slope;
   const float* bias;               // [cout_pad]
-  const __nv_bfloat16* residual;   // padded NHWC like the output, or null
   void* out;
   FastDiv d_ntiles, d_wp, d_hp;    // divisions of the epilogue's per-tile index arithmetic
 };
 
-template <int BN>
+// RES: the same-grid epilogue adds a residual (shortcut, dgrad accumulate) that TMA loads into the staging tile.
+template <int BN, bool RES>
 struct ConvSmem {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // operand ring + the output staging tile; 144 / 192 / 192 KB of ring
-  static constexpr int kStages = BN == 256 ? 3 : (BN == 128 ? 6 : 8);
+  // Operand ring next to the output staging tiles.  Residual launches at BN <= 128 double-buffer the staging tile, so
+  // that the store of one tile and the residual load of the next are in flight together; the BN = 128 ring gives up a
+  // stage for it (5 instead of 6).  At BN = 256 a second 64 KB tile would leave a 2-stage ring, which exposes the
+  // operand latency on every k-step, so one tile is kept and the residual of the next tile is loaded as soon as the
+  // store has read it.  144 / 192 (160) / 192 KB of ring.
+  static constexpr int kStages = BN == 256 ? 3 : (BN == 128 ? (RES ? 5 : 6) : 8);
+  static constexpr int kStagingTiles = RES && BN < 256 ? 2 : 1;
   static constexpr int kStagingOffset = kStages * kStageBytes;
   static constexpr int kStagingBytes = BM * BN * 2;   // per warp group and 64 filters: one [64 px x 64 ch] box, 8 KB
-  static constexpr int kBarOffset = kStagingOffset + kStagingBytes;
-  static constexpr int kTotal = kBarOffset + 2 * kStages * 8 + 1024 /*alignment slack*/;
+  static constexpr int kBiasOffset = kStagingOffset + kStagingTiles * kStagingBytes;   // fp32 [kStagingTiles][BN]
+  static constexpr int kBarOffset = kBiasOffset + kStagingTiles * BN * 4;
+  static constexpr int kTotal = kBarOffset + (2 * kStages + 2 * kStagingTiles) * 8 + 1024 /*alignment slack*/;
 };
 
-template <int BN>
+template <int BN, bool RES>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                  const __grid_constant__ CUtensorMap map_out, const ConvParams p) {
-  using S = ConvSmem<BN>;
+                  const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
+                  const ConvParams p) {
+  using S = ConvSmem<BN, RES>;
   constexpr int NS = BN / 64;   // m64n64 sub-tiles per warp group
+  constexpr int NT = S::kStagingTiles;
   extern __shared__ unsigned char smem_raw[];
   // 1024-byte alignment required by the 128B swizzle atoms
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  unsigned char* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + S::kBarOffset;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S::kStages + s); };
+  // staging tile b is `ready` when it may be written (its last store has read it; the residual and bias have landed),
+  // `filled` when the MMA warps have written the tile's output into it
+  auto ready_bar = [&](int b) { return bar_base + 8u * (2 * S::kStages + b); };
+  auto filled_bar = [&](int b) { return bar_base + 8u * (2 * S::kStages + NT + b); };
 
   const int wg = threadIdx.x >> 7;
   const int total_tiles = p.m_tiles * p.n_tiles;
@@ -100,14 +115,72 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 8);   // one arrive per MMA warp
     }
+    for (int b = 0; b < NT; b++) {
+      mbar_init(ready_bar(b), 1);
+      mbar_init(filled_bar(b), 8);   // one arrive per MMA warp
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if (wg == 0) {
-    // ===================== TMA producer =====================
     regs_dealloc<40>();
+    if (threadIdx.x >= 32 && threadIdx.x < 64 && p.same_grid) {
+      // ===================== epilogue DMA (same-grid outputs) =====================
+      const int lane = threadIdx.x & 31;
+      // make staging tile b ready for `tile`: its bias values, then its residual boxes or a plain arrive
+      auto prepare = [&](int tile, int b) {
+        int mt, nt;
+        fast_divmod(tile, p.d_ntiles, mt, nt);
+        float* const sb = reinterpret_cast<float*>(smem + S::kBiasOffset) + b * BN;
+        for (int c = lane; c < BN; c += 32) sb[c] = __ldg(p.bias + nt * BN + c);
+        __syncwarp();
+        if (lane != 0) return;
+        if constexpr (RES) {
+          // The map's inner extent is cout: filters at and above it load as zeros.  A box that starts at or beyond
+          // cout also starts at or beyond store_cols = round_up(cout, 32), and one that starts at or beyond np is
+          // clipped whole: neither is stored, so neither is loaded.
+          const int nc = min(NS, (p.cout - nt * BN + 63) / 64);
+          const int nh = mt * BM + 64 < p.np ? 2 : 1;
+          mbar_expect_tx(ready_bar(b), (uint32_t)(nh * nc * 8192));
+          const uint32_t stg = smem_base + S::kStagingOffset + b * S::kStagingBytes;
+          for (int h = 0; h < nh; h++)
+            for (int n = 0; n < nc; n++)
+              tma_load_2d(stg + (h * NS + n) * 8192, &map_res, ready_bar(b), nt * BN + n * 64, mt * BM + h * 64);
+        } else {
+          mbar_arrive(ready_bar(b));
+        }
+      };
+      int j = 0;
+      for (int tile = blockIdx.x; tile < total_tiles && j < NT; tile += gridDim.x, j++) prepare(tile, j);
+      j = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, j++) {
+        const int b = j % NT;
+        mbar_wait(filled_bar(b), (j / NT) & 1);
+        if (lane == 0) {
+          // the output map's extents (store_cols channels, np rows) clip what lies beyond them
+          int mt, nt;
+          fast_divmod(tile, p.d_ntiles, mt, nt);
+          const uint32_t stg = smem_base + S::kStagingOffset + b * S::kStagingBytes;
+          for (int h = 0; h < 2; h++) {
+            const int row0 = mt * BM + h * 64;
+            if (row0 >= p.np) break;
+            for (int n = 0; n < NS; n++)
+              if (nt * BN + n * 64 < p.store_cols) tma_store_2d(&map_out, stg + (h * NS + n) * 8192, nt * BN + n * 64, row0);
+          }
+          bulk_commit();
+        }
+        const int next = tile + NT * gridDim.x;
+        if (next < total_tiles) {
+          // the tiles partition the output: a later tile's residual never overlaps a store still in flight
+          if (lane == 0) bulk_wait_read();
+          prepare(next, b);
+        }
+      }
+      if (lane == 0) bulk_wait();   // the CTA's last stores are complete before it exits
+    }
     if (threadIdx.x == 0) {
+      // ===================== TMA producer =====================
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -138,7 +211,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   float acc[BN / 2];   // m64n{BN} fragment: [32 n + i] is entry i of the 64-filter sub-tile n
   int stage = 0;
   uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+  int jt = 0;          // tiles of this CTA so far: staging tile jt % NT
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, jt++) {
     int mt, nt;
     fast_divmod(tile, p.d_ntiles, mt, nt);
     int prev = -1;
@@ -169,15 +243,46 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     if (p.same_grid) {
       // The tile's rows ARE output rows: the warp group converts its 64 x BN fragment into its half of the staging tile
       // (one 128B-swizzled [64 px x 64 ch] TMA box per 64 filters: a warp's 8 rows x 16 bytes land in 8 distinct 16-byte
-      // chunks, no bank conflicts) and one thread stores it with TMA.  The output map's extents (store_cols channels, np
-      // rows) clip what lies beyond them; the MMAs of the next tile start while the store drains.
-      const uint32_t stg = smem_base + S::kStagingOffset + half * NS * 8192;
-      if (t == 0) bulk_wait_read();   // the previous tile's stores have read the staging tile
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
+      // chunks, no bank conflicts), over the residual the DMA warp loaded there, and the DMA warp stores it.  Every
+      // shared-memory read comes before the first write, so that the compiler may batch the reads.
+      const int sbuf = jt % NT;
+      mbar_wait(ready_bar(sbuf), (jt / NT) & 1);
+      uint32_t* const stg =
+          reinterpret_cast<uint32_t*>(smem + S::kStagingOffset + sbuf * S::kStagingBytes + half * NS * 8192);
+      const float* const sb = reinterpret_cast<const float*>(smem + S::kBiasOffset) + sbuf * BN;
+      // word index of this thread's pair (row warp * 16 + lane / 4 + 8 i, filters n * 64 + 8 j + 2 quad + {0, 1})
+      auto widx = [&](int i, int n, int j) {
+        const int row = warp * 16 + (lane >> 2) + 8 * i;
+        return n * 2048 + row * 32 + ((j ^ (row & 7)) << 2) + quad;
+      };
+#pragma unroll
+      for (int n = 0; n < NS; n++) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          const float2 bb = *reinterpret_cast<const float2*>(sb + n * 64 + 8 * j + 2 * quad);
+#pragma unroll
+          for (int i = 0; i < 2; i++) {
+            float& x0 = acc[32 * n + 4 * j + 2 * i];
+            float& x1 = acc[32 * n + 4 * j + 2 * i + 1];
+            // + bias even where it is zero: -0 + 0 = +0
+            x0 += bb.x;
+            x1 += bb.y;
+            if (p.has_act) {
+              x0 = x0 > 0.f ? x0 : p.slope * x0;
+              x1 = x1 > 0.f ? x1 : p.slope * x1;
+            }
+            if constexpr (RES) {
+              // filters at and above cout read as zeros; __fadd_rn is never contracted with the PReLU multiply
+              const uint32_t rw = stg[widx(i, n, j)];
+              x0 = __fadd_rn(x0, __uint_as_float(rw << 16));
+              x1 = __fadd_rn(x1, __uint_as_float(rw & 0xffff0000u));
+            }
+          }
+        }
+      }
 #pragma unroll
       for (int i = 0; i < 2; i++) {
-        const int row = warp * 16 + (lane >> 2) + 8 * i;
-        const int pix = mt * BM + half * 64 + row;   // flat padded pixel; >= np is clipped by the store
+        const int pix = mt * BM + half * 64 + warp * 16 + (lane >> 2) + 8 * i;   // flat padded pixel; >= np is clipped
         int b, yp, xp, tt;
         fast_divmod(pix, p.d_wp, tt, xp);
         fast_divmod(tt, p.d_hp, b, yp);
@@ -187,39 +292,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         for (int n = 0; n < NS; n++) {
 #pragma unroll
           for (int j = 0; j < 8; j++) {
-            const int col = nt * BN + n * 64 + 8 * j + 2 * quad;   // even filter index of this thread's pair
-            uint32_t hw = 0u;
-            if (valid) {
-              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-              float x0 = acc[32 * n + 4 * j + 2 * i] + bb.x, x1 = acc[32 * n + 4 * j + 2 * i + 1] + bb.y;
-              if (p.has_act) {
-                x0 = x0 > 0.f ? x0 : p.slope * x0;
-                x1 = x1 > 0.f ? x1 : p.slope * x1;
-              }
-              if (p.has_res && col < p.cout) {
-                // filters >= cout read as zero; a residual that is the output itself is read before the tile is stored
-                const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(p.residual + (size_t)pix * p.res_cs + col));
-                x0 += __uint_as_float(rw << 16);
-                if (col + 1 < p.cout) x1 += __uint_as_float(rw & 0xffff0000u);
-              }
-              const __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
-              hw = *reinterpret_cast<const uint32_t*>(&h);
-            }
-            st_shared_u32(stg + n * 8192 + row * 128 + ((j ^ (row & 7)) << 4) + quad * 4, hw);
+            const __nv_bfloat162 h = __floats2bfloat162_rn(acc[32 * n + 4 * j + 2 * i], acc[32 * n + 4 * j + 2 * i + 1]);
+            stg[widx(i, n, j)] = valid ? *reinterpret_cast<const uint32_t*>(&h) : 0u;
           }
         }
       }
       fence_proxy_async_smem();
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
-      if (t == 0) {
-        const int row0 = mt * BM + half * 64;
-        if (row0 < p.np) {
-#pragma unroll
-          for (int n = 0; n < NS; n++)
-            if (nt * BN + n * 64 < p.store_cols) tma_store_2d(&map_out, stg + n * 8192, nt * BN + n * 64, row0);
-        }
-        bulk_commit();
-      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(filled_bar(sbuf));
       continue;
     }
     if (p.out_f32_nchw && p.stride == 1 && !p.upsample2x) {
@@ -330,7 +410,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       }
     }
   }
-  if (p.same_grid && t == 0) bulk_wait();   // the CTA's last stores are complete before it exits
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -428,18 +507,24 @@ int encode_map_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t row
   return RYOLO_OK;
 }
 
-template <int BN>
-static int launch_conv(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const ConvParams& p,
-                       cudaStream_t stream) {
-  using S = ConvSmem<BN>;
+template <int BN, bool RES>
+static int launch_conv(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr,
+                       const ConvParams& p, cudaStream_t stream) {
+  using S = ConvSmem<BN, RES>;
   static_assert(S::kTotal <= 227 * 1024, "shared memory budget");
-  RYOLO_SMEM_OPT_IN(conv_igemm_kernel<BN>, S::kTotal);
+  RYOLO_SMEM_OPT_IN((conv_igemm_kernel<BN, RES>), S::kTotal);
   const int num_sms = gemm_sm_count();
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < num_sms ? total : num_sms;
-  conv_igemm_kernel<BN><<<grid, CONV_THREADS, S::kTotal, stream>>>(ma, mb, mo, p);
+  conv_igemm_kernel<BN, RES><<<grid, CONV_THREADS, S::kTotal, stream>>>(ma, mb, mo, mr, p);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
+}
+
+template <int BN>
+static int launch_conv(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr,
+                       bool has_res, const ConvParams& p, cudaStream_t stream) {
+  return has_res ? launch_conv<BN, true>(ma, mb, mo, mr, p, stream) : launch_conv<BN, false>(ma, mb, mo, mr, p, stream);
 }
 
 }  // namespace ryolo
@@ -535,14 +620,11 @@ extern "C" int ryolo_conv_bn_act_fwd(const ryolo_conv_desc* d, const void* x, co
   p.ow = d->stride == 2 ? (d->in_w + 1) / 2 : d->in_w;
   p.out_cs = d->cout_stride;
   p.store_cols = round_up(d->cout, 32);   // never touch channels beyond the 32-column chunk that holds the last filter
-  p.res_cs = d->res_stride;
   p.has_act = d->has_act;
-  p.has_res = d->has_residual;
   p.upsample2x = d->upsample2x;
   p.out_f32_nchw = d->out_dtype == RYOLO_DT_F32;
   p.slope = d->slope;
   p.bias = bias;
-  p.residual = static_cast<const __nv_bfloat16*>(residual);
   p.out = y;
   p.same_grid = (d->out_dtype == RYOLO_DT_BF16 && d->stride == 1 && !d->upsample2x) ? 1 : 0;
   CUtensorMap ma, mb;
@@ -554,13 +636,21 @@ extern "C" int ryolo_conv_bn_act_fwd(const ryolo_conv_desc* d, const void* x, co
   if (st != RYOLO_OK) return st;
   // same-grid output: the epilogue's TMA store map.  Base = the output view, inner extent = store_cols: channels at or
   // beyond it (a concat neighbour, the rest of a wider buffer) are never written.  Other outputs leave it unused.
-  CUtensorMap mo;
+  CUtensorMap mo, mr;
   memset(&mo, 0, sizeof(mo));
+  memset(&mr, 0, sizeof(mr));
   if (p.same_grid) {
     st = encode_map_2d(&mo, y, (uint64_t)p.store_cols, (uint64_t)p.np, (uint64_t)p.out_cs * 2, 64, BM / 2);
     if (st != RYOLO_OK) return st;
   }
-  if (g.bn == 256) return launch_conv<256>(ma, mb, mo, p, stream);
-  if (g.bn == 128) return launch_conv<128>(ma, mb, mo, p, stream);
-  return launch_conv<64>(ma, mb, mo, p, stream);
+  // residual (same grid: checked above): the same boxes as the store map; inner extent cout, so TMA zero-fills the
+  // filters at and above it.  It may be the output view itself, a view into a wider buffer, or a separate buffer.
+  const bool has_res = d->has_residual != 0;
+  if (has_res) {
+    st = encode_map_2d(&mr, residual, (uint64_t)d->cout, (uint64_t)p.np, (uint64_t)d->res_stride * 2, 64, BM / 2);
+    if (st != RYOLO_OK) return st;
+  }
+  if (g.bn == 256) return launch_conv<256>(ma, mb, mo, mr, has_res, p, stream);
+  if (g.bn == 128) return launch_conv<128>(ma, mb, mo, mr, has_res, p, stream);
+  return launch_conv<64>(ma, mb, mo, mr, has_res, p, stream);
 }

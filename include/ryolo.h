@@ -342,6 +342,24 @@ int ryolo_depth_to_space(const void* dxs, int dxs_cstride, int batch, int h, int
  * fp32.  Eval path. */
 int ryolo_se_block(void* x, int x_cstride, int batch, int h, int w, int c, const float* w1, const float* w2,
                    int reduced, float* sums_scratch, float* scale_scratch, void* stream);
+/* The same block out of place and deterministic, for graphs whose SE input x is read again (the reference's *_se.cfg: the
+ * shortcut three blocks later adds x, concat routes read x) and for training.  Per image b, channel c:
+ *   m = mean_hw x,  p = W1 m,  s = sigmoid(W2 relu(p)),  u = bf16(x s)  (u's halo is not written).
+ * m, s [batch, c] and p [batch, reduced] fp32 are outputs the backward reads.  Backward, gu = dL/du:
+ *   ds = sum_hw gu x,  da = ds s (1 - s),  dhid = (W2^T da) [p > 0],  dm = W1^T dhid,
+ *   gx = bf16([gx +] gu s + dm / hw)  (accumulate = 1 adds to the gradient other writers left in gx),
+ *   gw1 = sum_b dhid m^T [reduced, c],  gw2 = sum_b da relu(p)^T [c, reduced]  (overwritten; fp32).
+ * ds, dm [batch, c] fp32 are outputs.  Every reduction runs in a fixed order, none uses float atomics; an image's
+ * results do not depend on the batch it is in.  c % 8 == 0, c <= 2048; x, u, gu, gx 16-byte aligned.  workspace
+ * (caller-owned, >= ryolo_se_workspace_bytes) serves both directions; no allocation, no host synchronisation. */
+size_t ryolo_se_workspace_bytes(int batch, int h, int w, int c, int reduced);
+int ryolo_se_fwd(const void* x, int x_cstride, void* u, int u_cstride, int batch, int h, int w, int c,
+                 const float* w1, const float* w2, int reduced, float* m, float* p, float* s, void* workspace,
+                 size_t workspace_bytes, void* stream);
+int ryolo_se_bwd(const void* gu, int gu_cstride, const void* x, int x_cstride, void* gx, int gx_cstride,
+                 int accumulate, int batch, int h, int w, int c, const float* w1, const float* w2, int reduced,
+                 const float* m, const float* p, const float* s, float* ds, float* dm, float* gw1, float* gw2,
+                 void* workspace, size_t workspace_bytes, void* stream);
 /* 2x2 max pooling of a padded-NHWC bf16 tensor (reference: the maxpool blocks of
  * cfg/yolov3-tiny.cfg, model/models.py:79-87).  stride 2: [in_h/2, in_w/2] output; stride 1: same
  * size, the window past the right/bottom edge reads the zero halo exactly like the reference's

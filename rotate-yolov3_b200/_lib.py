@@ -96,6 +96,10 @@ SIGNATURES = {
     "ryolo_space_to_depth": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_depth_to_space": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "ryolo_se_block": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "ryolo_se_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "ryolo_se_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ryolo_se_bwd": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                          _vp, _sz, _vp]),
     "ryolo_maxpool2x2": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_nchw_to_padded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_im2col_first": (_i, [_vp, _i, _i, _i, _vp, _vp]),

@@ -27,7 +27,8 @@ from .parse_config import parse_model_cfg
 
 class SELayer(nn.Module):
     """reference model/models.py:16-31 (same parameter names: fc.0.weight [c/r, c], fc.2.weight [c, c/r]); executed by
-    ryolo_se_block inside the eval plan, this forward exists only for module-tree parity."""
+    ryolo_se_block / ryolo_se_fwd inside the eval plan and ryolo_se_fwd / ryolo_se_bwd inside the training plan, this
+    forward exists only for module-tree parity."""
 
     def __init__(self, channel, reduction=16):
         super().__init__()
@@ -376,12 +377,28 @@ class Darknet(nn.Module):
                 i += 2 if (fuse_res or fuse_up) else 1
                 continue
             if t == "se":
-                # squeeze-and-excitation rescales the previous block's output IN PLACE; legal when nothing else reads the
-                # unscaled tensor (the reference's graphs: [se] directly follows the down-sampling conv)
                 src = views[i - 1]
-                if src is None or (i - 1) in self.routes or src.c != int(d["channels"]):
-                    raise NotImplementedError("[se] block whose input is routed elsewhere / channel mismatch")
+                if src is None or src.c != int(d["channels"]):
+                    raise NotImplementedError("[se] block at %d: no materialised input / channel mismatch" % i)
                 fc = self.module_list[i].fc
+                cr = fc[0].weight.shape[0]
+                if (i - 1) in self.routes:
+                    # the unscaled input is read again (the reference's *_se.cfg: the shortcut three blocks later adds it,
+                    # concat routes read it): u = x * s goes to a buffer of its own
+                    v = out_view(i)
+                    steps.append(("se_fwd", dict(x=src.ptr, xcs=src.cs, u=v.ptr, ucs=v.cs, h=src.h, w=src.w, c=src.c,
+                                                 w1=fc[0].weight.detach().float().contiguous(),
+                                                 w2=fc[2].weight.detach().float().contiguous(), cr=cr,
+                                                 m=torch.zeros(batch * src.c, dtype=torch.float32, device=device),
+                                                 p=torch.zeros(batch * cr, dtype=torch.float32, device=device),
+                                                 s=torch.zeros(batch * src.c, dtype=torch.float32, device=device),
+                                                 ws=torch.empty(_lib.lib.ryolo_se_workspace_bytes(batch, src.h, src.w,
+                                                                                                  src.c, cr),
+                                                                dtype=torch.uint8, device=device), keep=(src, v))))
+                    views[i] = v
+                    i += 1
+                    continue
+                # otherwise the scale is applied IN PLACE: nothing else reads the unscaled tensor
                 steps.append(("se", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c,
                                          w1=fc[0].weight.detach().float().contiguous(),
                                          w2=fc[2].weight.detach().float().contiguous(), cr=fc[0].weight.shape[0],
@@ -486,6 +503,11 @@ class Darknet(nn.Module):
                 st = lib.ryolo_se_block(ctypes.c_void_p(a["x"]), a["xcs"], b, a["h"], a["w"], a["c"], _lib.ptr(a["w1"]),
                                         _lib.ptr(a["w2"]), a["cr"], _lib.ptr(a["sums"]), _lib.ptr(a["scale"]), stream)
                 _lib.check(st, "ryolo_se_block")
+            elif kind == "se_fwd":
+                st = lib.ryolo_se_fwd(ctypes.c_void_p(a["x"]), a["xcs"], ctypes.c_void_p(a["u"]), a["ucs"], b, a["h"], a["w"],
+                                      a["c"], _lib.ptr(a["w1"]), _lib.ptr(a["w2"]), a["cr"], _lib.ptr(a["m"]),
+                                      _lib.ptr(a["p"]), _lib.ptr(a["s"]), _lib.ptr(a["ws"]), a["ws"].numel(), stream)
+                _lib.check(st, "ryolo_se_fwd")
             elif kind == "s2d":
                 st = lib.ryolo_space_to_depth(ctypes.c_void_p(a["x"]), a["xcs"], b, a["h"], a["w"], a["c"],
                                               _lib.ptr(a["xs"]), a["xs"].shape[-1], stream)

@@ -90,6 +90,8 @@ class ParityPlan:
                 ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
                 c = sum(shape[l][0] for l in ls)
                 h, w = shape[ls[0]][1], shape[ls[0]][2]
+            elif t == "se":
+                raise NotImplementedError("[se] blocks have no parity-precision kernel; SE graphs run in precision='bf16'")
             elif t not in ("shortcut", "yolo"):
                 raise NotImplementedError("block type %r has no parity-precision kernel" % t)
             shape[i] = (c, h, w)

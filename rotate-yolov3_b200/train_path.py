@@ -44,7 +44,7 @@ class TrainPlan:
                 ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
                 c = sum(shape[l][0] for l in ls)
                 h, w = shape[ls[0]][1], shape[ls[0]][2]
-            elif t not in ("shortcut", "yolo"):
+            elif t not in ("shortcut", "yolo", "se"):
                 raise NotImplementedError("block type %r has no training kernel" % t)
             shape[i] = (c, h, w)
         self.shape = shape
@@ -105,6 +105,7 @@ class TrainPlan:
                     blk.src, blk.gsrc = views[i - 1], gviews[i - 1]
                     blk.k_eff = blk.k
                 blk.s2d = False
+                blk.se = None
                 blk.fuse_res = nxt == "shortcut" and i not in model.routes
                 blk.fuse_up = nxt == "upsample" and i not in model.routes and int(defs[i + 1]["stride"]) == 2
                 blk.is_head = nxt == "yolo"
@@ -165,7 +166,24 @@ class TrainPlan:
                 blocks.append(blk)
                 i += 2 if (blk.fuse_res or blk.fuse_up) else 1
                 continue
-            if t == "route":
+            if t == "se":
+                # out of place: u = x * s gets a buffer pair of its own and views[i]; views[i - 1] stays x, so that the
+                # shortcut three blocks later (`from=-4`) and concat routes read the unscaled tensor like the reference.
+                # The SE runs with the block that produced x: forward after its bn_act_fwd, backward before its bn_act_bwd.
+                x, gx = views[i - 1], gviews[i - 1]
+                prod = [p_ for p_ in blocks if not p_.is_head and p_.y is x]
+                if len(prod) != 1 or prod[0].se is not None or x.c != int(d["channels"]):
+                    raise NotImplementedError("[se] at block %d does not follow a conv block's output" % i)
+                se = _Block()
+                se.i, se.x, se.gx, se.c, se.h, se.w = i, x, gx, x.c, x.h, x.w
+                se.cr = model.module_list[i].fc[0].weight.shape[0]
+                ub, gub = alloc_pair(x.h, x.w, L.round_up(x.c, 32))
+                se.u, se.gu = _mk_view(ub, 0, x.c, x.h, x.w), _mk_view(gub, 0, x.c, x.h, x.w)
+                se.m, se.s, se.ds, se.dm = (torch.zeros(batch * x.c, dtype=torch.float32, device=device) for _ in range(4))
+                se.p = torch.zeros(batch * se.cr, dtype=torch.float32, device=device)
+                views[i], gviews[i] = se.u, se.gu
+                prod[0].se = se
+            elif t == "route":
                 ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
                 if len(ls) == 1:
                     views[i], gviews[i] = views[ls[0]], gviews[ls[0]]
@@ -173,6 +191,9 @@ class TrainPlan:
                 raise NotImplementedError("%s at block %d does not follow a convolution it can be fused into" % (t, i))
             i += 1
         self.blocks = blocks
+        ses = [b.se for b in blocks if b.se is not None]
+        self.se_ws = torch.empty(max([_lib.lib.ryolo_se_workspace_bytes(batch, se.h, se.w, se.c, se.cr) for se in ses] + [0]),
+                                 dtype=torch.uint8, device=device)
         # a block whose output feeds a space-to-depth (3x3 / stride 2) block writes the s2d copy itself (bn_act_fwd_s2d)
         for c_ in blocks:
             c_.xs_from_producer = False
@@ -193,6 +214,8 @@ class TrainPlan:
             written.setdefault(key, []).append((lo, hi))
             return covered
         for blk in reversed(blocks):
+            if blk.se is not None:
+                blk.se.gx_acc = claim(blk.se.gx)
             blk.gres_acc = claim(blk.gres) if blk.gres is not None else False
             blk.gsrc_acc = claim(blk.gsrc) if blk.gsrc is not None else False
         # A producer whose output gradient has ONE writer -- the depth_to_space of its space-to-depth consumer -- reads that
@@ -239,6 +262,13 @@ class TrainPlan:
         bounds = []
         for blk in reversed(self.blocks):
             seq = m.module_list[blk.i]
+            if blk.se is not None:         # the SE's backward runs first in this block's backward
+                se = blk.se
+                n = se.c * se.cr
+                se.gw1_off, se.gw2_off = off, off + L.round_up(n, 4)
+                self.param_slots[(se.i, "fc.0.weight")] = (se.gw1_off, n, (se.cr, se.c))
+                self.param_slots[(se.i, "fc.2.weight")] = (se.gw2_off, n, (se.c, se.cr))
+                off += 2 * L.round_up(n, 4)
             wshape = tuple(seq.Conv2d.weight.shape)
             n = seq.Conv2d.weight.numel()
             blk.gw_off = off
@@ -265,6 +295,10 @@ class TrainPlan:
             blk.gw = self.garena[blk.gw_off:blk.gw_off + n].view(tuple(seq.Conv2d.weight.shape))
             if not blk.is_head:
                 blk.bsums = self.garena[blk.bs_off:blk.bs_off + 2 * blk.cout + 1]
+            if blk.se is not None:
+                se, n = blk.se, blk.se.c * blk.se.cr
+                se.gw1 = self.garena[se.gw1_off:se.gw1_off + n]
+                se.gw2 = self.garena[se.gw2_off:se.gw2_off + n]
         ddp = getattr(m, "_ddp", None)
         from .parallel import GradBuckets
         self.buckets = GradBuckets(self.garena, bounds, bucket_bytes=ddp["bucket_bytes"] if ddp else (1 << 62),
@@ -427,12 +461,14 @@ class TrainPlan:
                                                     blk.res.cs if blk.res is not None else 0, ctypes.c_void_p(blk.y.ptr),
                                                     blk.y.cs, ctypes.c_void_p(blk.slope_dev), _lib.ptr(xs_out),
                                                     xs_out.shape[-1], st), "bn_act_fwd_s2d")
-                continue
-            _lib.check(lib.ryolo_bn_act_fwd(_lib.ptr(blk.z), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout,
-                                            _lib.ptr(blk.scale), _lib.ptr(blk.shift), blk.slope, int(blk.has_act),
-                                            ctypes.c_void_p(blk.res.ptr) if blk.res is not None else None,
-                                            blk.res.cs if blk.res is not None else 0, ctypes.c_void_p(blk.y.ptr), blk.y.cs,
-                                            int(blk.fuse_up), ctypes.c_void_p(blk.slope_dev), st), "bn_act_fwd")
+            else:
+                _lib.check(lib.ryolo_bn_act_fwd(_lib.ptr(blk.z), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout,
+                                                _lib.ptr(blk.scale), _lib.ptr(blk.shift), blk.slope, int(blk.has_act),
+                                                ctypes.c_void_p(blk.res.ptr) if blk.res is not None else None,
+                                                blk.res.cs if blk.res is not None else 0, ctypes.c_void_p(blk.y.ptr),
+                                                blk.y.cs, int(blk.fuse_up), ctypes.c_void_p(blk.slope_dev), st), "bn_act_fwd")
+            if blk.se is not None:
+                self._se_fwd(blk.se, st)
         if bn_counters:
             with torch.no_grad():
                 torch._foreach_add_(bn_counters, 1)
@@ -497,6 +533,22 @@ class TrainPlan:
                                                           blk.zcs, _lib.ptr(gb) if gb is not None else None, st),
                        "head_grad_nchw_to_padded")
 
+    def _se_fwd(self, se, st):
+        fc = self.model.module_list[se.i].fc
+        _lib.check(_lib.lib.ryolo_se_fwd(ctypes.c_void_p(se.x.ptr), se.x.cs, ctypes.c_void_p(se.u.ptr), se.u.cs, self.batch,
+                                         se.h, se.w, se.c, _lib.ptr(fc[0].weight), _lib.ptr(fc[2].weight), se.cr,
+                                         _lib.ptr(se.m), _lib.ptr(se.p), _lib.ptr(se.s), _lib.ptr(self.se_ws),
+                                         self.se_ws.numel(), st), "se_fwd")
+
+    def _se_bwd(self, se, st):
+        fc = self.model.module_list[se.i].fc
+        _lib.check(_lib.lib.ryolo_se_bwd(ctypes.c_void_p(se.gu.ptr), se.gu.cs, ctypes.c_void_p(se.x.ptr), se.x.cs,
+                                         ctypes.c_void_p(se.gx.ptr), se.gx.cs, int(se.gx_acc), self.batch, se.h, se.w,
+                                         se.c, _lib.ptr(fc[0].weight), _lib.ptr(fc[2].weight), se.cr, _lib.ptr(se.m),
+                                         _lib.ptr(se.p), _lib.ptr(se.s), _lib.ptr(se.ds), _lib.ptr(se.dm),
+                                         _lib.ptr(se.gw1), _lib.ptr(se.gw2), _lib.ptr(self.se_ws), self.se_ws.numel(), st),
+                   "se_bwd")
+
     def _backward_block(self, blk):
         m = self.model
         lib = _lib.lib
@@ -505,6 +557,8 @@ class TrainPlan:
         if blk.is_head:
             dz = blk.dz
         else:
+            if blk.se is not None:
+                self._se_bwd(blk.se, st)
             src_c = getattr(blk, "dy_s2d", None)
             dy_ptr, dy_cs, dy_mode = (blk.gy.ptr, blk.gy.cs, int(blk.fuse_up)) if src_c is None else \
                 (src_c.dxs.data_ptr(), src_c.xs_cs, 2)
@@ -598,8 +652,8 @@ class TrainPlan:
         self.consumed = True
         out = []
         for name in self.names:
-            parts = name.split(".")            # module_list.{i}.{Module}.{param}
-            slot = self.param_slots.get((int(parts[1]), parts[2] + "." + parts[3]))
+            parts = name.split(".")            # module_list.{i}.{Module}.{param} (SE: module_list.{i}.fc.{0|2}.weight)
+            slot = self.param_slots.get((int(parts[1]), ".".join(parts[2:])))
             out.append(out_flat[slot[0]:slot[0] + slot[1]].view(slot[2]) if slot is not None else None)
         return out
 

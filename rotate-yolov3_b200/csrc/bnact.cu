@@ -533,31 +533,45 @@ __global__ void __launch_bounds__(256) head_grad_to_padded_kernel(const float* _
 }
 
 // im2col of the 3-channel image for the first 3x3/stride-1/pad-1 conv: column index = c*9 + kh*3 + kw (the flattening
-// of nn.Conv2d.weight[co]), 27 real + zero padding to 64 channels, bf16 padded NHWC
+// of nn.Conv2d.weight[co]), 27 real + zero padding to 64 channels, bf16 padded NHWC.  A thread builds one pixel's
+// 128-byte row in shared memory; the block then stores its rows as 16-byte chunks in address order, so a warp writes
+// 4 consecutive pixels (512 contiguous bytes) per instruction instead of 16 bytes in each of 32 rows.
 __global__ void __launch_bounds__(256) im2col_first_kernel(const float* __restrict__ img, int batch, int h, int w,
                                                            __nv_bfloat16* __restrict__ dst /*cs = 64*/) {
-  const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= (size_t)batch * h * w) return;
-  const int x = (int)(pix % w);
-  const int y = (int)((pix / w) % h);
-  const int b = (int)(pix / ((size_t)w * h));
-  float v[32];
+  __shared__ uint4 rows[256 * 8];      // [pixel][chunk ^ (pixel % 8)]: the per-pixel writes hit distinct banks
+  __shared__ size_t offs[256];         // element offset of the pixel's row in dst
+  const size_t npix = (size_t)batch * h * w;
+  const size_t pix0 = (size_t)blockIdx.x * 256;
+  const int t = threadIdx.x;
+  const size_t pix = pix0 + t;
+  if (pix < npix) {
+    const int x = (int)(pix % w);
+    const int y = (int)((pix / w) % h);
+    const int b = (int)(pix / ((size_t)w * h));
+    float v[32];
 #pragma unroll
-  for (int k = 0; k < 32; k++) v[k] = 0.f;
+    for (int k = 0; k < 32; k++) v[k] = 0.f;
 #pragma unroll
-  for (int c = 0; c < 3; c++)
+    for (int c = 0; c < 3; c++)
 #pragma unroll
-    for (int dy = 0; dy < 3; dy++)
+      for (int dy = 0; dy < 3; dy++)
 #pragma unroll
-      for (int dx = 0; dx < 3; dx++) {
-        const int yy = y + dy - 1, xx = x + dx - 1;
-        if (yy >= 0 && yy < h && xx >= 0 && xx < w) v[c * 9 + dy * 3 + dx] = __ldg(img + (((size_t)b * 3 + c) * h + yy) * w + xx);
-      }
-  __nv_bfloat16* o = dst + pad_off(b, y, x, h, w, 64);
+        for (int dx = 0; dx < 3; dx++) {
+          const int yy = y + dy - 1, xx = x + dx - 1;
+          if (yy >= 0 && yy < h && xx >= 0 && xx < w) v[c * 9 + dy * 3 + dx] = __ldg(img + (((size_t)b * 3 + c) * h + yy) * w + xx);
+        }
 #pragma unroll
-  for (int q = 0; q < 4; q++) *reinterpret_cast<uint4*>(o + q * 8) = pack8(v + q * 8);
+    for (int q = 0; q < 4; q++) rows[t * 8 + (q ^ (t & 7))] = pack8(v + q * 8);
 #pragma unroll
-  for (int q = 4; q < 8; q++) *reinterpret_cast<uint4*>(o + q * 8) = make_uint4(0, 0, 0, 0);
+    for (int q = 4; q < 8; q++) rows[t * 8 + (q ^ (t & 7))] = make_uint4(0, 0, 0, 0);
+    offs[t] = pad_off(b, y, x, h, w, 64);
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    const int k = i * 256 + t, px = k >> 3, q = k & 7;
+    if (pix0 + px < npix) *reinterpret_cast<uint4*>(dst + offs[px] + q * 8) = rows[px * 8 + (q ^ (px & 7))];
+  }
 }
 
 static inline Geo mk_geo(int batch, int h, int w, int c) {

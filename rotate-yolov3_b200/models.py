@@ -21,6 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from . import graph as G
 from . import layout as L
 from .parse_config import parse_model_cfg
 
@@ -155,21 +156,6 @@ def create_modules(module_defs, arc, hyp):
     return module_list, routes
 
 
-class _View:
-    """a [B, H, W, C] activation living in a (possibly wider) padded-NHWC buffer"""
-
-    def __init__(self, buf, ch_off, c, h, w):
-        self.buf, self.ch_off, self.c, self.h, self.w = buf, ch_off, c, h, w
-
-    @property
-    def cs(self):
-        return self.buf.shape[-1] if self.buf is not None else 0
-
-    @property
-    def ptr(self):          # buf None: the activation exists only in a consumer's space-to-depth buffer
-        return self.buf.data_ptr() + 2 * self.ch_off if self.buf is not None else None
-
-
 class Darknet(nn.Module):
     def __init__(self, cfg, hyp, arc="default", precision="bf16"):
         """precision: "bf16" = throughput mode (bf16 operands / activations, fp32 accumulate); "parity" = fp32-grade
@@ -244,100 +230,36 @@ class Darknet(nn.Module):
         return w, scale, bias, slope
 
     def _build_plan(self, batch, height, width, device):
-        defs = self.module_defs
-        n = len(defs)
-        # ---- static shape walk ----
-        shape = [None] * n   # (C, H, W) of every block's output
-        c, h, w = 3, height, width
-        for i, d in enumerate(defs):
-            t = d["type"]
-            if t == "convolutional":
-                s = int(d["stride"])
-                c, h, w = int(d["filters"]), (h + s - 1) // s, (w + s - 1) // s
-            elif t == "upsample":
-                h, w = h * int(d["stride"]), w * int(d["stride"])
-            elif t == "maxpool":
-                if int(d["size"]) != 2 or int(d["stride"]) not in (1, 2):
-                    raise NotImplementedError("only the 2x2 max pools of yolov3-tiny have a kernel")
-                if int(d["stride"]) == 2:
-                    h, w = h // 2, w // 2
-            elif t == "route":
-                ls = [int(x) for x in d["layers"].split(",")]
-                ls = [l if l > 0 else i + l for l in ls]
-                c = sum(shape[l][0] for l in ls)
-                h, w = shape[ls[0]][1], shape[ls[0]][2]
-            elif t in ("shortcut", "yolo", "se"):
-                pass
-            else:
-                raise NotImplementedError("block type %r has no sm_90a kernel yet" % t)
-            shape[i] = (c, h, w)
-        # ---- concat groups: route blocks with >1 source write-share one buffer ----
-        target = {}   # materialised layer index -> (buffer, channel offset)
-        views = [None] * n
-        for i, d in enumerate(defs):
-            if d["type"] == "route":
-                ls = [int(x) for x in d["layers"].split(",")]
-                ls = [l if l > 0 else i + l for l in ls]
-                if len(ls) > 1:
-                    ctot = sum(shape[l][0] for l in ls)
-                    for l in ls:
-                        if shape[l][0] % 8:
-                            raise NotImplementedError("concat source with channels % 8 != 0")
-                    buf = L.alloc_padded(batch, shape[i][1], shape[i][2], L.round_up(ctot, 64), device)
-                    off = 0
-                    for l in ls:
-                        target[l] = (buf, off)
-                        off += shape[l][0]
-                    views[i] = _View(buf, 0, ctot, shape[i][1], shape[i][2])
-
-        def out_view(layer):
-            cc, hh, ww = shape[layer]
-            if layer in target:
-                buf, off = target[layer]
-                return _View(buf, off, cc, hh, ww)
-            return _View(L.alloc_padded(batch, hh, ww, L.round_up(cc, 32), device), 0, cc, hh, ww)
-
+        g = G.Graph(self, height, width, ("se", "maxpool"), "block type %r has no sm_90a kernel yet")
+        bufs = G.Buffers(g, lambda h, w, cs: (L.alloc_padded(batch, h, w, cs, device), None), 32)
         steps = []
         heads = []
         first_xs = None
-        i = 0
-        while i < n:
-            d = defs[i]
-            t = d["type"]
+        for t, i in g.ops:
             if t == "convolutional":
-                nxt = defs[i + 1]["type"] if i + 1 < n else None
-                cin = 3 if i == 0 else shape[i - 1][0] if defs[i - 1]["type"] != "yolo" else None
-                src = None if i == 0 else views[i - 1]
-                cout, oh, ow = shape[i]
-                k, s = int(d["size"]), int(d["stride"])
+                cv = g.convs[i]
+                src = None if i == 0 else bufs.view(i - 1)
+                cout, oh, ow, k, s = cv.cout, cv.oh, cv.ow, cv.k, cv.stride
                 wt, scale, bias, slope = self._folded(i, device)
                 if i == 0:
                     if not (k == 3 and s == 1 and wt.shape[1] == 3 and cout in (16, 32) and slope is not None):
                         raise NotImplementedError("first layer must be 3x3/1 conv, 3 -> 16|32 channels, leaky")
                     wf = (wt * scale.view(-1, 1, 1, 1)).contiguous() if scale is not None else wt.contiguous()
-                    nd = defs[1] if n > 1 else {}
-                    first_s2d = (nd.get("type") == "convolutional" and int(nd["size"]) == 3 and int(nd["stride"]) == 2
-                                 and height % 2 == 0 and width % 2 == 0 and 0 not in self.routes)
-                    v = out_view(0) if not first_s2d else _View(None, 0, cout, height, width)
+                    first_s2d = 1 in g.convs and g.convs[1].s2d and 0 not in self.routes
                     if first_s2d:
                         # layer 0 feeds only the stride-2 layer 1: write its output directly in that layer's
                         # space-to-depth layout (no [B, H+2, W+2, 32] tensor, no s2d pass over it)
                         first_xs = L.alloc_padded(batch, height // 2, width // 2, L.round_up(4 * cout, 64), device)
-                    steps.append(("first", dict(w=wf, b=bias.contiguous(), cout=cout, slope=slope, out=v,
-                                                xs=first_xs if first_s2d else None)))
-                    views[0] = v
-                    i += 1
+                        v = bufs.views[0] = G.View(None, 0, cout, height, width)
+                    else:
+                        v = bufs.out(0)[0]
+                    steps.append(("first", dict(w=wf, b=bias.contiguous(), cout=cout, slope=slope, out=v, xs=first_xs)))
                     continue
-                fuse_res = nxt == "shortcut" and i not in self.routes
-                fuse_up = nxt == "upsample" and i not in self.routes and int(defs[i + 1]["stride"]) == 2
-                # head = the linear, BN-less conv feeding a YOLO layer (or, in YOLO-less trunk graphs, any such conv)
-                is_head = nxt == "yolo" or (not self.yolo_layers and slope is None and not hasattr(self.module_list[i], "BatchNorm2d"))
-                mat = i + 1 if (fuse_res or fuse_up) else i       # the layer index whose output is materialised
+                fuse_res, fuse_up, is_head = cv.fuse_res, cv.fuse_up, cv.is_head
                 if src.c != wt.shape[1]:
                     raise RuntimeError("channel mismatch at block %d" % i)
                 x_ptr = src.ptr
-                use_s2d = s == 2 and k == 3 and src.h % 2 == 0 and src.w % 2 == 0 and src.c % 8 == 0
-                if use_s2d:
+                if cv.s2d:
                     # 3x3/stride-2 as a 2x2-tap stride-1 conv on the space-to-depth copy of the input (1.78x instead of
                     # 4x MMA work; also removes the 32->64 channel padding of the first down-sampling layer)
                     if i == 1 and first_xs is not None:
@@ -358,34 +280,26 @@ class Darknet(nn.Module):
                     out_ptr = out.data_ptr()
                     heads.append((i, out))
                 else:
-                    v = out_view(mat)
-                    desc.cout_stride = v.cs
-                    out_ptr = v.ptr
-                    views[mat] = v
-                    views[i] = v if mat == i else None
+                    out = bufs.out(cv.mat)[0]
+                    desc.cout_stride = out.cs
+                    out_ptr = out.ptr
                     if fuse_res:
-                        frm = int(defs[i + 1]["from"])
-                        res = views[i + 1 + frm if frm < 0 else frm]
-                        if res is None or (res.c, res.h, res.w) != (cout, oh, ow):
-                            raise NotImplementedError("shortcut source layout")
+                        res = bufs.view(cv.shortcut)
                         desc.res_stride = res.cs
                 pw = L.pack_weights(desc, wt, scale)
                 pb = L.padded_bias(desc, bias)
                 steps.append(("conv", dict(desc=desc, x=x_ptr, w=pw, b=pb, y=out_ptr,
-                                           r=res.ptr if res is not None else None,
-                                           keep=(src, res, views[mat] if not is_head else out))))
-                i += 2 if (fuse_res or fuse_up) else 1
-                continue
-            if t == "se":
-                src = views[i - 1]
-                if src is None or src.c != int(d["channels"]):
+                                           r=res.ptr if res is not None else None, keep=(src, res, out))))
+            elif t == "se":
+                src = bufs.view(i - 1)
+                if src is None or src.c != int(g.defs[i]["channels"]):
                     raise NotImplementedError("[se] block at %d: no materialised input / channel mismatch" % i)
                 fc = self.module_list[i].fc
                 cr = fc[0].weight.shape[0]
                 if (i - 1) in self.routes:
                     # the unscaled input is read again (the reference's *_se.cfg: the shortcut three blocks later adds it,
                     # concat routes read it): u = x * s goes to a buffer of its own
-                    v = out_view(i)
+                    v = bufs.out(i)[0]
                     steps.append(("se_fwd", dict(x=src.ptr, xcs=src.cs, u=v.ptr, ucs=v.cs, h=src.h, w=src.w, c=src.c,
                                                  w1=fc[0].weight.detach().float().contiguous(),
                                                  w2=fc[2].weight.detach().float().contiguous(), cr=cr,
@@ -395,8 +309,6 @@ class Darknet(nn.Module):
                                                  ws=torch.empty(_lib.lib.ryolo_se_workspace_bytes(batch, src.h, src.w,
                                                                                                   src.c, cr),
                                                                 dtype=torch.uint8, device=device), keep=(src, v))))
-                    views[i] = v
-                    i += 1
                     continue
                 # otherwise the scale is applied IN PLACE: nothing else reads the unscaled tensor
                 steps.append(("se", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c,
@@ -404,27 +316,13 @@ class Darknet(nn.Module):
                                          w2=fc[2].weight.detach().float().contiguous(), cr=fc[0].weight.shape[0],
                                          sums=torch.zeros(batch * src.c, dtype=torch.float32, device=device),
                                          scale=torch.zeros(batch * src.c, dtype=torch.float32, device=device), keep=src)))
-                views[i] = src
-                i += 1
-                continue
-            if t == "maxpool":
-                src = views[i - 1]
-                v = out_view(i)
-                steps.append(("maxpool", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c, stride=int(d["stride"]),
-                                              y=v.ptr, ycs=v.cs, keep=(src, v))))
-                views[i] = v
-            elif t == "route":
-                ls = [int(x) for x in d["layers"].split(",")]
-                ls = [l if l > 0 else i + l for l in ls]
-                if len(ls) == 1:
-                    views[i] = views[ls[0]]
-                # multi-source: views[i] was set above and is filled by its producers
-            elif t == "yolo":
-                views[i] = None
-            elif t in ("shortcut", "upsample"):
-                raise NotImplementedError("%s at block %d does not follow a convolution it can be fused into" % (t, i))
-            i += 1
-        rows = [self.module_list[j].na * shape[j][1] * shape[j][2] for j in self.yolo_layers]
+                bufs.views[i] = src
+            else:                                        # maxpool
+                src = bufs.view(i - 1)
+                v = bufs.out(i)[0]
+                steps.append(("maxpool", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c,
+                                              stride=int(g.defs[i]["stride"]), y=v.ptr, ycs=v.cs, keep=(src, v))))
+        rows = [self.module_list[j].na * g.shape[j][1] * g.shape[j][2] for j in self.yolo_layers]
         return dict(steps=steps, heads=heads, rows=rows, img=(height, width))
 
     # ------------------------------------------------------------------------------------------------------

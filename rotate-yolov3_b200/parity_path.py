@@ -17,7 +17,9 @@ import ctypes
 import torch
 
 from . import _lib
+from . import graph as G
 from . import layout as L
+from .train_path import check_activations
 
 NP = 3             # bf16 planes per operand: 3 = all 24 bits of an fp32 (2 = 16 bits: enough for eval, not for training BN)
 
@@ -34,26 +36,9 @@ def _terms(planes):
 NTERMS, A_CODE, W_CODE = _terms(NP)
 
 
-class _SView:
-    """a [B, H, W, C] activation in a split bf16 buffer [B, H+2, W+2, NP*P]: plane k at channel ch_off + k*P"""
-
-    def __init__(self, buf, ch_off, c, h, w):
-        self.buf, self.ch_off, self.c, self.h, self.w = buf, ch_off, c, h, w
-
-    cs = property(lambda self: self.buf.shape[-1])
-    lo = property(lambda self: self.buf.shape[-1] // NP)
-    ptr = property(lambda self: self.buf.data_ptr() + 2 * self.ch_off)
-    base = property(lambda self: self.buf.data_ptr())
-
-
-class _FView:
-    """the fp32 gradient twin of an _SView: [B, H+2, W+2, P] float32"""
-
-    def __init__(self, buf, ch_off, c, h, w):
-        self.buf, self.ch_off, self.c, self.h, self.w = buf, ch_off, c, h, w
-
-    cs = property(lambda self: self.buf.shape[-1])
-    ptr = property(lambda self: self.buf.data_ptr() + 4 * self.ch_off)
+def _lo(v):
+    """channel stride of one plane of a split bf16 view: plane k of the activation starts at channel ch_off + k * _lo(v)"""
+    return v.cs // NP
 
 
 def _split_buf(batch, h, w, plane, device):
@@ -73,142 +58,72 @@ class ParityPlan:
         self.model, self.batch, self.h, self.w, self.device, self.train = model, batch, height, width, device, train
         self.gen = 0            # forward generation (DarknetParityFn checks that backward sees the activations it saved)
         self.consumed = True
-        defs = model.module_defs
-        n = len(defs)
-        shape = [None] * n
-        c, h, w = 3, height, width
-        for i, d in enumerate(defs):
-            t = d["type"]
-            if t == "convolutional":
-                s = int(d["stride"])
-                if s == 2 and (h % 2 or w % 2):
-                    raise NotImplementedError("parity precision: stride-2 convs need even input sizes")
-                c, h, w = int(d["filters"]), (h + s - 1) // s, (w + s - 1) // s
-            elif t == "upsample":
-                h, w = h * int(d["stride"]), w * int(d["stride"])
-            elif t == "route":
-                ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
-                c = sum(shape[l][0] for l in ls)
-                h, w = shape[ls[0]][1], shape[ls[0]][2]
-            elif t == "se":
-                raise NotImplementedError("[se] blocks have no parity-precision kernel; SE graphs run in precision='bf16'")
-            elif t not in ("shortcut", "yolo"):
-                raise NotImplementedError("block type %r has no parity-precision kernel" % t)
-            shape[i] = (c, h, w)
-
-        target, views, gviews = {}, [None] * n, [None] * n
-
-        def alloc_pair(hh, ww, plane):
-            return (_split_buf(batch, hh, ww, plane, device),
-                    _f32_buf(batch, hh, ww, plane, device) if train else None)
-
-        for i, d in enumerate(defs):
-            if d["type"] == "route":
-                ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
-                if len(ls) > 1:
-                    ctot = sum(shape[l][0] for l in ls)
-                    if any(shape[l][0] % 8 for l in ls):
-                        raise NotImplementedError("concat source with channels % 8 != 0")
-                    buf, gbuf = alloc_pair(shape[i][1], shape[i][2], L.round_up(ctot, 64))
-                    off = 0
-                    for l in ls:
-                        target[l] = (buf, gbuf, off)
-                        off += shape[l][0]
-                    views[i] = _SView(buf, 0, ctot, shape[i][1], shape[i][2])
-                    gviews[i] = _FView(gbuf, 0, ctot, shape[i][1], shape[i][2]) if train else None
-
-        def out_views(layer):
-            cc, hh, ww = shape[layer]
-            if layer in target:
-                buf, gbuf, off = target[layer]
-            else:
-                buf, gbuf = alloc_pair(hh, ww, L.round_up(cc, 64))
-                off = 0
-            return _SView(buf, off, cc, hh, ww), (_FView(gbuf, off, cc, hh, ww) if train else None)
+        if any(d["type"] == "se" for d in model.module_defs):
+            raise NotImplementedError("[se] blocks have no parity-precision kernel; SE graphs run in precision='bf16'")
+        g = G.Graph(model, height, width, (), "block type %r has no parity-precision kernel")
+        if any(cv.stride == 2 and (cv.ih % 2 or cv.iw % 2) for cv in g.convs.values()):
+            raise NotImplementedError("parity precision: stride-2 convs need even input sizes")
+        # activations in split bf16 buffers [B, H+2, W+2, NP*P] (plane k at channel ch_off + k*P), gradients fp32
+        bufs = G.Buffers(g, lambda hh, ww, plane: (_split_buf(batch, hh, ww, plane, device),
+                                                   _f32_buf(batch, hh, ww, plane, device) if train else None), 64)
 
         self.col = _split_buf(batch, height, width, 64, device)     # im2col of the image: 27 real channels per plane
         blocks = []
-        i = 0
-        while i < n:
-            d = defs[i]
-            t = d["type"]
-            if t == "convolutional":
-                nxt = defs[i + 1]["type"] if i + 1 < n else None
-                seq = model.module_list[i]
-                b = _Blk()
-                b.i, b.k, b.stride = i, int(d["size"]), int(d["stride"])
-                b.has_bn, b.has_act = hasattr(seq, "BatchNorm2d"), hasattr(seq, "activation")
-                b.cout, b.oh, b.ow = shape[i]
-                b.po = L.round_up(b.cout, 64)
-                if i == 0:
-                    if not (b.k == 3 and b.stride == 1 and seq.Conv2d.weight.shape[1] == 3):
-                        raise NotImplementedError("first layer must be a 3x3 stride-1 conv on 3 channels")
-                    b.src, b.gsrc = _SView(self.col, 0, 27, height, width), None
-                    b.k_eff = 1
+        for _, i in g.ops:
+            seq = model.module_list[i]
+            b = g.convs[i]
+            b.po = L.round_up(b.cout, 64)
+            if i == 0:
+                if not (b.k == 3 and b.stride == 1 and seq.Conv2d.weight.shape[1] == 3):
+                    raise NotImplementedError("first layer must be a 3x3 stride-1 conv on 3 channels")
+                b.src, b.gsrc = G.View(self.col, 0, 27, height, width), None
+                b.k_eff = 1
+            else:
+                b.src, b.gsrc = bufs.view(i - 1), bufs.gview(i - 1)
+                b.k_eff = b.k
+            b.cin = b.src.c
+            b.s2d = i > 0 and b.stride == 2 and b.k == 3
+            if b.stride == 2 and not b.s2d:
+                raise NotImplementedError("parity precision: only 3x3 stride-2 convs")
+            if b.s2d:
+                b.p4 = L.round_up(4 * b.cin, 64)
+                b.xs = _split_buf(batch, b.src.h // 2, b.src.w // 2, b.p4, device)
+                b.dxs = _f32_buf(batch, b.src.h // 2, b.src.w // 2, b.p4, device) if train else None
+                b.k_eff = 2
+                b.gh, b.gw_ = b.src.h // 2, b.src.w // 2          # GEMM grid
+                b.cin_eff = 4 * b.cin
+            else:
+                b.gh, b.gw_ = b.src.h, b.src.w
+                b.cin_eff = b.cin
+            b.z = _f32_buf(batch, b.oh, b.ow, b.po, device)
+            if b.is_head:
+                b.out = torch.empty((batch, b.cout, b.oh, b.ow), dtype=torch.float32, device=device)
+                b.res = b.gres = None
+            else:
+                if not b.has_bn:
+                    raise NotImplementedError("conv block without BatchNorm that is not a YOLO head")
+                b.y, b.gy = bufs.out(b.mat)
+                if b.fuse_res:
+                    b.res, b.gres = bufs.view(b.shortcut), bufs.gview(b.shortcut)
                 else:
-                    b.src, b.gsrc = views[i - 1], gviews[i - 1]
-                    b.k_eff = b.k
-                b.fuse_res = nxt == "shortcut" and i not in model.routes
-                b.fuse_up = nxt == "upsample" and i not in model.routes and int(defs[i + 1]["stride"]) == 2
-                b.is_head = nxt == "yolo" or (not model.yolo_layers and not b.has_bn and not b.has_act)
-                b.mat = i + 1 if (b.fuse_res or b.fuse_up) else i
-                b.cin = b.src.c
-                b.s2d = i > 0 and b.stride == 2 and b.k == 3
-                if b.stride == 2 and not b.s2d:
-                    raise NotImplementedError("parity precision: only 3x3 stride-2 convs")
-                if b.s2d:
-                    b.p4 = L.round_up(4 * b.cin, 64)
-                    b.xs = _split_buf(batch, b.src.h // 2, b.src.w // 2, b.p4, device)
-                    b.dxs = _f32_buf(batch, b.src.h // 2, b.src.w // 2, b.p4, device) if train else None
-                    b.k_eff = 2
-                    b.gh, b.gw_ = b.src.h // 2, b.src.w // 2          # GEMM grid
-                    b.cin_eff = 4 * b.cin
-                else:
-                    b.gh, b.gw_ = b.src.h, b.src.w
-                    b.cin_eff = b.cin
-                b.z = _f32_buf(batch, b.oh, b.ow, b.po, device)
-                if b.is_head:
-                    b.out = torch.empty((batch, b.cout, b.oh, b.ow), dtype=torch.float32, device=device)
                     b.res = b.gres = None
-                else:
-                    if not b.has_bn:
-                        raise NotImplementedError("conv block without BatchNorm that is not a YOLO head")
-                    b.y, b.gy = out_views(b.mat)
-                    views[b.mat], gviews[b.mat] = b.y, b.gy
-                    if b.fuse_res:
-                        frm = int(defs[i + 1]["from"])
-                        ridx = i + 1 + frm if frm < 0 else frm
-                        b.res, b.gres = views[ridx], gviews[ridx]
-                        if (b.res.c, b.res.h, b.res.w) != (b.cout, b.oh, b.ow):
-                            raise NotImplementedError("shortcut source layout")
-                    else:
-                        b.res = b.gres = None
-                    b.sums = torch.zeros(2 * b.cout, dtype=torch.float64, device=device)
-                    b.mean, b.invstd, b.scale, b.shift = (torch.zeros(b.cout, dtype=torch.float32, device=device)
-                                                          for _ in range(4))
-                b.pw = torch.empty(_lib.lib.ryolo_px_packed_weight_bytes(b.cout, b.cin_eff, b.k_eff, NTERMS),
-                                   dtype=torch.uint8, device=device)
-                b.pw_ver = None
-                if train:
-                    b.bsums = torch.zeros(2 * b.cout + 1, dtype=torch.float64, device=device)
-                    # wgrad over all planes of dz and of the WHOLE source buffer (a slice of a concat buffer is picked
-                    # out by px_unpack_wgrad's cin_off)
-                    b.xw_buf = b.xs if b.s2d else b.src.buf
-                    b.dz_shape = (batch, b.oh + 2, b.ow + 2, NP * b.po)
-                    b.dw_shape = (b.k_eff * b.k_eff, NP * b.po, b.xw_buf.shape[-1])
-                    if i > 0:
-                        b.pwd = torch.empty(_lib.lib.ryolo_px_packed_weight_bytes(b.cin_eff, b.cout, b.k_eff, NTERMS),
-                                            dtype=torch.uint8, device=device)
-                blocks.append(b)
-                i += 2 if (b.fuse_res or b.fuse_up) else 1
-                continue
-            if t == "route":
-                ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
-                if len(ls) == 1:
-                    views[i], gviews[i] = views[ls[0]], gviews[ls[0]]
-            elif t in ("shortcut", "upsample"):
-                raise NotImplementedError("%s at block %d does not follow a convolution it can be fused into" % (t, i))
-            i += 1
+                b.sums = torch.zeros(2 * b.cout, dtype=torch.float64, device=device)
+                b.mean, b.invstd, b.scale, b.shift = (torch.zeros(b.cout, dtype=torch.float32, device=device)
+                                                      for _ in range(4))
+            b.pw = torch.empty(_lib.lib.ryolo_px_packed_weight_bytes(b.cout, b.cin_eff, b.k_eff, NTERMS),
+                               dtype=torch.uint8, device=device)
+            b.pw_ver = None
+            if train:
+                b.bsums = torch.zeros(2 * b.cout + 1, dtype=torch.float64, device=device)
+                # wgrad over all planes of dz and of the WHOLE source buffer (a slice of a concat buffer is picked
+                # out by px_unpack_wgrad's cin_off)
+                b.xw_buf = b.xs if b.s2d else b.src.buf
+                b.dz_shape = (batch, b.oh + 2, b.ow + 2, NP * b.po)
+                b.dw_shape = (b.k_eff * b.k_eff, NP * b.po, b.xw_buf.shape[-1])
+                if i > 0:
+                    b.pwd = torch.empty(_lib.lib.ryolo_px_packed_weight_bytes(b.cin_eff, b.cout, b.k_eff, NTERMS),
+                                        dtype=torch.uint8, device=device)
+            blocks.append(b)
         self.blocks = blocks
         self.heads = [b for b in blocks if b.is_head]
         if train:
@@ -230,16 +145,9 @@ class ParityPlan:
                     b.dz_shared = True
                 b.dw = self._dw_scratch[:math.prod(b.dw_shape)].view(b.dw_shape)
             written = {}
-
-            def claim(view):
-                key = view.buf.data_ptr()
-                lo, hi = view.ch_off, view.ch_off + view.c
-                covered = any(a <= lo and hi <= bb for a, bb in written.get(key, []))
-                written.setdefault(key, []).append((lo, hi))
-                return covered
             for b in reversed(blocks):
-                b.gres_acc = claim(b.gres) if b.gres is not None else False
-                b.gsrc_acc = claim(b.gsrc) if b.gsrc is not None else False
+                b.gres_acc = G.claim(written, b.gres) if b.gres is not None else False
+                b.gsrc_acc = G.claim(written, b.gsrc) if b.gsrc is not None else False
 
     # ------------------------------------------------------------------------------------------------------
     def forward(self, x):
@@ -256,12 +164,12 @@ class ParityPlan:
                 raise NotImplementedError("parity precision needs fp32 parameters")
             if b.s2d:
                 for plane in range(NP):
-                    _lib.check(lib.ryolo_space_to_depth(vp(b.src.ptr + 2 * plane * b.src.lo), b.src.cs, B, b.src.h, b.src.w,
+                    _lib.check(lib.ryolo_space_to_depth(vp(b.src.ptr + 2 * plane * _lo(b.src)), b.src.cs, B, b.src.h, b.src.w,
                                                         b.cin, vp(b.xs.data_ptr() + 2 * plane * b.p4), b.xs.shape[-1], st),
                                "s2d")
                 xbase, xcs, xoff, xlo = b.xs.data_ptr(), b.xs.shape[-1], 0, b.p4
             else:
-                xbase, xcs, xoff, xlo = b.src.base, b.src.cs, b.src.ch_off, b.src.lo
+                xbase, xcs, xoff, xlo = b.src.buf.data_ptr(), b.src.cs, b.src.ch_off, _lo(b.src)
             if b.pw_ver != w._version:
                 wt = w.detach()
                 if b.i == 0:
@@ -294,8 +202,8 @@ class ParityPlan:
                 b.slope_dev = None
             _lib.check(lib.ryolo_px_bn_act_fwd(_lib.ptr(b.z), b.po, B, b.oh, b.ow, b.cout, _lib.ptr(b.scale), _lib.ptr(b.shift),
                                                vp(b.slope_dev), vp(b.res.ptr) if b.res is not None else None,
-                                               b.res.cs if b.res is not None else 0, b.res.lo if b.res is not None else 0,
-                                               vp(b.y.ptr), b.y.cs, b.y.lo, int(b.fuse_up), NP, st), "px_bn_act_fwd")
+                                               b.res.cs if b.res is not None else 0, _lo(b.res) if b.res is not None else 0,
+                                               vp(b.y.ptr), b.y.cs, _lo(b.y), int(b.fuse_up), NP, st), "px_bn_act_fwd")
         if bn_counters:
             with torch.no_grad():
                 torch._foreach_add_(bn_counters, 1)
@@ -383,9 +291,7 @@ class DarknetParityFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         plan = ctx.plan
-        if plan.gen != ctx.gen or plan.consumed:
-            raise RuntimeError("Darknet training plan: the activations of this forward were overwritten by a later forward "
-                               "(or already consumed by a backward); one forward -> one backward per step is supported")
+        check_activations(plan, ctx.gen)
         m = plan.model
         gl = []
         for g, b, yi in zip(grads, plan.heads, m.yolo_layers):

@@ -17,6 +17,7 @@ import ctypes
 import torch
 
 from . import _lib
+from . import graph as G
 from . import layout as L
 
 _EPS = 1e-5
@@ -29,87 +30,30 @@ class _Block:
 class TrainPlan:
     def __init__(self, model, batch, height, width, device):
         self.model, self.batch, self.h, self.w, self.device = model, batch, height, width, device
-        defs = model.module_defs
-        n = len(defs)
-        shape = [None] * n
-        c, h, w = 3, height, width
-        for i, d in enumerate(defs):
-            t = d["type"]
-            if t == "convolutional":
-                s = int(d["stride"])
-                c, h, w = int(d["filters"]), (h + s - 1) // s, (w + s - 1) // s
-            elif t == "upsample":
-                h, w = h * int(d["stride"]), w * int(d["stride"])
-            elif t == "route":
-                ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
-                c = sum(shape[l][0] for l in ls)
-                h, w = shape[ls[0]][1], shape[ls[0]][2]
-            elif t not in ("shortcut", "yolo", "se"):
-                raise NotImplementedError("block type %r has no training kernel" % t)
-            shape[i] = (c, h, w)
-        self.shape = shape
-
+        g = G.Graph(model, height, width, ("se",), "block type %r has no training kernel")
+        if not model.yolo_layers and any(cv.is_head for cv in g.convs.values()):
+            # the head bookkeeping (create_grids, the gradients autograd hands back) zips the heads with yolo_layers
+            raise NotImplementedError("training needs the YOLO layers of the graph; YOLO-less trunks run in eval only")
         # activation buffers (y) and their gradient twins; concat groups share one buffer
-        target = {}
-        views = [None] * n
-        gviews = [None] * n
-
-        def alloc_pair(hh, ww, cs):
-            return L.alloc_padded(batch, hh, ww, cs, device), L.alloc_padded(batch, hh, ww, cs, device)
-
-        for i, d in enumerate(defs):
-            if d["type"] == "route":
-                ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
-                if len(ls) > 1:
-                    ctot = sum(shape[l][0] for l in ls)
-                    buf, gbuf = alloc_pair(shape[i][1], shape[i][2], L.round_up(ctot, 64))
-                    off = 0
-                    for l in ls:
-                        target[l] = (buf, gbuf, off)
-                        off += shape[l][0]
-                    views[i] = _mk_view(buf, 0, ctot, shape[i][1], shape[i][2])
-                    gviews[i] = _mk_view(gbuf, 0, ctot, shape[i][1], shape[i][2])
-
-        def out_views(layer):
-            cc, hh, ww = shape[layer]
-            if layer in target:
-                buf, gbuf, off = target[layer]
-            else:
-                buf, gbuf = alloc_pair(hh, ww, L.round_up(cc, 32))
-                off = 0
-            return _mk_view(buf, off, cc, hh, ww), _mk_view(gbuf, off, cc, hh, ww)
+        bufs = G.Buffers(g, lambda hh, ww, cs: (L.alloc_padded(batch, hh, ww, cs, device),
+                                                L.alloc_padded(batch, hh, ww, cs, device)), 32)
 
         # first layer input: im2col of the image (27 real channels in a 64-channel padded NHWC buffer)
         self.col = L.alloc_padded(batch, height, width, 64, device)
         blocks = []
-        i = 0
-        while i < n:
-            d = defs[i]
-            t = d["type"]
+        for t, i in g.ops:
             if t == "convolutional":
-                nxt = defs[i + 1]["type"] if i + 1 < n else None
-                blk = _Block()
-                blk.i = i
-                blk.k, blk.stride = int(d["size"]), int(d["stride"])
-                seq = model.module_list[i]
-                blk.has_bn = hasattr(seq, "BatchNorm2d")
-                blk.has_act = hasattr(seq, "activation")
-                blk.cout, blk.oh, blk.ow = shape[i]
+                blk = g.convs[i]
                 if i == 0:
                     if not (blk.k == 3 and blk.stride == 1):
                         raise NotImplementedError("first layer must be 3x3 stride 1")
-                    blk.src = _mk_view(self.col, 0, 27, height, width)
+                    blk.src = G.View(self.col, 0, 27, height, width)
                     blk.gsrc = None
                     blk.k_eff = 1                       # runs as a 1x1 conv over the im2col buffer
                 else:
-                    blk.src, blk.gsrc = views[i - 1], gviews[i - 1]
+                    blk.src, blk.gsrc = bufs.view(i - 1), bufs.gview(i - 1)
                     blk.k_eff = blk.k
-                blk.s2d = False
                 blk.se = None
-                blk.fuse_res = nxt == "shortcut" and i not in model.routes
-                blk.fuse_up = nxt == "upsample" and i not in model.routes and int(defs[i + 1]["stride"]) == 2
-                blk.is_head = nxt == "yolo"
-                blk.mat = i + 1 if (blk.fuse_res or blk.fuse_up) else i
                 bn_ = 256 if blk.cout > 128 else (128 if blk.cout > 64 else 64)
                 blk.cout_pad = L.round_up(blk.cout, bn_)     # GEMM tile extent (weights / dW)
                 blk.zcs = L.round_up(blk.cout, 32)           # channel stride of z / dz (TMA zero-fills up to the tile)
@@ -121,19 +65,15 @@ class TrainPlan:
                     blk.res = blk.gres = None
                 else:
                     blk.z = L.alloc_padded(batch, blk.oh, blk.ow, blk.zcs, device)     # raw conv output / dz
-                    blk.y, blk.gy = out_views(blk.mat)
-                    views[blk.mat], gviews[blk.mat] = blk.y, blk.gy
+                    blk.y, blk.gy = bufs.out(blk.mat)
                     if blk.fuse_res:
-                        frm = int(defs[i + 1]["from"])
-                        ridx = i + 1 + frm if frm < 0 else frm
-                        blk.res, blk.gres = views[ridx], gviews[ridx]
+                        blk.res, blk.gres = bufs.view(blk.shortcut), bufs.gview(blk.shortcut)
                     else:
                         blk.res = blk.gres = None
                     blk.sums = torch.zeros(2 * blk.cout + 1, dtype=torch.float32, device=device)
                     blk.mean, blk.invstd, blk.scale, blk.shift = (torch.zeros(blk.cout, dtype=torch.float32, device=device)
                                                                   for _ in range(4))
-                blk.s2d = (i > 0 and blk.stride == 2 and blk.k == 3 and blk.src.h % 2 == 0 and blk.src.w % 2 == 0
-                           and blk.src.c % 8 == 0)
+                blk.s2d = i > 0 and blk.s2d
                 if blk.s2d:
                     # 3x3/stride-2 block on the space-to-depth copy of its input: 2x2 taps, 4C channels, stride 1
                     blk.xs_cs = L.round_up(4 * blk.src.c, 64)
@@ -164,32 +104,21 @@ class TrainPlan:
                     blk.pwd = torch.empty(_lib.lib.ryolo_conv_packed_weight_bytes(ctypes.byref(blk.ddesc)), dtype=torch.uint8,
                                           device=device)
                 blocks.append(blk)
-                i += 2 if (blk.fuse_res or blk.fuse_up) else 1
-                continue
-            if t == "se":
+            else:
                 # out of place: u = x * s gets a buffer pair of its own and views[i]; views[i - 1] stays x, so that the
                 # shortcut three blocks later (`from=-4`) and concat routes read the unscaled tensor like the reference.
                 # The SE runs with the block that produced x: forward after its bn_act_fwd, backward before its bn_act_bwd.
-                x, gx = views[i - 1], gviews[i - 1]
+                x, gx = bufs.view(i - 1), bufs.gview(i - 1)
                 prod = [p_ for p_ in blocks if not p_.is_head and p_.y is x]
-                if len(prod) != 1 or prod[0].se is not None or x.c != int(d["channels"]):
+                if len(prod) != 1 or prod[0].se is not None or x.c != int(g.defs[i]["channels"]):
                     raise NotImplementedError("[se] at block %d does not follow a conv block's output" % i)
                 se = _Block()
                 se.i, se.x, se.gx, se.c, se.h, se.w = i, x, gx, x.c, x.h, x.w
                 se.cr = model.module_list[i].fc[0].weight.shape[0]
-                ub, gub = alloc_pair(x.h, x.w, L.round_up(x.c, 32))
-                se.u, se.gu = _mk_view(ub, 0, x.c, x.h, x.w), _mk_view(gub, 0, x.c, x.h, x.w)
+                se.u, se.gu = bufs.out(i)
                 se.m, se.s, se.ds, se.dm = (torch.zeros(batch * x.c, dtype=torch.float32, device=device) for _ in range(4))
                 se.p = torch.zeros(batch * se.cr, dtype=torch.float32, device=device)
-                views[i], gviews[i] = se.u, se.gu
                 prod[0].se = se
-            elif t == "route":
-                ls = [l if l > 0 else i + l for l in (int(x) for x in d["layers"].split(","))]
-                if len(ls) == 1:
-                    views[i], gviews[i] = views[ls[0]], gviews[ls[0]]
-            elif t in ("shortcut", "upsample"):
-                raise NotImplementedError("%s at block %d does not follow a convolution it can be fused into" % (t, i))
-            i += 1
         self.blocks = blocks
         ses = [b.se for b in blocks if b.se is not None]
         self.se_ws = torch.empty(max([_lib.lib.ryolo_se_workspace_bytes(batch, se.h, se.w, se.c, se.cr) for se in ses] + [0]),
@@ -206,18 +135,11 @@ class TrainPlan:
         self.zero_bias = torch.zeros(2048, dtype=torch.float32, device=device)
         # static accumulate flags for the backward writers (first writer of a gradient range overwrites)
         written = {}
-
-        def claim(view):
-            key = id(view.buf)
-            lo, hi = view.ch_off, view.ch_off + view.c
-            covered = any(a <= lo and hi <= b for a, b in written.get(key, []))
-            written.setdefault(key, []).append((lo, hi))
-            return covered
         for blk in reversed(blocks):
             if blk.se is not None:
-                blk.se.gx_acc = claim(blk.se.gx)
-            blk.gres_acc = claim(blk.gres) if blk.gres is not None else False
-            blk.gsrc_acc = claim(blk.gsrc) if blk.gsrc is not None else False
+                blk.se.gx_acc = G.claim(written, blk.se.gx)
+            blk.gres_acc = G.claim(written, blk.gres) if blk.gres is not None else False
+            blk.gsrc_acc = G.claim(written, blk.gsrc) if blk.gsrc is not None else False
         # A producer whose output gradient has ONE writer -- the depth_to_space of its space-to-depth consumer -- reads that
         # gradient straight from the consumer's dgrad output (bn_act_bwd mode 2): no d2s pass, no gy buffer traffic.
         for c_ in blocks:
@@ -670,9 +592,14 @@ def _comm_wait_ms(self):
 TrainPlan.last_comm_wait_ms = _comm_wait_ms
 
 
-def _mk_view(buf, ch_off, c, h, w):
-    from .models import _View
-    return _View(buf, ch_off, c, h, w)
+def check_activations(plan, gen):
+    """the backward of a plan's forward `gen` needs that forward's activations: they live in the plan (not per call), so a
+    second forward overwrote them, or a backward already turned z into dz in place.  Stock autograd would handle or
+    reject these cases; silently wrong gradients are not an option."""
+    if plan.gen != gen or plan.consumed:
+        raise RuntimeError("Darknet training plan: the activations of this forward were overwritten by a later forward "
+                           "or already consumed by a backward (retain_graph / two forwards before one backward are "
+                           "not supported by the fused training path)")
 
 
 class DarknetTrainFn(torch.autograd.Function):
@@ -686,12 +613,7 @@ class DarknetTrainFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         plan = ctx.plan
-        if plan.gen != ctx.gen or plan.consumed:
-            # activations live in the plan (not per call): a second forward overwrote them, or a backward already turned
-            # z into dz in place.  Stock autograd would handle or reject these cases; silently wrong gradients are not an option.
-            raise RuntimeError("Darknet training plan: the activations of this forward were overwritten by a later forward "
-                               "or already consumed by a backward (retain_graph / two forwards before one backward are "
-                               "not supported by the fused training path)")
+        check_activations(plan, ctx.gen)
         gl = []
         for g, blk, yi in zip(grads, plan.heads, plan.model.yolo_layers):
             if g is None:

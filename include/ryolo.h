@@ -390,6 +390,14 @@ int ryolo_obj_bce_fwd(const float* x, const long long* strides, int batch, int n
                       const float* tobj, float pos_weight, double* sum_out, void* stream);
 int ryolo_obj_bce_bwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
                       const float* tobj, float pos_weight, const float* scale_dev, float* grad, void* stream);
+/* Focal form of the same term (arcs containing 'F', reference model/loss.py:126-146, 284-286): per cell the BCE loss l
+ * becomes l * (1.000001 - exp(-l))^gamma (alpha = 1), the factor evaluated as (2^-20 - expm1(-l))^gamma.  Arguments and
+ * outputs as ryolo_obj_bce_*, plus gamma (finite, >= 0); gamma = 0 gives the bits of ryolo_obj_bce_*. */
+int ryolo_obj_focal_fwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
+                        const float* tobj, float pos_weight, float gamma, double* sum_out, void* stream);
+int ryolo_obj_focal_bwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
+                        const float* tobj, float pos_weight, float gamma, const float* scale_dev, float* grad,
+                        void* stream);
 /* The matched (anchor, target) rows of compute_loss (reference model/loss.py:300-338 indexes `pi[b, a, gj, gi]`): int64
  * device index vectors b / a / gj / gi and a 0/1 byte mask, `rows` entries each.  gather: out[r, k] = x[b, a, gj, gi, k]
  * (0 for masked-out or out-of-range rows); set_tobj: tobj[b, a, gj, gi] = 1 (tobj contiguous [batch, na, ny, nx]);

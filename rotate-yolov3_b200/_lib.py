@@ -85,6 +85,8 @@ SIGNATURES = {
     "ryolo_loss_rows_set_tobj": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "ryolo_obj_bce_fwd": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _i, _vp, _f, _vp, _vp]),
     "ryolo_obj_bce_bwd": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _i, _vp, _f, _vp, _vp, _vp]),
+    "ryolo_obj_focal_fwd": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _i, _vp, _f, _f, _vp, _vp]),
+    "ryolo_obj_focal_bwd": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _i, _vp, _f, _f, _vp, _vp, _vp]),
     "ryolo_conv_wgrad": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_bn_stats": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_bn_stats_finalize": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

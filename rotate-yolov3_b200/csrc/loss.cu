@@ -11,6 +11,11 @@
 //
 // BCE with logits, PyTorch's formulation (aten/native/Loss.cpp binary_cross_entropy_with_logits):
 //   lw = 1 + (pos_weight - 1) t;   l = (1 - t) x + lw (log1p(exp(-|x|)) + max(-x, 0));   dl/dx = (1 - t) + lw (sigmoid(x) - 1)
+// Focal form (arcs with 'F', reference model/loss.py:126-146: FocalLoss(BCEobj, gamma), alpha = 1), per cell:
+//   base = 1.000001f - exp(-l) = (1.000001f - 1) - expm1(-l)   (>= 9.5e-7: the expm1 form does not cancel for small l)
+//   lf = l base^gamma;   dlf/dx = dl/dx (base^gamma + gamma l exp(-l) base^(gamma - 1))
+// gamma = 0 gives the BCE bits (pow(base, 0) = 1, the second term is 0).  The same two kernels serve both forms through
+// the FOCAL template flag; the BCE instantiation compiles to the code it had before the flag existed.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -41,16 +46,25 @@ __device__ __forceinline__ size_t cell_offset(const HeadView& v, size_t cell) {
   return (size_t)(b * v.sb + a * v.sa + y * v.sy + x * v.sx);
 }
 
+// 1.000001f - 1 (= 2^-20): the reference's constant as the fp32 arithmetic of its focal factor sees it
+constexpr float FOCAL_EPS = 1.000001f - 1.f;
+// base of the focal factor; l >= 0 for targets in [0, 1], the clamp keeps base >= FOCAL_EPS when rounding says otherwise
+__device__ __forceinline__ float focal_base(float l) { return FOCAL_EPS - expm1f(-fmaxf(l, 0.f)); }
+
+// gamma is the last parameter so that the BCE instantiation (which never reads it) keeps its parameter layout
+template <bool FOCAL>
 __global__ void __launch_bounds__(256) obj_bce_fwd_kernel(const float* __restrict__ x, HeadView v, int ch,
                                                           const float* __restrict__ tobj, float pw,
-                                                          double* __restrict__ partials /*[gridDim.x]*/) {
+                                                          double* __restrict__ partials /*[gridDim.x]*/, float gamma) {
   const size_t n = (size_t)v.B * v.na * v.ny * v.nx;
   double acc = 0.0;
   for (size_t cell = (size_t)blockIdx.x * blockDim.x + threadIdx.x; cell < n; cell += (size_t)gridDim.x * blockDim.x) {
     const float xv = x[cell_offset(v, cell) + (size_t)ch * v.sc];
     const float t = tobj[cell];
     const float lw = 1.f + (pw - 1.f) * t;
-    acc += (double)((1.f - t) * xv + lw * (log1pf(expf(-fabsf(xv))) + fmaxf(-xv, 0.f)));
+    float l = (1.f - t) * xv + lw * (log1pf(expf(-fabsf(xv))) + fmaxf(-xv, 0.f));
+    if (FOCAL) l *= powf(focal_base(l), gamma);
+    acc += (double)l;
   }
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   __shared__ double part[8];
@@ -90,10 +104,12 @@ __global__ void __launch_bounds__(256) ordered_rows_add_kernel(const float* __re
   }
 }
 
-// g[cell, k] = k == ch ? scale * dl/dx : 0, for every channel k (g has the strides of the head tensor)
+// g[cell, k] = k == ch ? scale * dl/dx : 0, for every channel k (g has the strides of the head tensor); FOCAL: dlf/dx
+template <bool FOCAL>
 __global__ void __launch_bounds__(256) obj_bce_bwd_kernel(const float* __restrict__ x, HeadView v, int ch,
                                                           const float* __restrict__ tobj, float pw,
-                                                          const float* __restrict__ scale_dev, float* __restrict__ g) {
+                                                          const float* __restrict__ scale_dev, float* __restrict__ g,
+                                                          float gamma) {
   const size_t n = (size_t)v.B * v.na * v.ny * v.nx;
   const float scale = __ldg(scale_dev);
   for (size_t cell = (size_t)blockIdx.x * blockDim.x + threadIdx.x; cell < n; cell += (size_t)gridDim.x * blockDim.x) {
@@ -102,7 +118,16 @@ __global__ void __launch_bounds__(256) obj_bce_bwd_kernel(const float* __restric
     const float t = tobj[cell];
     const float lw = 1.f + (pw - 1.f) * t;
     const float sg = 1.f / (1.f + expf(-xv));
-    const float d = scale * ((1.f - t) + lw * (sg - 1.f));
+    float d;
+    if (FOCAL) {
+      const float l = (1.f - t) * xv + lw * (log1pf(expf(-fabsf(xv))) + fmaxf(-xv, 0.f));
+      const float base = focal_base(l);
+      const float pg = powf(base, gamma);
+      const float fac = pg + gamma * l * expf(-l) * (pg / base);     // base^(gamma - 1) = base^gamma / base
+      d = scale * (((1.f - t) + lw * (sg - 1.f)) * fac);
+    } else {
+      d = scale * ((1.f - t) + lw * (sg - 1.f));
+    }
     for (int k = 0; k < v.no; k++) g[off + (size_t)k * v.sc] = k == ch ? d : 0.f;
   }
 }
@@ -307,8 +332,9 @@ static inline bool mk_view(const long long* strides, int batch, int na, int ny, 
   return true;
 }
 
-extern "C" int ryolo_obj_bce_fwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
-                                 const float* tobj, float pos_weight, double* sum_out, void* stream_) {
+template <bool FOCAL>
+static int obj_fwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
+                   const float* tobj, float pos_weight, float gamma, double* sum_out, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   HeadView v;
   RYOLO_ARG_CHECK(x && tobj && sum_out && mk_view(strides, batch, na, ny, nx, no, &v) && ch >= 0 && ch < no);
@@ -316,22 +342,46 @@ extern "C" int ryolo_obj_bce_fwd(const float* x, const long long* strides, int b
   const int grid = loss_grid(n);
   double* partials = static_cast<double*>(stream_scratch(stream, SCRATCH_LOSS, (size_t)grid * sizeof(double)));
   if (!partials) return RYOLO_E_CUDA;
-  obj_bce_fwd_kernel<<<grid, 256, 0, stream>>>(x, v, ch, tobj, pos_weight, partials);
+  obj_bce_fwd_kernel<FOCAL><<<grid, 256, 0, stream>>>(x, v, ch, tobj, pos_weight, partials, gamma);
   RYOLO_LAUNCH_CHECK();
   ordered_sum_add_kernel<<<1, 32, 0, stream>>>(partials, grid, sum_out);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }
 
-extern "C" int ryolo_obj_bce_bwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
-                                 const float* tobj, float pos_weight, const float* scale_dev, float* grad, void* stream_) {
+template <bool FOCAL>
+static int obj_bwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
+                   const float* tobj, float pos_weight, float gamma, const float* scale_dev, float* grad, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   HeadView v;
   RYOLO_ARG_CHECK(x && tobj && scale_dev && grad && mk_view(strides, batch, na, ny, nx, no, &v) && ch >= 0 && ch < no);
   const size_t n = (size_t)batch * na * ny * nx;
-  obj_bce_bwd_kernel<<<loss_grid(n), 256, 0, stream>>>(x, v, ch, tobj, pos_weight, scale_dev, grad);
+  obj_bce_bwd_kernel<FOCAL><<<loss_grid(n), 256, 0, stream>>>(x, v, ch, tobj, pos_weight, scale_dev, grad, gamma);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
+}
+
+extern "C" int ryolo_obj_bce_fwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
+                                 const float* tobj, float pos_weight, double* sum_out, void* stream_) {
+  return obj_fwd<false>(x, strides, batch, na, ny, nx, no, ch, tobj, pos_weight, 0.f, sum_out, stream_);
+}
+
+extern "C" int ryolo_obj_bce_bwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no, int ch,
+                                 const float* tobj, float pos_weight, const float* scale_dev, float* grad, void* stream_) {
+  return obj_bwd<false>(x, strides, batch, na, ny, nx, no, ch, tobj, pos_weight, 0.f, scale_dev, grad, stream_);
+}
+
+extern "C" int ryolo_obj_focal_fwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no,
+                                   int ch, const float* tobj, float pos_weight, float gamma, double* sum_out, void* stream_) {
+  RYOLO_ARG_CHECK(gamma >= 0.f && gamma < INFINITY);
+  return obj_fwd<true>(x, strides, batch, na, ny, nx, no, ch, tobj, pos_weight, gamma, sum_out, stream_);
+}
+
+extern "C" int ryolo_obj_focal_bwd(const float* x, const long long* strides, int batch, int na, int ny, int nx, int no,
+                                   int ch, const float* tobj, float pos_weight, float gamma, const float* scale_dev,
+                                   float* grad, void* stream_) {
+  RYOLO_ARG_CHECK(gamma >= 0.f && gamma < INFINITY);
+  return obj_bwd<true>(x, strides, batch, na, ny, nx, no, ch, tobj, pos_weight, gamma, scale_dev, grad, stream_);
 }
 
 extern "C" int ryolo_head_grad_nchw_to_padded(const float* g, int batch, int c, int ny, int nx, void* dst, int dst_cstride,

@@ -2,9 +2,11 @@
 utils/utils.py:346-361), restated device-agnostically (the reference hard-codes ``.cuda()`` at loss.py:197).  This is the
 CONSUMER of the training hot path (SURVEY.md 8a row a6): tiny tensors, plain PyTorch on whatever device ``p`` lives on.
 
-Covered: the shipped configuration -- arc 'default' (separate obj / cls BCE), NoSampler, reject=True target assignment
-with the orphan-GT rescue.  Regression loss = SmoothL1(sigmoid xy) + 2 SmoothL1(theta) + giou * mean(1 - wh_iou): there
-is no rotated IoU in the reference loss (SURVEY.md D1)."""
+Covered: the arcs containing 'default' (separate obj / cls BCE) -- 'default', and with 'F' ('Fdefault', 'Fdefaultpw')
+the focal form of model/loss.py:126-146, 284-286 with gamma = hyp['fl_gamma'] -- NoSampler, reject=True target
+assignment with the orphan-GT rescue.  Regression loss = SmoothL1(sigmoid xy) + 2 SmoothL1(theta) + giou * mean(1 -
+wh_iou): there is no rotated IoU in the reference loss (SURVEY.md D1).  The unified arcs ('uBCE', 'uFBCE', 'uCE',
+'uFCE') raise NotImplementedError."""
 import ctypes
 import math
 
@@ -85,9 +87,31 @@ def _targets_masked(model, targets, hyp):
     return out
 
 
+# 1.000001 - 1 as the reference's fp32 focal factor sees it (the scalar rounds to the float 1 + 2^-20)
+_FOCAL_EPS = 2.0 ** -20
+
+
+def _focal_gamma(model):
+    """the focal exponent of the model's arc: None for the plain arcs, hyp['fl_gamma'] for arcs with 'F' (a missing key
+    raises KeyError like model/loss.py:285); arcs without 'default' are not restated"""
+    arc = model.arc
+    if "default" not in arc:
+        raise NotImplementedError("arc %r is not supported: compute_loss restates the arcs containing 'default' "
+                                  "('default', 'Fdefault', 'Fdefaultpw'), not the unified 'uBCE' / 'uCE' forms" % (arc,))
+    return float(model.hyp["fl_gamma"]) if "F" in arc else None
+
+
+def _focal(l, gamma):
+    """FocalLoss of model/loss.py:126-146 on the element losses l (alpha = 1): l * (1.000001 - exp(-l))^gamma, the base
+    written as 2^-20 - expm1(-l) so that it does not cancel for small l; gamma None = the plain loss"""
+    if gamma is None:
+        return l
+    return l * (_FOCAL_EPS - torch.expm1(-l.clamp(min=0.0))) ** gamma
+
+
 def compute_loss(p, targets, model, hyp):
     """p: list of [B, na, ny, nx, nc+6] raw head tensors (training-mode output of Darknet); returns (loss[1],
-    detached (lobj, lcls, lreg, loss)) like model/loss.py:266-367 for arc 'default'.
+    detached (lobj, lcls, lreg, loss)) like model/loss.py:266-367 for the arcs containing 'default' (with 'F': focal).
 
     The reference selects the matched (anchor, target) rows with data-dependent indexing (build_targets, loss.py:161-258:
     ~350 device-to-host reads per step); this evaluates the same sums over ALL (anchor, target) rows weighted by the 0/1
@@ -104,18 +128,28 @@ def _compute_loss_no_targets(p, model):
     """no ground truth in the batch: only the objectness term over the whole maps remains (loss.py:346-348)"""
     dev = p[0].device
     h = model.hyp
-    BCEobj = nn.BCEWithLogitsLoss(pos_weight=torch.full((1,), float(h["obj_pw"]), device=dev))
+    gamma = _focal_gamma(model)
+    obj_pw = torch.full((1,), float(h["obj_pw"]), device=dev)
     lobj = torch.zeros(1, device=dev)
     for pi in p:
-        lobj = lobj + BCEobj(pi[..., 5], torch.zeros_like(pi[..., 0]))
+        lobj = lobj + _obj_term(pi, torch.zeros_like(pi[..., 0]), obj_pw, gamma)
     lobj = lobj * h["obj"]
     zero = torch.zeros(1, device=dev)
     return lobj + zero, torch.cat((lobj, zero, zero, lobj)).detach()
 
 
-def _sparse_terms(ps, r, model, h, cls_pw):
+def _obj_term(pi, tobj, obj_pw, gamma):
+    """mean objectness BCE (focal when gamma is not None) over every cell of one head (model/loss.py:348)"""
+    if gamma is None:
+        return nn.functional.binary_cross_entropy_with_logits(pi[..., 5], tobj, pos_weight=obj_pw)
+    e = nn.functional.binary_cross_entropy_with_logits(pi[..., 5], tobj, pos_weight=obj_pw, reduction="none")
+    return _focal(e, gamma).mean()
+
+
+def _sparse_terms(ps, r, model, h, cls_pw, gamma=None):
     """regression (+ class) loss of one head over ALL (anchor, target) rows weighted by the 0/1 assignment mask; ps =
-    pi[b, a, gj, gi] with the unselected rows already zeroed.  Returns (lreg_i, lcls_i), unweighted."""
+    pi[b, a, gj, gi] with the unselected rows already zeroed.  Returns (lreg_i, lcls_i), unweighted.  gamma: the focal
+    exponent of the SmoothL1 and class BCE terms (model/loss.py:286; the wh-IoU term is never focal), None = plain."""
     av, tbox = r["av"], r["tbox"]
     mf = r["mask"].to(ps.dtype)
     cnt = mf.sum().clamp(min=1.0)              # an empty selection contributes 0 like the reference's `if nb:`
@@ -123,14 +157,15 @@ def _sparse_terms(ps, r, model, h, cls_pw):
     pwh = torch.exp(ps[:, 2:4]).clamp(max=1e3) * av[:, :-1]
     pa = torch.atan(ps[:, 4]) + av[:, -1]
     liou = ((1.0 - wh_iou(tbox[:, 2:4], pwh)) * mf).sum() / cnt
-    sm_xy = (nn.functional.smooth_l1_loss(pxy, tbox[:, 0:2], reduction="none") * mf[:, None]).sum() / (2.0 * cnt)
-    sm_a = (nn.functional.smooth_l1_loss(pa, tbox[:, 4], reduction="none") * mf).sum() / cnt
+    sm_xy = (_focal(nn.functional.smooth_l1_loss(pxy, tbox[:, 0:2], reduction="none"), gamma)
+             * mf[:, None]).sum() / (2.0 * cnt)
+    sm_a = (_focal(nn.functional.smooth_l1_loss(pa, tbox[:, 4], reduction="none"), gamma) * mf).sum() / cnt
     lreg = sm_xy + 2 * sm_a + liou * h["giou"]
     lcls = None
     if model.nc > 1:
         t = torch.zeros_like(ps[:, 6:])
         t[torch.arange(len(r["b"]), device=ps.device), r["tcls"]] = 1.0
-        e = nn.functional.binary_cross_entropy_with_logits(ps[:, 6:], t, pos_weight=cls_pw, reduction="none")
+        e = _focal(nn.functional.binary_cross_entropy_with_logits(ps[:, 6:], t, pos_weight=cls_pw, reduction="none"), gamma)
         lcls = (e * mf[:, None]).sum() / (cnt * e.shape[1])
     return lreg, lcls
 
@@ -145,25 +180,24 @@ def _tobj_of(pi, r):
 def _compute_loss_masked(p, targets, model, hyp):
     dev = p[0].device
     h = model.hyp
-    if "default" not in model.arc or "F" in model.arc:
-        raise NotImplementedError("only arc='default' is restated (the configuration the reference ships)")
+    gamma = _focal_gamma(model)
     lcls = torch.zeros(1, device=dev)
     lobj = torch.zeros(1, device=dev)
     lreg = torch.zeros(1, device=dev)
     rows = _targets_masked(model, targets, hyp)
     # torch.full, not torch.tensor([...], device=...): the latter is a (synchronising) pageable host-to-device copy
-    BCEobj = nn.BCEWithLogitsLoss(pos_weight=torch.full((1,), float(h["obj_pw"]), device=dev))
+    obj_pw = torch.full((1,), float(h["obj_pw"]), device=dev)
     cls_pw = torch.full((1,), float(h["cls_pw"]), device=dev)
     for pi, r in zip(p, rows):
         tobj = _tobj_of(pi, r)
         ps = pi[r["b"], r["a"], r["gj"], r["gi"]]
         # rows the reference never touches must not poison the sums: exp(inf) * 0 would be NaN in forward AND backward
         ps = torch.where(r["mask"][:, None], ps, torch.zeros_like(ps))
-        lreg_i, lcls_i = _sparse_terms(ps, r, model, h, cls_pw)
+        lreg_i, lcls_i = _sparse_terms(ps, r, model, h, cls_pw, gamma)
         lreg = lreg + lreg_i
         if lcls_i is not None:
             lcls = lcls + lcls_i
-        lobj = lobj + BCEobj(pi[..., 5], tobj)
+        lobj = lobj + _obj_term(pi, tobj, obj_pw, gamma)
     lobj = lobj * h["obj"]
     lcls = lcls * h["cls"]
     lreg = lreg * h["reg"]
@@ -225,7 +259,7 @@ def _targets_masked_stacked(model, targets, hyp):
                 gi=rep(gij[..., 0:1]).reshape(nl, R).contiguous(), mask=mask, tbox=tbox, av=av, tcls=tcls, nl=nl, R=R)
 
 
-def _sparse_terms_stacked(ps, r, model, h, cls_pw):
+def _sparse_terms_stacked(ps, r, model, h, cls_pw, gamma=None):
     """_sparse_terms over all layers at once: ps [nl, R, no]; returns (lreg, lcls) summed over the layers, unweighted"""
     av, tbox = r["av"], r["tbox"]
     mf = r["mask"].to(ps.dtype)                                                   # [nl, R]
@@ -237,14 +271,15 @@ def _sparse_terms_stacked(ps, r, model, h, cls_pw):
     inter = torch.min(w1, w2) * torch.min(h1, h2)
     iou = inter / ((w1 * h1 + 1e-16) + w2 * h2 - inter)
     liou = ((1.0 - iou) * mf).sum(1) / cnt
-    sm_xy = (nn.functional.smooth_l1_loss(pxy, tbox[..., 0:2], reduction="none") * mf[..., None]).sum((1, 2)) / (2.0 * cnt)
-    sm_a = (nn.functional.smooth_l1_loss(pa, tbox[..., 4], reduction="none") * mf).sum(1) / cnt
+    sm_xy = (_focal(nn.functional.smooth_l1_loss(pxy, tbox[..., 0:2], reduction="none"), gamma)
+             * mf[..., None]).sum((1, 2)) / (2.0 * cnt)
+    sm_a = (_focal(nn.functional.smooth_l1_loss(pa, tbox[..., 4], reduction="none"), gamma) * mf).sum(1) / cnt
     lreg = (sm_xy + 2 * sm_a + liou * h["giou"]).sum()
     lcls = None
     if model.nc > 1:
         nc = ps.shape[-1] - 6
         t = (torch.arange(nc, device=ps.device).view(1, 1, nc) == r["tcls"].view(1, -1, 1)).to(ps.dtype).expand(ps.shape[0], -1, -1)
-        e = nn.functional.binary_cross_entropy_with_logits(ps[..., 6:], t, pos_weight=cls_pw, reduction="none")
+        e = _focal(nn.functional.binary_cross_entropy_with_logits(ps[..., 6:], t, pos_weight=cls_pw, reduction="none"), gamma)
         lcls = ((e * mf[..., None]).sum((1, 2)) / (cnt * nc)).sum()
     return lreg, lcls
 
@@ -260,7 +295,9 @@ class _FusedLoss(torch.autograd.Function):
               over all 35 M cells is ONE kernel per head reading the head tensor through its strides (so the permuted
               view of the NCHW buffer the head convolution wrote is consumed in place).
     backward: ONE kernel per head writes the whole cotangent (objectness channel, zeros elsewhere) with the strides of
-              the input, the row gradients are scattered on top.  Nothing reads a device value on the host."""
+              the input, the row gradients are scattered on top.  Nothing reads a device value on the host.
+    gamma (focal arcs): the objectness kernels are the ryolo_obj_focal_* instantiations, the matched-row terms take
+    the focal factor through _sparse_terms_stacked; None runs exactly the plain BCE path."""
 
     @staticmethod
     def _row_ptrs(r, m8, i):
@@ -271,7 +308,7 @@ class _FusedLoss(torch.autograd.Function):
                 ctypes.c_void_p(m8.data_ptr() + i * r["R"]), int(r["R"]))
 
     @staticmethod
-    def forward(ctx, model, r, h, *p):
+    def forward(ctx, model, r, h, gamma, *p):
         from . import _lib
         lib = _lib.lib
         dev = p[0].device
@@ -295,15 +332,21 @@ class _FusedLoss(torch.autograd.Function):
                     _lib.check(lib.ryolo_loss_rows_gather(_lib.ptr(pi), strides, B, na, ny, nx, no, *ra,
                                                           ctypes.c_void_p(ps_all[i].data_ptr()), st), "loss_rows_gather")
                     _lib.check(lib.ryolo_loss_rows_set_tobj(_lib.ptr(tobj), B, na, ny, nx, *ra, st), "loss_rows_set_tobj")
-                _lib.check(lib.ryolo_obj_bce_fwd(_lib.ptr(pi), strides, B, na, ny, nx, no, 5, _lib.ptr(tobj),
-                                                 float(h["obj_pw"]), ctypes.c_void_p(sums[i:].data_ptr()), st), "obj_bce_fwd")
+                if gamma is None:
+                    _lib.check(lib.ryolo_obj_bce_fwd(_lib.ptr(pi), strides, B, na, ny, nx, no, 5, _lib.ptr(tobj),
+                                                     float(h["obj_pw"]), ctypes.c_void_p(sums[i:].data_ptr()), st),
+                               "obj_bce_fwd")
+                else:
+                    _lib.check(lib.ryolo_obj_focal_fwd(_lib.ptr(pi), strides, B, na, ny, nx, no, 5, _lib.ptr(tobj),
+                                                       float(h["obj_pw"]), gamma, ctypes.c_void_p(sums[i:].data_ptr()),
+                                                       st), "obj_focal_fwd")
                 tobjs.append(tobj)
                 counts.append(float(B * na * ny * nx))
             if r is not None:
                 cls_pw = torch.full((1,), float(h["cls_pw"]), device=dev)
                 with torch.enable_grad():
                     ps_all.requires_grad_()
-                    lreg_s, lcls_s = _sparse_terms_stacked(ps_all, r, model, h, cls_pw)
+                    lreg_s, lcls_s = _sparse_terms_stacked(ps_all, r, model, h, cls_pw, gamma)
                     sparse = lreg_s * h["reg"]
                     lreg = lreg + lreg_s.detach()
                     if lcls_s is not None:
@@ -318,7 +361,7 @@ class _FusedLoss(torch.autograd.Function):
         lcls = lcls * h["cls"]
         loss = lobj + lcls + lreg
         ctx.rows, ctx.tobjs, ctx.row_grads, ctx.counts, ctx.keep = r, tobjs, row_grads, counts, m8
-        ctx.obj_w, ctx.obj_pw = float(h["obj"]), float(h["obj_pw"])
+        ctx.obj_w, ctx.obj_pw, ctx.gamma = float(h["obj"]), float(h["obj_pw"]), gamma
         ctx.save_for_backward(*p)
         items = torch.cat((lobj, lcls, lreg, loss)).detach()
         ctx.mark_non_differentiable(items)
@@ -341,23 +384,27 @@ class _FusedLoss(torch.autograd.Function):
                 g = torch.empty_strided(pi.shape, pi.stride(), dtype=pi.dtype, device=dev)   # every element is written
                 scale = gloss * (ctx.obj_w / ctx.counts[i])
                 strides = (ctypes.c_longlong * 5)(*pi.stride())
-                _lib.check(lib.ryolo_obj_bce_bwd(_lib.ptr(pi), strides, B, na, ny, nx, no, 5, _lib.ptr(ctx.tobjs[i]),
-                                                 ctx.obj_pw, _lib.ptr(scale), _lib.ptr(g), st), "obj_bce_bwd")
+                if ctx.gamma is None:
+                    _lib.check(lib.ryolo_obj_bce_bwd(_lib.ptr(pi), strides, B, na, ny, nx, no, 5, _lib.ptr(ctx.tobjs[i]),
+                                                     ctx.obj_pw, _lib.ptr(scale), _lib.ptr(g), st), "obj_bce_bwd")
+                else:
+                    _lib.check(lib.ryolo_obj_focal_bwd(_lib.ptr(pi), strides, B, na, ny, nx, no, 5, _lib.ptr(ctx.tobjs[i]),
+                                                       ctx.obj_pw, ctx.gamma, _lib.ptr(scale), _lib.ptr(g), st),
+                               "obj_focal_bwd")
                 if ctx.rows is not None:
                     ra = _FusedLoss._row_ptrs(ctx.rows, ctx.keep, i)
                     _lib.check(lib.ryolo_loss_rows_scatter_add(_lib.ptr(g), strides, B, na, ny, nx, no, *ra,
                                                                ctypes.c_void_p(ctx.row_grads[i].data_ptr()), _lib.ptr(gloss),
                                                                st), "loss_rows_scatter_add")
                 grads.append(g)
-        return (None, None, None) + tuple(grads)
+        return (None, None, None, None) + tuple(grads)
 
 
 def _compute_loss_fused(p, targets, model, hyp):
     h = model.hyp
-    if "default" not in model.arc or "F" in model.arc:
-        raise NotImplementedError("only arc='default' is restated (the configuration the reference ships)")
+    gamma = _focal_gamma(model)
     nas = {int(pi.shape[1]) for pi in p}
     if len(nas) != 1 or len({int(pi.shape[-1]) for pi in p}) != 1:      # ragged anchor counts: the per-layer framework form
         return _compute_loss_masked(p, targets, model, hyp) if len(targets) else _compute_loss_no_targets(p, model)
     rows = _targets_masked_stacked(model, targets, hyp) if len(targets) else None
-    return _FusedLoss.apply(model, rows, h, *p)
+    return _FusedLoss.apply(model, rows, h, gamma, *p)

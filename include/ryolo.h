@@ -98,6 +98,26 @@ int ryolo_detect_select(const float* io, int batch, int p, int nc, float conf_th
                         float* dets_out, int cap, int32_t* n_out, void* workspace, size_t workspace_bytes,
                         void* stream);
 
+/* Class-aware forms, for configs with any number of classes (reference: the per-class loop of non_max_suppression,
+ * utils/nms/nms.py:47-56).
+ * ryolo_detect_select_classes: the same selection as ryolo_detect_select, written as 8 columns dets_out
+ * [batch, cap, 8] = (x, y, w, h, theta, conf, class_conf, class): class_conf, class = max / first argmax of the class
+ * scores.  Workspace: ryolo_detect_select_workspace_bytes.  nc must be <= 2^24.
+ * ryolo_rnms_batched_classes: one NMS per class within each segment, in one set of launches.  dets8 [segments, cap, 8]
+ * with the score in column 5 and the class id in column 7; all n_dev[s] rows of segment s enter.  Each segment is sorted
+ * by (class asc, score desc, row asc) and the suppression mask only holds same-class pairs, so its memory is that of
+ * ryolo_rnms_batched at the same cap, whatever the number of classes.  keep_out / num_keep as ryolo_rnms_batched:
+ * kept row indices within the segment, ascending; per class, the kept list is bit-identical to ryolo_rnms on that
+ * class's rows.  Class ids must be integers in [0, 2^24) and scores > 0: a row that breaks this (checked on the
+ * device) is never suppressed and suppresses nothing. */
+int ryolo_detect_select_classes(const float* io, int batch, int p, int nc, float conf_thres, float min_wh, int limit,
+                                float* dets_out, int cap, int32_t* n_out, void* workspace, size_t workspace_bytes,
+                                void* stream);
+size_t ryolo_rnms_batched_classes_workspace_bytes(int segments, int cap);
+int ryolo_rnms_batched_classes(const float* dets8, int segments, int cap, const int32_t* n_dev, float thr,
+                               int64_t* keep_out, int32_t* num_keep, void* workspace, size_t workspace_bytes,
+                               void* stream);
+
 /* Introspection of the last ryolo_rnms_full_mask call that used `workspace` (valid until the workspace is
  * reused): device pointers to the score-sorted boxes [n,6], the sort permutation order[n]
  * (int32, sorted position -> original index) and the suppression mask [n, ceil(n/64)] uint64 in the

@@ -59,6 +59,9 @@ SIGNATURES = {
     "ryolo_rnms_batched": (_i, [_vp, _i, _i, _vp, _i, _f, _vp, _vp, _vp, _sz, _vp]),
     "ryolo_detect_select_workspace_bytes": (_sz, [_i, _i]),
     "ryolo_detect_select": (_i, [_vp, _i, _i, _i, _f, _f, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "ryolo_detect_select_classes": (_i, [_vp, _i, _i, _i, _f, _f, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "ryolo_rnms_batched_classes_workspace_bytes": (_sz, [_i, _i]),
+    "ryolo_rnms_batched_classes": (_i, [_vp, _i, _i, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
     "ryolo_rnms_debug_views": (_i, [_vp, _i, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp)]),
     "ryolo_riou_paired": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_riou_pairwise": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _vp, _vp]),

@@ -15,6 +15,8 @@
 #include <cub/device/device_segmented_radix_sort.cuh>
 #include <cub/util_type.cuh>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "rbox_exact.cuh"
 
@@ -35,7 +37,8 @@ enum {
   F_HW = 22, F_HH = 23
 };
 
-// Segments: S independent NMS problems (one per (image, class)) in ONE set of launches.  Segment s owns rows
+// Segments: S independent NMS problems (one per image; the CLASSES kernels run one NMS per class inside it) in ONE set
+// of launches.  Segment s owns rows
 // [s*cap, s*cap + count_s) of dets; count_s comes from device memory (the candidate selection never visits the host) or
 // from the host (the single-problem r_nms entry point); at most `limit` boxes (the best-scored) enter the NMS.
 struct SegArgs {
@@ -70,15 +73,51 @@ __global__ void rnms_keys_kernel(const float* __restrict__ dets, SegArgs sa, flo
   }
 }
 
-// One thread per score-sorted box: gather, pinned corner arithmetic, filter data.
+// Class-aware form (CLASSES): dets rows are (x, y, w, h, theta, score, class_conf, class).  A segment is one image with
+// its boxes of every class, sorted by (class asc, score desc, row asc); the mask only sets bits of same-class pairs, so
+// the greedy scan over that order is exactly one NMS per class.  A box's "group" encodes its class so that it is
+// non-increasing along the sort order: 2^24 - class for a class id that is an integer in [0, 2^24) with a score > 0,
+// else 0 -- such a box sorts last and neither suppresses nor is suppressed.
+constexpr float kClassLimit = 16777216.f;   // 2^24: class ids below it are exact in fp32
+__device__ __forceinline__ int class_group(float score, float cls) {
+  return (score > 0.f && cls >= 0.f && cls < kClassLimit && cls == floorf(cls)) ? (int)(kClassLimit - cls) : 0;
+}
+
+__global__ void rnms_class_keys_kernel(const float* __restrict__ dets, SegArgs sa, u64* __restrict__ keys,
+                                       int* __restrict__ vals, int* __restrict__ seg_begin, int* __restrict__ seg_end) {
+  const int seg = blockIdx.y;
+  const int n = seg_count(sa, seg);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) {
+    seg_begin[seg] = seg * sa.cap;
+    seg_end[seg] = seg * sa.cap + n;
+  }
+  if (i < n) {
+    const float* d = dets + ((size_t)seg * sa.cap + i) * 8;
+    const float score = d[5];
+    const int grp = class_group(score, d[7]);
+    keys[(size_t)seg * sa.cap + i] = grp ? ((u64)grp << 32) | __float_as_uint(score) : 0ull;
+    vals[(size_t)seg * sa.cap + i] = i;
+  }
+}
+
+// One thread per score-sorted box: gather, pinned corner arithmetic, filter data.  CLASSES: 8-column rows, and the
+// box's group goes to grp[seg * n_pad + i] (0 for padding).
+template <bool CLASSES>
 __global__ void rnms_prep_kernel(const float* __restrict__ dets, const int* __restrict__ order_in, SegArgs sa,
                                  float* __restrict__ sorted_boxes, int* __restrict__ order_out,
-                                 float* __restrict__ geom, unsigned char* __restrict__ keep_flag) {
+                                 float* __restrict__ geom, unsigned char* __restrict__ keep_flag, int* __restrict__ grp) {
+  constexpr int DW = CLASSES ? 8 : 6;
   const int seg = blockIdx.y;
   const int n = seg_n(sa, seg), n_pad = sa.n_pad;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pad) return;
-  dets += (size_t)seg * sa.cap * 6;
+  if constexpr (CLASSES) {
+    const int src = i < n ? order_in[(size_t)seg * sa.cap + i] : 0;
+    const float* d = dets + ((size_t)seg * sa.cap + src) * 8;
+    grp[(size_t)seg * n_pad + i] = i < n ? class_group(d[5], d[7]) : 0;
+  }
+  dets += (size_t)seg * sa.cap * DW;
   order_in += (size_t)seg * sa.cap;
   sorted_boxes += (size_t)seg * sa.cap * 6;
   order_out += (size_t)seg * sa.cap;
@@ -94,7 +133,7 @@ __global__ void rnms_prep_kernel(const float* __restrict__ dets, const int* __re
     float b[6];
 #pragma unroll
     for (int k = 0; k < 6; k++) {
-      b[k] = dets[(size_t)src * 6 + k];
+      b[k] = dets[(size_t)src * DW + k];
       sorted_boxes[(size_t)i * 6 + k] = b[k];
     }
     const float cx = b[0], cy = b[1], w = b[2], h = b[3], ang = b[4];
@@ -152,6 +191,10 @@ struct MaskSmem {
   unsigned short queue2[TB * TB];   // stage A2 survivors (separating axes) = exact-path work list
   int cnt, cnt2;
 };
+struct MaskSmemClasses : MaskSmem {
+  int grp_row[TB];
+  int grp_col[TB];
+};
 
 // Conservative "provably no intersection" test.  true => the exact path would find 0 candidate
 // points (so IoU == 0 exactly); false => unknown, run the exact path.  NaN/inf anywhere => false.
@@ -173,11 +216,21 @@ __device__ __forceinline__ bool surely_disjoint(float rcx, float rcy, float rrad
 // `remv` (optional): suppression state at launch time (bit set = box already suppressed by a kept box of an earlier
 // row chunk).  Rows and columns that are already suppressed are skipped: their mask bits can never influence the
 // greedy scan (a suppressed row is never kept, so its mask row is never read; a suppressed column stays suppressed).
+// CLASSES: only same-group pairs are candidates, and the column loop stops at the first later tile whose first group is
+// below the row tile's last group (groups never increase along the rows, so no later tile can hold a same-class pair);
+// the words it does not evaluate are written as zeros.
+template <bool CLASSES>
 __global__ void __launch_bounds__(MASK_THREADS, 3) rnms_mask_kernel(const float* __restrict__ geom, SegArgs sa, float thr,
                                                                  int use_filter, u64* __restrict__ mask, int rb_begin,
-                                                                 const u64* __restrict__ remv) {
+                                                                 const u64* __restrict__ remv, const int* __restrict__ grp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   MaskSmem& sm = *reinterpret_cast<MaskSmem*>(smem_raw);
+  int* grp_row = nullptr;
+  int* grp_col = nullptr;
+  if constexpr (CLASSES) {
+    grp_row = reinterpret_cast<MaskSmemClasses*>(smem_raw)->grp_row;
+    grp_col = reinterpret_cast<MaskSmemClasses*>(smem_raw)->grp_col;
+  }
   const int seg = blockIdx.z;
   const int n = seg_n(sa, seg), n_pad = sa.n_pad, cbs = sa.cbs;
   const int col_blocks = (n + TB - 1) / TB;          // of THIS segment
@@ -197,6 +250,12 @@ __global__ void __launch_bounds__(MASK_THREADS, 3) rnms_mask_kernel(const float*
     sm.row[e] = geom[(size_t)f * n_pad + rb * TB + i];
   }
   for (int e = tid; e < TB * CH; e += MASK_THREADS) sm.mask[e] = 0ull;
+  int grp_last = 0;   // group of the row tile's last box
+  if constexpr (CLASSES) {
+    grp += (size_t)seg * n_pad;
+    for (int e = tid; e < TB; e += MASK_THREADS) grp_row[e] = grp[rb * TB + e];
+    grp_last = grp[min(n, (rb + 1) * TB) - 1];
+  }
 
   const int r = tid & (TB - 1);
   const int g = tid >> 6;  // 4 groups of 16 columns
@@ -204,12 +263,19 @@ __global__ void __launch_bounds__(MASK_THREADS, 3) rnms_mask_kernel(const float*
 
   for (int cc = 0; cc < ncols; cc++) {
     const int cbi = cb0 + cc;
+    if constexpr (CLASSES) {
+      const int grp_first = grp[cbi * TB];
+      if (cbi > rb && (grp_first == 0 || grp_first < grp_last)) break;   // uniform for the CTA
+    }
     const u64 col_dead = remv ? remv[cbi] : 0ull;
     if (col_dead == ~0ull) continue;   // uniform for the CTA: whole column tile already suppressed
     __syncthreads();  // previous tile fully consumed (also covers the row-tile load on cc == 0)
     for (int e = tid; e < kGeomFields * TB; e += MASK_THREADS) {
       const int f = e / TB, i = e % TB;
       sm.col[e] = geom[(size_t)f * n_pad + cbi * TB + i];
+    }
+    if constexpr (CLASSES) {
+      for (int e = tid; e < TB; e += MASK_THREADS) grp_col[e] = grp[cbi * TB + e];
     }
     if (tid == 0) { sm.cnt = 0; sm.cnt2 = 0; }
     __syncthreads();
@@ -224,6 +290,7 @@ __global__ void __launch_bounds__(MASK_THREADS, 3) rnms_mask_kernel(const float*
         for (int k = 0; k < 16; k++) {
           const int c = g * 16 + k;   // same column for the whole warp: shared-memory broadcast
           bool cand = (cbi * TB + c < n) && (cbi > rb || c > r) && !((col_dead >> c) & 1ull);
+          if constexpr (CLASSES) cand = cand && grp_col[c] == grp_row[r] && grp_row[r] != 0;
           if (use_filter) {
             const float dx = sm.col[F_CX * TB + c] - rcx, dy = sm.col[F_CY * TB + c] - rcy;
             const float R = rrad + sm.col[F_RAD * TB + c];
@@ -452,6 +519,8 @@ struct RnmsPlan {
   float* sorted_boxes;
   int* order;
   float* keys[2];
+  u64* keys64[2];    // class-aware form: (group << 32 | score bits) sort keys instead of keys[]
+  int* grp;          // class-aware form: [segs][n_pad] group of each sorted box
   int* vals[2];
   float* geom;
   u64* mask;
@@ -464,17 +533,20 @@ struct RnmsPlan {
   size_t total;
 };
 
-static size_t cub_temp_bytes(int items, int segs) {
+constexpr int kClassKeyBits = 57;   // group (<= 2^24, 25 bits) << 32 | score bits
+
+template <typename K>
+static size_t cub_temp_bytes(int items, int segs, int end_bit) {
   size_t bytes = 0, bytes2 = 0;
-  cub::DoubleBuffer<float> k(nullptr, nullptr);
+  cub::DoubleBuffer<K> k(nullptr, nullptr);
   cub::DoubleBuffer<int> v(nullptr, nullptr);
-  cudaError_t e = cub::DeviceRadixSort::SortPairsDescending(nullptr, bytes, k, v, items, 0, 32, (cudaStream_t)0);
+  cudaError_t e = cub::DeviceRadixSort::SortPairsDescending(nullptr, bytes, k, v, items, 0, end_bit, (cudaStream_t)0);
   if (e != cudaSuccess) {
     cudaGetLastError();  // clear (no device in this process: size-only query)
     bytes = 0;
   }
   e = cub::DeviceSegmentedRadixSort::SortPairsDescending(nullptr, bytes2, k, v, items, segs, (const int*)nullptr,
-                                                         (const int*)nullptr, 0, 32, (cudaStream_t)0);
+                                                         (const int*)nullptr, 0, end_bit, (cudaStream_t)0);
   if (e != cudaSuccess) {
     cudaGetLastError();
     bytes2 = 0;
@@ -485,18 +557,28 @@ static size_t cub_temp_bytes(int items, int segs) {
   return bytes > floor_bytes ? bytes : floor_bytes + (size_t)16 * (size_t)(items > 0 ? items : 0);
 }
 
-static void plan_rnms(int segs, int cap, void* ws, RnmsPlan* p) {
+static void plan_rnms(int segs, int cap, void* ws, RnmsPlan* p, bool classes = false) {
   p->segs = segs;
   p->cap = cap;
   p->n_pad = (cap + TB - 1) / TB * TB;
   p->cbs = p->n_pad / TB;
   const size_t items = (size_t)segs * cap;
-  p->cub_bytes = cub_temp_bytes((int)items, segs);
+  p->cub_bytes = classes ? cub_temp_bytes<u64>((int)items, segs, kClassKeyBits)
+                         : cub_temp_bytes<float>((int)items, segs, 32);
   Carver c(ws);
   p->sorted_boxes = c.take<float>(items * 6);
   p->order = c.take<int>(items);
-  p->keys[0] = c.take<float>(items);
-  p->keys[1] = c.take<float>(items);
+  p->keys[0] = p->keys[1] = nullptr;
+  p->keys64[0] = p->keys64[1] = nullptr;
+  p->grp = nullptr;
+  if (classes) {
+    p->keys64[0] = c.take<u64>(items);
+    p->keys64[1] = c.take<u64>(items);
+    p->grp = c.take<int>((size_t)segs * p->n_pad);
+  } else {
+    p->keys[0] = c.take<float>(items);
+    p->keys[1] = c.take<float>(items);
+  }
   p->vals[0] = c.take<int>(items);
   p->vals[1] = c.take<int>(items);
   p->geom = c.take<float>((size_t)segs * kGeomFields * p->n_pad);
@@ -527,16 +609,47 @@ extern "C" size_t ryolo_rnms_batched_workspace_bytes(int segments, int cap) {
   return p.total;
 }
 
+template <bool CLASSES>
+static int rnms_mask_and_scan(const RnmsPlan& p, const SegArgs& sa, float thr, bool full_mask, int64_t* keep_out,
+                              int32_t* num_keep, cudaStream_t stream) {
+  using MaskSmemT = typename std::conditional<CLASSES, MaskSmemClasses, MaskSmem>::type;
+  RYOLO_SMEM_OPT_IN(rnms_mask_kernel<CLASSES>, sizeof(MaskSmemT));
+  const size_t smem = (size_t)p.cbs * sizeof(u64) * 2;
+  if (smem > 200 * 1024) {
+    set_err("ryolo_rnms: cap=%d too large for the single-CTA scan (col_blocks=%d)", p.cap, p.cbs);
+    return RYOLO_E_UNSUPPORTED;
+  }
+  if (smem > 40 * 1024)
+    RYOLO_CUDA_TRY(cudaFuncSetAttribute(rnms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  RYOLO_CUDA_TRY(cudaMemsetAsync(p.remv_g, 0, 2 * (size_t)p.segs * p.cbs * sizeof(u64), stream));
+  // Row chunks of `chunk` blocks: mask(chunk rows x all later columns, skipping what earlier chunks suppressed),
+  // then scan(chunk) -- for ALL segments at once (grid z / one scan CTA per segment).  full_mask computes every
+  // upper-triangle tile in one launch like the reference.
+  const int chunk = full_mask ? p.cbs : kRowChunkBlocks;
+  for (int b0 = 0; b0 < p.cbs; b0 += chunk) {
+    const int b1 = b0 + chunk < p.cbs ? b0 + chunk : p.cbs;
+    dim3 grid((p.cbs - b0 + CH - 1) / CH, b1 - b0, p.segs);
+    rnms_mask_kernel<CLASSES><<<grid, MASK_THREADS, sizeof(MaskSmemT), stream>>>(
+        p.geom, sa, thr, thr >= 0.f ? 1 : 0, p.mask, b0, full_mask ? nullptr : p.remv_g, p.grp);
+    RYOLO_LAUNCH_CHECK();
+    rnms_scan_kernel<<<p.segs, SCAN_THREADS, smem, stream>>>(p.mask, sa, p.order, p.keep_flag,
+                                                             reinterpret_cast<long long*>(keep_out), num_keep, b0, b1,
+                                                             p.remv_g, p.keptw_g, b1 == p.cbs ? 1 : 0);
+    RYOLO_LAUNCH_CHECK();
+  }
+  return RYOLO_OK;
+}
+
 static int rnms_impl(const float* dets, int segs, int cap, const int32_t* n_dev, int n_host, int limit, float thr,
                      int64_t* keep_out, int32_t* num_keep, void* workspace, size_t workspace_bytes, void* stream_,
-                     bool full_mask) {
+                     bool full_mask, bool classes = false) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RYOLO_ARG_CHECK(dets != nullptr && keep_out != nullptr && workspace != nullptr && num_keep != nullptr);
   RYOLO_ARG_CHECK(segs > 0 && segs <= 65535 && cap > 0 && limit > 0);
   RYOLO_ARG_CHECK((long long)segs * cap < (1ll << 31));
   RYOLO_ARG_CHECK((reinterpret_cast<uintptr_t>(workspace) & 255) == 0);
   RnmsPlan p;
-  plan_rnms(segs, cap, workspace, &p);
+  plan_rnms(segs, cap, workspace, &p, classes);
   if (p.total > workspace_bytes) {
     set_err("ryolo_rnms: workspace %zu B < required %zu B", workspace_bytes, p.total);
     return RYOLO_E_WORKSPACE;
@@ -550,13 +663,34 @@ static int rnms_impl(const float* dets, int segs, int cap, const int32_t* n_dev,
   sa.cbs = p.cbs;
   const int T = 256;
   const bool segmented = segs > 1 || n_dev != nullptr;
-  rnms_keys_kernel<<<dim3((cap + T - 1) / T, segs), T, 0, stream>>>(dets, sa, p.keys[0], p.vals[0],
-                                                                   segmented ? p.seg_begin : nullptr, p.seg_end);
-  RYOLO_LAUNCH_CHECK();
   cub::DoubleBuffer<float> dk(p.keys[0], p.keys[1]);
   cub::DoubleBuffer<int> dv(p.vals[0], p.vals[1]);
   size_t need = 0;
   const int items = segs * cap;
+  if (classes) {
+    // stable per-segment sort by (group desc = class asc, score desc); rows beyond a segment's count are never read
+    rnms_class_keys_kernel<<<dim3((cap + T - 1) / T, segs), T, 0, stream>>>(dets, sa, p.keys64[0], p.vals[0],
+                                                                           p.seg_begin, p.seg_end);
+    RYOLO_LAUNCH_CHECK();
+    cub::DoubleBuffer<u64> dk64(p.keys64[0], p.keys64[1]);
+    RYOLO_CUDA_TRY(cub::DeviceSegmentedRadixSort::SortPairsDescending(nullptr, need, dk64, dv, items, segs, p.seg_begin,
+                                                                      p.seg_end, 0, kClassKeyBits, stream));
+    if (need > p.cub_bytes) {
+      set_err("ryolo_rnms: sort scratch %zu B > planned %zu B", need, p.cub_bytes);
+      return RYOLO_E_WORKSPACE;
+    }
+    size_t tmp = p.cub_bytes;
+    RYOLO_CUDA_TRY(cub::DeviceSegmentedRadixSort::SortPairsDescending(p.cub_temp, tmp, dk64, dv, items, segs,
+                                                                      p.seg_begin, p.seg_end, 0, kClassKeyBits, stream));
+    count_launch(4);
+    rnms_prep_kernel<true><<<dim3((p.n_pad + T - 1) / T, segs), T, 0, stream>>>(
+        dets, dv.Current(), sa, p.sorted_boxes, p.order, p.geom, p.keep_flag, p.grp);
+    RYOLO_LAUNCH_CHECK();
+    return rnms_mask_and_scan<true>(p, sa, thr, full_mask, keep_out, num_keep, stream);
+  }
+  rnms_keys_kernel<<<dim3((cap + T - 1) / T, segs), T, 0, stream>>>(dets, sa, p.keys[0], p.vals[0],
+                                                                   segmented ? p.seg_begin : nullptr, p.seg_end);
+  RYOLO_LAUNCH_CHECK();
   if (!segmented) {
     RYOLO_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, need, dk, dv, n_host, 0, 32, stream));
   } else {
@@ -576,36 +710,10 @@ static int rnms_impl(const float* dets, int segs, int cap, const int32_t* n_dev,
                                                                       p.seg_end, 0, 32, stream));
   }
   count_launch(4);  // radix sort passes (library kernels, counted as a lower bound)
-  rnms_prep_kernel<<<dim3((p.n_pad + T - 1) / T, segs), T, 0, stream>>>(dets, dv.Current(), sa, p.sorted_boxes, p.order,
-                                                                        p.geom, p.keep_flag);
+  rnms_prep_kernel<false><<<dim3((p.n_pad + T - 1) / T, segs), T, 0, stream>>>(
+      dets, dv.Current(), sa, p.sorted_boxes, p.order, p.geom, p.keep_flag, nullptr);
   RYOLO_LAUNCH_CHECK();
-  {
-    RYOLO_SMEM_OPT_IN(rnms_mask_kernel, sizeof(MaskSmem));
-    const size_t smem = (size_t)p.cbs * sizeof(u64) * 2;
-    if (smem > 200 * 1024) {
-      set_err("ryolo_rnms: cap=%d too large for the single-CTA scan (col_blocks=%d)", cap, p.cbs);
-      return RYOLO_E_UNSUPPORTED;
-    }
-    if (smem > 40 * 1024)
-      RYOLO_CUDA_TRY(cudaFuncSetAttribute(rnms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    RYOLO_CUDA_TRY(cudaMemsetAsync(p.remv_g, 0, 2 * (size_t)segs * p.cbs * sizeof(u64), stream));
-    // Row chunks of `chunk` blocks: mask(chunk rows x all later columns, skipping what earlier chunks suppressed),
-    // then scan(chunk) -- for ALL segments at once (grid z / one scan CTA per segment).  full_mask computes every
-    // upper-triangle tile in one launch like the reference.
-    const int chunk = full_mask ? p.cbs : kRowChunkBlocks;
-    for (int b0 = 0; b0 < p.cbs; b0 += chunk) {
-      const int b1 = b0 + chunk < p.cbs ? b0 + chunk : p.cbs;
-      dim3 grid((p.cbs - b0 + CH - 1) / CH, b1 - b0, segs);
-      rnms_mask_kernel<<<grid, MASK_THREADS, sizeof(MaskSmem), stream>>>(p.geom, sa, thr, thr >= 0.f ? 1 : 0, p.mask, b0,
-                                                                          full_mask ? nullptr : p.remv_g);
-      RYOLO_LAUNCH_CHECK();
-      rnms_scan_kernel<<<segs, SCAN_THREADS, smem, stream>>>(p.mask, sa, p.order, p.keep_flag,
-                                                             reinterpret_cast<long long*>(keep_out), num_keep, b0, b1,
-                                                             p.remv_g, p.keptw_g, b1 == p.cbs ? 1 : 0);
-      RYOLO_LAUNCH_CHECK();
-    }
-  }
-  return RYOLO_OK;
+  return rnms_mask_and_scan<false>(p, sa, thr, full_mask, keep_out, num_keep, stream);
 }
 
 static int rnms_single(const float* dets, int n, float thr, int64_t* keep_out, int32_t* num_keep, void* workspace,
@@ -633,6 +741,21 @@ extern "C" int ryolo_rnms_batched(const float* dets, int segments, int cap, cons
                                   void* stream_) {
   RYOLO_ARG_CHECK(n_dev != nullptr);
   return rnms_impl(dets, segments, cap, n_dev, 0, limit, thr, keep_out, num_keep, workspace, workspace_bytes, stream_, false);
+}
+
+extern "C" size_t ryolo_rnms_batched_classes_workspace_bytes(int segments, int cap) {
+  if (segments <= 0 || cap <= 0) return 256;
+  RnmsPlan p;
+  plan_rnms(segments, cap, nullptr, &p, true);
+  return p.total;
+}
+
+extern "C" int ryolo_rnms_batched_classes(const float* dets8, int segments, int cap, const int32_t* n_dev, float thr,
+                                          int64_t* keep_out, int32_t* num_keep, void* workspace, size_t workspace_bytes,
+                                          void* stream_) {
+  RYOLO_ARG_CHECK(n_dev != nullptr);
+  return rnms_impl(dets8, segments, cap, n_dev, 0, cap, thr, keep_out, num_keep, workspace, workspace_bytes, stream_,
+                   false, true);
 }
 
 extern "C" int ryolo_rnms_debug_views(void* workspace, int n, const float** sorted_boxes, const int32_t** order,

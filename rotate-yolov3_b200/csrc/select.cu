@@ -207,6 +207,9 @@ __device__ __forceinline__ int sel_block_prefix(int* s_warp, bool pred) {
   return prefix + __popc(bal & ((1u << lane) - 1u));
 }
 
+// CLASSES: 8-column rows (x, y, w, h, theta, conf, class_conf, class) like the reference's torch.cat((pred[:, :6],
+// class_conf, class_pred.float())) (nms.py:51)
+template <bool CLASSES>
 __global__ void __launch_bounds__(SEL_T) sel_write_kernel(const float* __restrict__ io, int p, int nc,
                                                           const unsigned* __restrict__ keys,
                                                           const SelState* __restrict__ st,
@@ -226,8 +229,14 @@ __global__ void __launch_bounds__(SEL_T) sel_write_kernel(const float* __restric
                           sel_block_prefix(s_warp[1], is_tied);
   if (is_above || (is_tied && tied_before < need)) {
     const float* row = io + ((size_t)b * p + i) * (6 + nc);
-    float* o = dets + ((size_t)b * cap + above_before + min(tied_before, need)) * 6;
+    constexpr int DW = CLASSES ? 8 : 6;
+    float* o = dets + ((size_t)b * cap + above_before + min(tied_before, need)) * DW;
     o[0] = row[0]; o[1] = row[1]; o[2] = row[2]; o[3] = row[3]; o[4] = row[4]; o[5] = __uint_as_float(key);
+    if constexpr (CLASSES) {
+      float best; int bi; bool fin;
+      class_max(row, nc, &best, &bi, &fin);
+      o[6] = best; o[7] = (float)bi;
+    }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) n_out[b] = totals[b * 2 + 0] + min(totals[b * 2 + 1], need);
 }
@@ -245,9 +254,10 @@ extern "C" size_t ryolo_detect_select_workspace_bytes(int batch, int p) {
          256;
 }
 
-extern "C" int ryolo_detect_select(const float* io, int batch, int p, int nc, float conf_thres, float min_wh, int limit,
-                                   float* dets_out, int cap, int32_t* n_out, void* workspace, size_t workspace_bytes,
-                                   void* stream_) {
+template <bool CLASSES>
+static int detect_select_impl(const float* io, int batch, int p, int nc, float conf_thres, float min_wh, int limit,
+                              float* dets_out, int cap, int32_t* n_out, void* workspace, size_t workspace_bytes,
+                              void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RYOLO_ARG_CHECK(io && dets_out && n_out && workspace && batch > 0 && p > 0 && nc >= 1 && limit > 0 && cap >= limit);
   RYOLO_ARG_CHECK(batch <= 65535);
@@ -281,7 +291,23 @@ extern "C" int ryolo_detect_select(const float* io, int batch, int p, int nc, fl
   RYOLO_LAUNCH_CHECK();
   sel_scan_kernel<<<batch * 2, 1024, 0, stream>>>(counts, nblocks, totals);
   RYOLO_LAUNCH_CHECK();
-  sel_write_kernel<<<gc, SEL_T, 0, stream>>>(io, p, nc, keys, st, counts, totals, nblocks, dets_out, cap, n_out);
+  sel_write_kernel<CLASSES><<<gc, SEL_T, 0, stream>>>(io, p, nc, keys, st, counts, totals, nblocks, dets_out, cap,
+                                                      n_out);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
+}
+
+extern "C" int ryolo_detect_select(const float* io, int batch, int p, int nc, float conf_thres, float min_wh, int limit,
+                                   float* dets_out, int cap, int32_t* n_out, void* workspace, size_t workspace_bytes,
+                                   void* stream_) {
+  return detect_select_impl<false>(io, batch, p, nc, conf_thres, min_wh, limit, dets_out, cap, n_out, workspace,
+                                   workspace_bytes, stream_);
+}
+
+extern "C" int ryolo_detect_select_classes(const float* io, int batch, int p, int nc, float conf_thres, float min_wh,
+                                           int limit, float* dets_out, int cap, int32_t* n_out, void* workspace,
+                                           size_t workspace_bytes, void* stream_) {
+  RYOLO_ARG_CHECK(nc <= (1 << 24));   // class ids in [0, 2^24): exact in fp32 and a valid class of the batched NMS
+  return detect_select_impl<true>(io, batch, p, nc, conf_thres, min_wh, limit, dets_out, cap, n_out, workspace,
+                                  workspace_bytes, stream_);
 }

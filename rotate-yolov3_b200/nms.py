@@ -202,3 +202,51 @@ def detect_postprocess(io, conf_thres, nms_thres, cap, filter_done_event=None):
         filter_done_event.record()
     keep, num = r_nms_batched(dets, counts, nms_thres)
     return {"dets": dets, "counts": counts, "keep": keep, "num_keep": num}
+
+
+def detect_postprocess_classes(io, conf_thres, nms_thres, cap, min_wh=2.0):
+    """detect_postprocess for any number of classes, still without host round trips: the same device-side selection of
+    the top-`cap` candidates per image (over all classes), written with the class columns, then one segmented rotated
+    NMS with one segment per image that suppresses only within a class -- the reference's per-class loop
+    (utils/nms/nms.py:47-56).  io [B, P, 6+nc] float32 CUDA, nc >= 1, not modified; conf_thres >= 0.
+    Returns dict(dets [B, cap, 8] = (x, y, w, h, theta, conf, class_conf, class) in input order, counts [B] int32,
+    keep [B, cap] int64, num_keep [B] int32): image b keeps rows dets[b, keep[b, :num_keep[b]]] (ascending rows)."""
+    if io.dim() != 3 or io.shape[-1] < 7:
+        raise ValueError("detect_postprocess_classes takes io [B, P, 6+nc] with nc >= 1, got %s" % (tuple(io.shape),))
+    if not io.is_contiguous():
+        io = io.contiguous()
+    bsz, p, no = io.shape
+    cap = int(cap)
+    with torch.cuda.device(io.device):
+        dets = torch.empty((bsz, cap, 8), dtype=torch.float32, device=io.device)
+        counts = torch.empty((bsz,), dtype=torch.int32, device=io.device)
+        ws_bytes = _lib.lib.ryolo_detect_select_workspace_bytes(bsz, p)
+        ws = _workspace(ws_bytes, io.device)
+        stream = _lib.stream_ptr(io.device)
+        st = _lib.lib.ryolo_detect_select_classes(_lib.ptr(io), bsz, p, no - 6, float(conf_thres), float(min_wh), cap,
+                                                  _lib.ptr(dets), cap, _lib.ptr(counts), _lib.ptr(ws), ws_bytes, stream)
+        _lib.check(st, "ryolo_detect_select_classes")
+        keep = torch.empty((bsz, cap), dtype=torch.long, device=io.device)
+        num = torch.empty((bsz,), dtype=torch.int32, device=io.device)
+        ws_bytes = _lib.lib.ryolo_rnms_batched_classes_workspace_bytes(bsz, cap)
+        ws = _workspace(ws_bytes, io.device)
+        st = _lib.lib.ryolo_rnms_batched_classes(_lib.ptr(dets), bsz, cap, _lib.ptr(counts), float(nms_thres),
+                                                 _lib.ptr(keep), _lib.ptr(num), _lib.ptr(ws), ws_bytes, stream)
+        _lib.check(st, "ryolo_rnms_batched_classes")
+    return {"dets": dets, "counts": counts, "keep": keep, "num_keep": num}
+
+
+def detections_per_image(res):
+    """The result of detect_postprocess_classes as non_max_suppression's list: per image a Tensor[k, 8] of the kept rows
+    ordered by confidence descending, ties by class ascending, then by input row -- or None when nothing is kept.
+    One host read (the kept counts) for the whole batch."""
+    nums = res["num_keep"].tolist()
+    out = []
+    for b, k in enumerate(nums):
+        if k == 0:
+            out.append(None)
+            continue
+        rows = res["dets"][b][res["keep"][b, :k]]                       # input order
+        rows = rows[torch.argsort(rows[:, 7], stable=True)]             # class ascending, input order within a class
+        out.append(rows[torch.argsort(rows[:, 5], descending=True, stable=True)])
+    return out

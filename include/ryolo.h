@@ -356,6 +356,20 @@ int ryolo_space_to_depth(const void* x, int x_cstride, int batch, int h, int w, 
                          int xs_cstride, void* stream);
 int ryolo_depth_to_space(const void* dxs, int dxs_cstride, int batch, int h, int w, int c, void* gx,
                          int gx_cstride, int accumulate, void* stream);
+/* Phase decomposition of a dilated 3x3 conv (reference `[d-convolutional]` blocks: F.conv2d with dilation (dh, dw),
+ * pad (dh, dw), model/models.py:262-265).  ryolo_dilate_split writes the dh*dw phase images of x ([B, H+2, W+2, >=C])
+ * into xp ([B*dh*dw, Hp+2, Wp+2, >=C], Hp = ceil(H/dh), Wp = ceil(W/dw), zero halo):
+ *   xp[(b*dh + ry)*dw + rx, Y, X, c] = x[b, Y*dh + ry, X*dw + rx, c], 0 where Y*dh + ry >= H or X*dw + rx >= W.
+ * On xp the dilated conv is an ordinary pad-1 3x3 conv with batch B*dh*dw.  ryolo_dilate_merge writes the interior of
+ * y back from the phase images: y[b, y, x, c] = xp[phase of (y, x)] (+ residual[b, y, x, c]) (+ y[b, y, x, c] when
+ * accumulate), summed in fp32 in that order and rounded to bf16 once.  Each is the other's adjoint.  C % 8 == 0,
+ * channel strides % 8 == 0, 16-byte aligned pointers.  The extents are not checked: xp must hold
+ * [B*dh*dw, Hp+2, Wp+2, xp_cstride] (x and y [B, H+2, W+2, their cstride]), and xp's halo must already be zero -- the
+ * split writes the interior (zero fill included) and channels [0, C) only; the merge writes y's interior only. */
+int ryolo_dilate_split(const void* x, int x_cstride, int batch, int h, int w, int c, int dh, int dw, void* xp,
+                       int xp_cstride, void* stream);
+int ryolo_dilate_merge(const void* xp, int xp_cstride, int batch, int h, int w, int c, int dh, int dw,
+                       const void* residual, int res_cstride, int accumulate, void* y, int y_cstride, void* stream);
 /* Squeeze-and-excitation block (reference SELayer, model/models.py:16-31; `[se]` blocks of cfg/ICDAR/yolov3_608_se.cfg,
  * cfg/HRSC+/yolov3_512_se.cfg): x[b,:,:,c] *= sigmoid(W2 . relu(W1 . mean_hw x[b]))[c], in place on a padded-NHWC bf16
  * tensor.  w1 [reduced, c], w2 [c, reduced] fp32 (nn.Linear weights, no bias); sums_scratch / scale_scratch [batch*c]

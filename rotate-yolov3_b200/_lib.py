@@ -100,6 +100,8 @@ SIGNATURES = {
     "ryolo_zero_insert2x": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "ryolo_space_to_depth": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_depth_to_space": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
+    "ryolo_dilate_split": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
+    "ryolo_dilate_merge": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _vp]),
     "ryolo_se_block": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "ryolo_se_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "ryolo_se_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),

@@ -450,6 +450,50 @@ __global__ void __launch_bounds__(256) depth_to_space_kernel(const __nv_bfloat16
   *reinterpret_cast<uint4*>(gp) = pack8(d);
 }
 
+// Phase decomposition of the dilated 3x3 convolutions ([d-convolutional] blocks, dilation (dh, dw), pad (dh, dw)):
+// xp[(b*dh + ry)*dw + rx, Y, X, c] = x[b, Y*dh + ry, X*dw + rx, c], zero where that pixel is past the edge.  On every
+// phase image the dilated conv is an ordinary pad-1 3x3 conv.  One thread per 16-byte group of the phase image; the
+// stores are contiguous, the loads contiguous within each pixel.
+__global__ void __launch_bounds__(256) dilate_split_kernel(const __nv_bfloat16* __restrict__ x, int xcs, Geo g /*of x*/,
+                                                           Geo gp /*of xp*/, int dh, int dw, __nv_bfloat16* __restrict__ xp,
+                                                           int pcs) {
+  const size_t item = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  int n, py, px, cg;
+  if (!decode_item(gp, item, n, py, px, cg)) return;
+  const int rx = n % dw, ry = (n / dw) % dh, b = n / (dw * dh);
+  const int y = py * dh + ry, xx = px * dw + rx;
+  uint4 v = make_uint4(0u, 0u, 0u, 0u);
+  if (y < g.h && xx < g.w) v = *reinterpret_cast<const uint4*>(x + pad_off(b, y, xx, g.h, g.w, xcs) + cg * 8);
+  *reinterpret_cast<uint4*>(xp + pad_off(n, py, px, gp.h, gp.w, pcs) + cg * 8) = v;
+}
+// its inverse on the interior pixels and its adjoint: y[b, y, x] = xp[phase of (y, x)] (+ residual) (+ y), summed in fp32
+// in that order and rounded to bf16 once
+__global__ void __launch_bounds__(256) dilate_merge_kernel(const __nv_bfloat16* __restrict__ xp, int pcs, Geo gp /*of xp*/,
+                                                           Geo g /*of y*/, int dh, int dw,
+                                                           const __nv_bfloat16* __restrict__ res, int rcs, int accumulate,
+                                                           __nv_bfloat16* __restrict__ y, int ycs) {
+  const size_t item = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  int b, yy, xx, cg;
+  if (!decode_item(g, item, b, yy, xx, cg)) return;
+  const int n = (b * dh + yy % dh) * dw + xx % dw;
+  float d[8];
+  unpack8(*reinterpret_cast<const uint4*>(xp + pad_off(n, yy / dh, xx / dw, gp.h, gp.w, pcs) + cg * 8), d);
+  if (res) {
+    float r[8];
+    unpack8(*reinterpret_cast<const uint4*>(res + pad_off(b, yy, xx, g.h, g.w, rcs) + cg * 8), r);
+#pragma unroll
+    for (int e = 0; e < 8; e++) d[e] += r[e];
+  }
+  __nv_bfloat16* yp = y + pad_off(b, yy, xx, g.h, g.w, ycs) + cg * 8;
+  if (accumulate) {
+    float o[8];
+    unpack8(*reinterpret_cast<const uint4*>(yp), o);
+#pragma unroll
+    for (int e = 0; e < 8; e++) d[e] += o[e];
+  }
+  *reinterpret_cast<uint4*>(yp) = pack8(d);
+}
+
 // 2x2 max pooling on padded NHWC (reference: nn.MaxPool2d(2, stride) blocks of cfg/yolov3-tiny.cfg, model/models.py:79-87).
 // stride 2: out[y, x] = max over in[2y..2y+1, 2x..2x+1].  stride 1: the reference zero-pads right/bottom
 // (nn.ZeroPad2d((0,1,0,1))) and pools with stride 1 -> out[y, x] = max over in[y..y+1, x..x+1] where the row/column past
@@ -840,6 +884,44 @@ extern "C" int ryolo_depth_to_space(const void* dxs, int dxs_cstride, int batch,
   depth_to_space_kernel<<<(unsigned)((items + 255) / 256), 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(dxs),
                                                                             dxs_cstride, g, static_cast<__nv_bfloat16*>(gx),
                                                                             gx_cstride, accumulate);
+  RYOLO_LAUNCH_CHECK();
+  return RYOLO_OK;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+extern "C" int ryolo_dilate_split(const void* x, int x_cstride, int batch, int h, int w, int c, int dh, int dw, void* xp,
+                                  int xp_cstride, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  RYOLO_ARG_CHECK(x && xp && aligned16(x) && aligned16(xp));
+  GEO_CHECK();
+  RYOLO_ARG_CHECK(dh >= 1 && dw >= 1 && (long long)batch * dh * dw < (1ll << 24));
+  RYOLO_ARG_CHECK(x_cstride >= c && x_cstride % 8 == 0 && xp_cstride >= c && xp_cstride % 8 == 0);
+  const Geo g = mk_geo(batch, h, w, c);
+  const Geo gp = mk_geo(batch * dh * dw, (h + dh - 1) / dh, (w + dw - 1) / dw, c);
+  const size_t items = n_items(gp);
+  dilate_split_kernel<<<(unsigned)((items + 255) / 256), 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), x_cstride,
+                                                                          g, gp, dh, dw, static_cast<__nv_bfloat16*>(xp),
+                                                                          xp_cstride);
+  RYOLO_LAUNCH_CHECK();
+  return RYOLO_OK;
+}
+
+extern "C" int ryolo_dilate_merge(const void* xp, int xp_cstride, int batch, int h, int w, int c, int dh, int dw,
+                                  const void* residual, int res_cstride, int accumulate, void* y, int y_cstride,
+                                  void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  RYOLO_ARG_CHECK(xp && y && aligned16(xp) && aligned16(y) && (!residual || aligned16(residual)));
+  GEO_CHECK();
+  RYOLO_ARG_CHECK(dh >= 1 && dw >= 1 && (long long)batch * dh * dw < (1ll << 24));
+  RYOLO_ARG_CHECK(xp_cstride >= c && xp_cstride % 8 == 0 && y_cstride >= c && y_cstride % 8 == 0);
+  RYOLO_ARG_CHECK(!residual || (res_cstride >= c && res_cstride % 8 == 0));
+  const Geo g = mk_geo(batch, h, w, c);
+  const Geo gp = mk_geo(batch * dh * dw, (h + dh - 1) / dh, (w + dw - 1) / dw, c);
+  const size_t items = n_items(g);
+  dilate_merge_kernel<<<(unsigned)((items + 255) / 256), 256, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(xp), xp_cstride, gp, g, dh, dw, static_cast<const __nv_bfloat16*>(residual),
+      res_cstride, accumulate, static_cast<__nv_bfloat16*>(y), y_cstride);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }

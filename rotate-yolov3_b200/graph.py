@@ -12,6 +12,7 @@ Refused everywhere, because every plan relies on the layout: a shortcut whose so
 conv's output shape (the epilogue reads the residual at the output's pixels and channels), and a concat source whose
 channel count is not a multiple of 8 (its producer stores at that channel offset through TMA, 16-byte aligned)."""
 from . import layout as L
+from .parse_config import dilation
 
 
 def route_sources(d, i):
@@ -47,7 +48,14 @@ class Conv:
         self.i, self.k, self.stride = i, int(d["size"]), int(d["stride"])
         self.cout, self.oh, self.ow = shape[i]
         self.cin, self.ih, self.iw = (3, height, width) if i == 0 else shape[i - 1]
-        self.has_bn, self.has_act = hasattr(seq, "BatchNorm2d"), hasattr(seq, "activation")
+        # owner: the block whose weight a `weight_from` block borrows; such a block is a purely linear conv (no bias, BN
+        # or activation, whatever its own modules hold).  dil: (dh, dw) of a [d-convolutional] block, else None.
+        self.owner = int(d["weight_from"]) if "weight_from" in d else None
+        self.dil = dilation(d) if d["type"] == "d-convolutional" else None
+        if self.owner is not None:
+            self.has_bn = self.has_act = False
+        else:
+            self.has_bn, self.has_act = hasattr(seq, "BatchNorm2d"), hasattr(seq, "activation")
         self.fuse_res = nxt == "shortcut" and i not in model.routes
         self.fuse_up = nxt == "upsample" and i not in model.routes and int(defs[i + 1]["stride"]) == 2
         # head = the linear, BN-less conv feeding a YOLO layer (or, in YOLO-less trunk graphs, any such conv)
@@ -58,12 +66,15 @@ class Conv:
             frm = int(defs[i + 1]["from"])
             self.shortcut = i + 1 + frm if frm < 0 else frm
         self.s2d = (self.stride == 2 and self.k == 3 and self.ih % 2 == 0 and self.iw % 2 == 0 and self.cin % 8 == 0)
+        if self.dil is not None and (self.fuse_up or self.is_head):
+            raise NotImplementedError("[d-convolutional] block %d feeding an upsample or a YOLO layer" % i)
 
 
 class Graph:
     def __init__(self, model, height, width, accept, refuse):
         """accept: the block types beyond convolutional / route / shortcut / upsample / yolo that the plan runs ("se",
-        "maxpool"); any other type raises NotImplementedError(refuse % type)."""
+        "maxpool", "d-convolutional": the dilated convs and every `weight_from` block); any other type raises
+        NotImplementedError(refuse % type)."""
         defs = self.defs = model.module_defs
         n = len(defs)
         shape = self.shape = [None] * n          # (C, H, W) of every block's output
@@ -72,7 +83,9 @@ class Graph:
         c, h, w = 3, height, width
         for i, d in enumerate(defs):
             t = d["type"]
-            if t == "convolutional":
+            if "weight_from" in d and "d-convolutional" not in accept:
+                raise NotImplementedError(refuse % ("%s with weight_from" % t))
+            if t == "convolutional" or (t == "d-convolutional" and t in accept):
                 s = int(d["stride"])
                 c, h, w = int(d["filters"]), (h + s - 1) // s, (w + s - 1) // s
             elif t == "upsample":
@@ -102,7 +115,7 @@ class Graph:
         i = 0
         while i < n:
             t = defs[i]["type"]
-            if t == "convolutional":
+            if t in ("convolutional", "d-convolutional"):
                 cv = self.convs[i] = Conv(model, i, shape, height, width)
                 if cv.shortcut is not None and (cv.shortcut not in made or shape[cv.shortcut] != shape[i]):
                     raise NotImplementedError("shortcut source layout")

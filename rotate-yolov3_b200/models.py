@@ -124,6 +124,21 @@ def create_modules(module_defs, arc, hyp):
                 modules.add_module("BatchNorm2d", nn.BatchNorm2d(filters, momentum=0.1))
             if mdef["activation"] == "leaky":
                 modules.add_module("activation", nn.PReLU(num_parameters=1, init=0.10))
+        elif t == "d-convolutional":
+            # reference models.py:68-77: the block's own layers are an empty Conv2d, BatchNorm2d and LeakyReLU; the
+            # forward runs only the conv with the weight of block `weight_from` (models.py:255-265)
+            if "weight_from" not in mdef:
+                raise NotImplementedError("[d-convolutional] block %d without weight_from (identity -> BN -> leaky) has "
+                                          "no kernel" % i)
+            if int(mdef["pad"]) != 1 or int(mdef["stride"]) != 1:
+                raise NotImplementedError("[d-convolutional] block %d: only pad=1, stride=1 ('same' size) runs" % i)
+            bn = int(mdef["batch_normalize"])
+            filters = int(mdef["filters"])
+            modules.add_module("Conv2d", nn.Sequential())
+            if bn:
+                modules.add_module("BatchNorm2d", nn.BatchNorm2d(filters, momentum=0.1))
+            if mdef["activation"] == "leaky":
+                modules.add_module("activation", nn.LeakyReLU(0.1, inplace=True))
         elif t == "maxpool":
             k, s = int(mdef["size"]), int(mdef["stride"])
             mp = nn.MaxPool2d(kernel_size=k, stride=s, padding=int((k - 1) // 2))
@@ -151,9 +166,26 @@ def create_modules(module_defs, arc, hyp):
                                 yolo_index=yolo_index, arc=arc)
         else:
             raise NotImplementedError("layer type %r is outside the hot-path scope (SURVEY.md section 2)" % t)
+        if "weight_from" in mdef:
+            _check_shared_weight(module_defs, module_list, i, output_filters[-1], filters)
         module_list.append(modules)
         output_filters.append(filters)
     return module_list, routes
+
+
+def _check_shared_weight(module_defs, module_list, i, cin, cout):
+    """A `weight_from = j` block runs F.conv2d(x, module_list[j].Conv2d.weight) with stride 1 and no bias, BN or
+    activation (reference models.py:255-265).  Only an earlier [convolutional] block that owns its weight may be j."""
+    mdef, j = module_defs[i], int(module_defs[i]["weight_from"])
+    if not (0 <= j < i and module_defs[j]["type"] == "convolutional" and "weight_from" not in module_defs[j]):
+        raise NotImplementedError("block %d: weight_from=%d is not an earlier [convolutional] block with its own "
+                                  "Conv2d" % (i, j))
+    k = int(mdef["size"])
+    if int(mdef["stride"]) != 1 or (k == 3 and int(mdef["pad"]) != 1):
+        raise NotImplementedError("block %d: weight_from blocks run with stride 1 and 'same' padding only" % i)
+    if tuple(module_list[j].Conv2d.weight.shape) != (cout, cin, k, k):
+        raise ValueError("block %d: weight_from=%d has weight %s, the block needs %s" % (
+            i, j, tuple(module_list[j].Conv2d.weight.shape), (cout, cin, k, k)))
 
 
 class Darknet(nn.Module):
@@ -230,17 +262,52 @@ class Darknet(nn.Module):
         return w, scale, bias, slope
 
     def _build_plan(self, batch, height, width, device):
-        g = G.Graph(self, height, width, ("se", "maxpool"), "block type %r has no sm_90a kernel yet")
+        g = G.Graph(self, height, width, ("se", "maxpool", "d-convolutional"), "block type %r has no sm_90a kernel yet")
         bufs = G.Buffers(g, lambda h, w, cs: (L.alloc_padded(batch, h, w, cs, device), None), 32)
         steps = []
         heads = []
         first_xs = None
+        raw = {}          # owner block -> its RAW packed weight, shared by every `weight_from` use
+        phase = {}        # (role, shape) -> phase-layout scratch of the dilated convs (the steps run in order)
+
+        def phase_buf(role, nb, h, w, cs):
+            key = (role, nb, h, w, cs)
+            if key not in phase:
+                phase[key] = L.alloc_padded(nb, h, w, cs, device)
+            return phase[key]
+
         for t, i in g.ops:
-            if t == "convolutional":
+            if t in ("convolutional", "d-convolutional"):
                 cv = g.convs[i]
                 src = None if i == 0 else bufs.view(i - 1)
                 cout, oh, ow, k, s = cv.cout, cv.oh, cv.ow, cv.k, cv.stride
-                wt, scale, bias, slope = self._folded(i, device)
+                if cv.owner is not None:
+                    # reference models.py:265: the owner's raw weight, no bias, BN or activation
+                    wt = self.module_list[cv.owner].Conv2d.weight
+                    scale, bias, slope = None, torch.zeros(cout, dtype=torch.float32, device=device), None
+                else:
+                    wt, scale, bias, slope = self._folded(i, device)
+                if cv.dil is not None:
+                    # dilated 3x3 = ordinary pad-1 3x3 conv on the dh*dw phase images (ryolo_dilate_split / _merge);
+                    # the shortcut that follows it is added by the merge
+                    dh, dw = cv.dil
+                    nb, hp, wp = batch * dh * dw, -(-src.h // dh), -(-src.w // dw)
+                    xp = phase_buf("x", nb, hp, wp, L.round_up(src.c, 64))
+                    yp = phase_buf("y", nb, hp, wp, L.round_up(cout, 32))
+                    desc = L.make_desc(nb, hp, wp, src.c, xp.shape[-1], cout, yp.shape[-1], 3, 1, False, 0.0)
+                    if cv.owner not in raw:
+                        raw[cv.owner] = L.pack_weights(desc, wt)
+                    out = bufs.out(cv.mat)[0]
+                    res = bufs.view(cv.shortcut) if cv.fuse_res else None
+                    steps.append(("dsplit", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c, dh=dh, dw=dw, xp=xp,
+                                                 keep=src)))
+                    steps.append(("conv", dict(desc=desc, x=xp.data_ptr(), w=raw[cv.owner], b=L.padded_bias(desc, bias),
+                                               y=yp.data_ptr(), r=None, keep=(xp, yp))))
+                    steps.append(("dmerge", dict(yp=yp, h=src.h, w=src.w, c=cout, dh=dh, dw=dw,
+                                                 r=res.ptr if res is not None else None,
+                                                 rcs=res.cs if res is not None else 0, y=out.ptr, ycs=out.cs,
+                                                 keep=(res, out))))
+                    continue
                 if i == 0:
                     if not (k == 3 and s == 1 and wt.shape[1] == 3 and cout in (16, 32) and slope is not None):
                         raise NotImplementedError("first layer must be 3x3/1 conv, 3 -> 16|32 channels, leaky")
@@ -286,7 +353,12 @@ class Darknet(nn.Module):
                     if fuse_res:
                         res = bufs.view(cv.shortcut)
                         desc.res_stride = res.cs
-                pw = L.pack_weights(desc, wt, scale)
+                if cv.owner is not None:
+                    if cv.owner not in raw:
+                        raw[cv.owner] = L.pack_weights(desc, wt)
+                    pw = raw[cv.owner]
+                else:
+                    pw = L.pack_weights(desc, wt, scale)
                 pb = L.padded_bias(desc, bias)
                 steps.append(("conv", dict(desc=desc, x=x_ptr, w=pw, b=pb, y=out_ptr,
                                            r=res.ptr if res is not None else None, keep=(src, res, out))))
@@ -410,6 +482,15 @@ class Darknet(nn.Module):
                 st = lib.ryolo_space_to_depth(ctypes.c_void_p(a["x"]), a["xcs"], b, a["h"], a["w"], a["c"],
                                               _lib.ptr(a["xs"]), a["xs"].shape[-1], stream)
                 _lib.check(st, "ryolo_space_to_depth")
+            elif kind == "dsplit":
+                st = lib.ryolo_dilate_split(ctypes.c_void_p(a["x"]), a["xcs"], b, a["h"], a["w"], a["c"], a["dh"], a["dw"],
+                                            _lib.ptr(a["xp"]), a["xp"].shape[-1], stream)
+                _lib.check(st, "ryolo_dilate_split")
+            elif kind == "dmerge":
+                st = lib.ryolo_dilate_merge(_lib.ptr(a["yp"]), a["yp"].shape[-1], b, a["h"], a["w"], a["c"], a["dh"],
+                                            a["dw"], ctypes.c_void_p(a["r"]) if a["r"] else None, a["rcs"], 0,
+                                            ctypes.c_void_p(a["y"]), a["ycs"], stream)
+                _lib.check(st, "ryolo_dilate_merge")
             elif kind == "first":
                 if a["xs"] is not None:
                     st = lib.ryolo_conv_first_s2d_fwd(_lib.ptr(x), b, h, w, _lib.ptr(a["w"]), _lib.ptr(a["b"]),

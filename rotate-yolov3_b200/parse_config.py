@@ -54,6 +54,13 @@ def parse_model_cfg(path):
     return mdefs
 
 
+def dilation(mdef):
+    """(dh, dw) of a [d-convolutional] block: the value stays the string '(a,b)' in the parsed cfg and is read as
+    (int(s[1]), int(s[3])) (reference model/models.py:263)"""
+    s = mdef["dilation"]
+    return int(s[1]), int(s[3])
+
+
 def hyp_parse(path):
     """'key: value  # comment' lines -> dict of floats (reference utils/utils.py:33-47; expressions such as
     '3.1415926/12' are evaluated arithmetically)."""

@@ -30,7 +30,7 @@ class _Block:
 class TrainPlan:
     def __init__(self, model, batch, height, width, device):
         self.model, self.batch, self.h, self.w, self.device = model, batch, height, width, device
-        g = G.Graph(model, height, width, ("se",), "block type %r has no training kernel")
+        g = G.Graph(model, height, width, ("se", "d-convolutional"), "block type %r has no training kernel")
         if not model.yolo_layers and any(cv.is_head for cv in g.convs.values()):
             # the head bookkeeping (create_grids, the gradients autograd hands back) zips the heads with yolo_layers
             raise NotImplementedError("training needs the YOLO layers of the graph; YOLO-less trunks run in eval only")
@@ -41,8 +41,9 @@ class TrainPlan:
         # first layer input: im2col of the image (27 real channels in a 64-channel padded NHWC buffer)
         self.col = L.alloc_padded(batch, height, width, 64, device)
         blocks = []
+        self.phase = {}          # (role, shape) -> phase-layout scratch of the dilated convs (blocks run one at a time)
         for t, i in g.ops:
-            if t == "convolutional":
+            if t in ("convolutional", "d-convolutional"):
                 blk = g.convs[i]
                 if i == 0:
                     if not (blk.k == 3 and blk.stride == 1):
@@ -97,7 +98,12 @@ class TrainPlan:
                         # dgrad: stride-1 conv of dz (at the INPUT resolution) with mirrored taps / transposed weights
                         blk.ddesc = L.make_desc(batch, blk.src.h, blk.src.w, blk.cout, blk.zcs, blk.cin, blk.gsrc.cs,
                                                 blk.k, 1, False, 0.0, False, blk.gsrc.cs, False, False)
+                if blk.owner is not None:
+                    self._linear_block(blk, batch, device)
                 blk.dw_shape = (blk.k_eff * blk.k_eff, blk.cout_pad, blk.cin_pad)
+                if blk.owner is not None:
+                    blocks.append(blk)           # shares the owner's pw / pwd / dw (set below)
+                    continue
                 blk.pw = torch.empty(_lib.lib.ryolo_conv_packed_weight_bytes(ctypes.byref(blk.fdesc)), dtype=torch.uint8,
                                      device=device)
                 if i > 0:
@@ -120,6 +126,22 @@ class TrainPlan:
                 se.p = torch.zeros(batch * se.cr, dtype=torch.float32, device=device)
                 prod[0].se = se
         self.blocks = blocks
+        by_index = {b.i: b for b in blocks}
+        for b in blocks:
+            if b.owner is not None:
+                ow = by_index[b.owner]
+                if ow.owner is not None or ow.s2d or ow.stride != 1 or ow.k != b.k or ow.cout_pad != b.cout_pad or \
+                        ow.cin_pad != b.cin_pad:
+                    raise NotImplementedError("block %d: weight_from=%d has a different training geometry" % (b.i, b.owner))
+                b.owner_blk = ow
+                b.pw, b.pwd = ow.pw, ow.pwd
+        # a bias (+ PReLU) conv without BatchNorm runs bn_act_fwd / bn_act_bwd with fixed statistics: scale 1, shift =
+        # the conv bias (mean 0, invstd 1 are never read with has_bn = 0); d-beta is the bias gradient
+        for b in blocks:
+            if not b.is_head and b.owner is None and not b.has_bn:
+                b.scale.fill_(1.0)
+                b.invstd.fill_(1.0)
+        self.scratch_sums = torch.zeros(2 * 2048 + 1, dtype=torch.float32, device=device)
         ses = [b.se for b in blocks if b.se is not None]
         self.se_ws = torch.empty(max([_lib.lib.ryolo_se_workspace_bytes(batch, se.h, se.w, se.c, se.cr) for se in ses] + [0]),
                                  dtype=torch.uint8, device=device)
@@ -128,7 +150,7 @@ class TrainPlan:
             c_.xs_from_producer = False
         for c_ in blocks:
             if c_.s2d:
-                prod = [p_ for p_ in blocks if not p_.is_head and p_.y is c_.src and not p_.fuse_up]
+                prod = [p_ for p_ in blocks if not p_.is_head and p_.y is c_.src and not p_.fuse_up and p_.owner is None]
                 if len(prod) == 1:
                     prod[0].xs_out = c_.xs
                     c_.xs_from_producer = True
@@ -150,20 +172,26 @@ class TrainPlan:
             key = id(c_.gsrc.buf)
             lo, hi = c_.gsrc.ch_off, c_.gsrc.ch_off + c_.gsrc.c
             writers = [r for r in written.get(key, []) if not (r[1] <= lo or hi <= r[0])]
-            prod = [p_ for p_ in blocks if not p_.is_head and p_.gy is c_.gsrc and not p_.fuse_up]
+            prod = [p_ for p_ in blocks if not p_.is_head and p_.gy is c_.gsrc and not p_.fuse_up and p_.owner is None]
             if len(writers) == 1 and len(prod) == 1:
                 prod[0].dy_s2d = c_
                 c_.dxs_direct = True
         self._build_arena()
         # split-K partial sums of every layer's weight gradient in ONE buffer: one fill per step instead of 75
+        # (a weight_from block's wgrad adds into its owner's slot: the owner's gradient sums every use, in backward order)
         off = 0
         for blk in blocks:
-            blk.dw_off = off
-            off += L.round_up(blk.dw_shape[0] * blk.dw_shape[1] * blk.dw_shape[2], 64)
+            if blk.owner is None:
+                blk.dw_off = off
+                off += L.round_up(blk.dw_shape[0] * blk.dw_shape[1] * blk.dw_shape[2], 64)
         self.dw_arena = torch.zeros(off, dtype=torch.float32, device=device)
         for blk in blocks:
-            n_ = blk.dw_shape[0] * blk.dw_shape[1] * blk.dw_shape[2]
-            blk.dw = self.dw_arena[blk.dw_off:blk.dw_off + n_].view(blk.dw_shape)
+            if blk.owner is None:
+                n_ = blk.dw_shape[0] * blk.dw_shape[1] * blk.dw_shape[2]
+                blk.dw = self.dw_arena[blk.dw_off:blk.dw_off + n_].view(blk.dw_shape)
+        for blk in blocks:
+            if blk.owner is not None:
+                blk.dw = blk.owner_blk.dw
         self._key_now = None
         self._multi = None           # job tables of the multi-tensor pack / unpack launches (keyed on parameter storage)
         self.gen = 0                 # forward generation: backward must see the activations of ITS forward
@@ -184,6 +212,11 @@ class TrainPlan:
         bounds = []
         for blk in reversed(self.blocks):
             seq = m.module_list[blk.i]
+            if blk.owner is not None:
+                # the reference never uses a weight_from block's own Conv2d / BatchNorm2d (nor a d-conv's BatchNorm2d):
+                # no slot, autograd receives None for them
+                blk.arena_end = None
+                continue
             if blk.se is not None:         # the SE's backward runs first in this block's backward
                 se = blk.se
                 n = se.c * se.cr
@@ -203,8 +236,11 @@ class TrainPlan:
                     off += L.round_up(blk.cout, 4)
             else:
                 blk.bs_off = off
-                self.param_slots[(blk.i, "BatchNorm2d.bias")] = (off, blk.cout, (blk.cout,))
-                self.param_slots[(blk.i, "BatchNorm2d.weight")] = (off + blk.cout, blk.cout, (blk.cout,))
+                if blk.has_bn:
+                    self.param_slots[(blk.i, "BatchNorm2d.bias")] = (off, blk.cout, (blk.cout,))
+                    self.param_slots[(blk.i, "BatchNorm2d.weight")] = (off + blk.cout, blk.cout, (blk.cout,))
+                elif seq.Conv2d.bias is not None:
+                    self.param_slots[(blk.i, "Conv2d.bias")] = (off, blk.cout, (blk.cout,))
                 if blk.has_act:
                     self.param_slots[(blk.i, "activation.weight")] = (off + 2 * blk.cout, 1, (1,))
                 off += L.round_up(2 * blk.cout + 1, 4)
@@ -212,6 +248,8 @@ class TrainPlan:
             blk.arena_end = off
         self.garena = torch.zeros(off, dtype=torch.float32, device=self.device)
         for blk in self.blocks:
+            if blk.owner is not None:
+                continue
             seq = m.module_list[blk.i]
             n = seq.Conv2d.weight.numel()
             blk.gw = self.garena[blk.gw_off:blk.gw_off + n].view(tuple(seq.Conv2d.weight.shape))
@@ -280,6 +318,8 @@ class TrainPlan:
             return L.round_up(cout, bn_), L.round_up(cin, 64)
         pack = []
         for blk in self.blocks:
+            if blk.owner is not None:
+                continue
             w = m.module_list[blk.i].Conv2d.weight
             if blk.i == 0:
                 cout, cin, ks, mode = blk.cout, 27, 1, 0                       # im2col form: [cout, 27, 1, 1]
@@ -302,6 +342,8 @@ class TrainPlan:
         for seg in self.segments:
             jobs = []
             for blk in seg:
+                if blk.owner is not None:
+                    continue
                 if blk.s2d:
                     jobs.append(_lib.UnpackJob(blk.dw.data_ptr(), blk.gw.data_ptr(), blk.cout_pad, blk.cin_pad, 2, blk.cout,
                                                blk.src.c, 3))
@@ -315,7 +357,7 @@ class TrainPlan:
     def _pack_all(self):
         """every forward AND dgrad weight operand of the step in one launch (the weights are constant within a step)"""
         for b in self.blocks:
-            if self.model.module_list[b.i].Conv2d.weight.dtype != torch.float32:
+            if b.owner is None and self.model.module_list[b.i].Conv2d.weight.dtype != torch.float32:
                 raise RuntimeError("fp32 parameters required")
         raw, prefix, n, total = self._multi_tables()["pack"]
         _lib.check(_lib.lib.ryolo_conv_pack_weights_multi(_lib.ptr(raw), n, _lib.ptr(prefix), total, _lib.stream_ptr(self.device)),
@@ -345,9 +387,9 @@ class TrainPlan:
         bn_counters = []
         for blk in self.blocks:
             seq = m.module_list[blk.i]
-            w = seq.Conv2d.weight.detach()
-            if blk.i == 0:
-                w = w.reshape(blk.cout, 27, 1, 1)
+            if blk.owner is not None and not blk.is_head:
+                self._linear_fwd(blk, st)
+                continue
             x_ptr = blk.src.ptr
             if blk.s2d:
                 if not blk.xs_from_producer:
@@ -357,7 +399,7 @@ class TrainPlan:
             if blk.is_head:
                 if getattr(blk, "bias_pad", None) is None:
                     blk.bias_pad = L.padded_bias(blk.fdesc, torch.zeros(blk.cout, device=self.device))
-                if seq.Conv2d.bias is not None:
+                if seq.Conv2d.bias is not None and blk.owner is None:     # a weight_from head runs without bias
                     blk.bias_pad[:blk.cout].copy_(seq.Conv2d.bias.detach())
                 _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), ctypes.c_void_p(x_ptr), _lib.ptr(blk.pw),
                                                      _lib.ptr(blk.bias_pad), None, _lib.ptr(blk.out), None, 0, st), "conv head")
@@ -373,8 +415,8 @@ class TrainPlan:
                                                        _lib.ptr(blk.scale), _lib.ptr(blk.shift), _lib.ptr(bn.running_mean),
                                                        _lib.ptr(bn.running_var), st), "bn_stats_finalize")
                 bn_counters.append(bn.num_batches_tracked)
-            else:
-                raise NotImplementedError("conv block without BatchNorm that is not a YOLO head")
+            elif seq.Conv2d.bias is not None:
+                blk.shift.copy_(seq.Conv2d.bias.detach())
             xs_out = getattr(blk, "xs_out", None)
             if xs_out is not None:
                 _lib.check(lib.ryolo_bn_act_fwd_s2d(_lib.ptr(blk.z), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout,
@@ -476,6 +518,9 @@ class TrainPlan:
         lib = _lib.lib
         st = _lib.stream_ptr(self.device)
         seq = m.module_list[blk.i]
+        if blk.owner is not None and not blk.is_head:
+            self._linear_bwd(blk, st)
+            return
         if blk.is_head:
             dz = blk.dz
         else:
@@ -487,7 +532,7 @@ class TrainPlan:
             _lib.check(lib.ryolo_bn_act_bwd(ctypes.c_void_p(dy_ptr), dy_cs, dy_mode, _lib.ptr(blk.z),
                                             blk.zcs, self.batch, blk.oh, blk.ow, blk.cout, _lib.ptr(blk.scale),
                                             _lib.ptr(blk.shift), _lib.ptr(blk.mean), _lib.ptr(blk.invstd), blk.slope,
-                                            int(blk.has_act), 1, _lib.ptr(blk.bsums),
+                                            int(blk.has_act), int(blk.has_bn), _lib.ptr(blk.bsums),
                                             ctypes.c_void_p(blk.gres.ptr) if blk.gres is not None else None,
                                             blk.gres.cs if blk.gres is not None else 0, int(blk.gres_acc),
                                             ctypes.c_void_p(blk.slope_dev), st),
@@ -516,6 +561,85 @@ class TrainPlan:
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
                                                  _lib.ptr(self.zero_bias), ctypes.c_void_p(gp) if blk.gsrc_acc else None,
                                                  ctypes.c_void_p(gp), None, 0, st), "dgrad")
+
+    # ---- weight_from blocks (reference models.py:255-265): a linear conv with the owner's weight, no bias / BN / activation.
+    # The forward writes y directly (the conv epilogue, or for a dilated conv the merge, adds the shortcut that follows).
+    # The backward takes dz = dy (and d-shortcut += dy) through bn_act_bwd with has_bn = has_act = 0, then the wgrad adds
+    # into the owner's dw and the dgrad runs on the owner's pwd.  A dilated 3x3 conv (dh, dw) is an ordinary 3x3 conv on
+    # the dh*dw phase images of its input (ryolo_dilate_split); the merge is the split's adjoint, so the backward splits
+    # dz, runs wgrad / dgrad on the phase images and merges dx into the source gradient.
+    def _phase_buf(self, role, nb, h, w, cs):
+        key = (role, nb, h, w, cs)
+        if key not in self.phase:
+            self.phase[key] = L.alloc_padded(nb, h, w, cs, self.device)
+        return self.phase[key]
+
+    def _linear_block(self, blk, batch, device):
+        if blk.fuse_up or blk.se is not None:
+            raise NotImplementedError("weight_from block %d feeding an upsample or an SE" % blk.i)
+        if blk.is_head:
+            return
+        # blk.z holds dz only: the forward writes y directly
+        if blk.dil is None:
+            blk.fdesc = L.make_desc(batch, blk.src.h, blk.src.w, blk.cin, blk.src.cs, blk.cout, blk.y.cs, blk.k, 1, False,
+                                    0.0, blk.res is not None, blk.res.cs if blk.res is not None else 0, False, False)
+            return
+        dh, dw = blk.dil
+        blk.nb, blk.hp, blk.wp = batch * dh * dw, -(-blk.src.h // dh), -(-blk.src.w // dw)
+        blk.xp = L.alloc_padded(blk.nb, blk.hp, blk.wp, blk.cin_pad, device)       # kept for the wgrad
+        blk.zp = self._phase_buf("z", blk.nb, blk.hp, blk.wp, blk.zcs)
+        blk.dxp = self._phase_buf("dx", blk.nb, blk.hp, blk.wp, blk.cin_pad)
+        blk.fdesc = L.make_desc(blk.nb, blk.hp, blk.wp, blk.cin, blk.cin_pad, blk.cout, blk.zcs, 3, 1, False, 0.0)
+        blk.ddesc = L.make_desc(blk.nb, blk.hp, blk.wp, blk.cout, blk.zcs, blk.cin, blk.cin_pad, 3, 1, False, 0.0)
+
+    def _linear_fwd(self, blk, st):
+        lib = _lib.lib
+        if blk.dil is None:
+            _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), ctypes.c_void_p(blk.src.ptr), _lib.ptr(blk.pw),
+                                                 _lib.ptr(self.zero_bias),
+                                                 ctypes.c_void_p(blk.res.ptr) if blk.res is not None else None,
+                                                 ctypes.c_void_p(blk.y.ptr), None, 0, st), "conv (weight_from)")
+            return
+        dh, dw = blk.dil
+        _lib.check(lib.ryolo_dilate_split(ctypes.c_void_p(blk.src.ptr), blk.src.cs, self.batch, blk.src.h, blk.src.w,
+                                          blk.cin, dh, dw, _lib.ptr(blk.xp), blk.cin_pad, st), "dilate_split")
+        _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), _lib.ptr(blk.xp), _lib.ptr(blk.pw),
+                                             _lib.ptr(self.zero_bias), None, _lib.ptr(blk.zp), None, 0, st), "conv (dilated)")
+        _lib.check(lib.ryolo_dilate_merge(_lib.ptr(blk.zp), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout, dh, dw,
+                                          ctypes.c_void_p(blk.res.ptr) if blk.res is not None else None,
+                                          blk.res.cs if blk.res is not None else 0, 0, ctypes.c_void_p(blk.y.ptr), blk.y.cs,
+                                          st), "dilate_merge")
+
+    def _linear_bwd(self, blk, st):
+        lib = _lib.lib
+        _lib.check(lib.ryolo_bn_act_bwd(ctypes.c_void_p(blk.gy.ptr), blk.gy.cs, 0, _lib.ptr(blk.z), blk.zcs, self.batch,
+                                        blk.oh, blk.ow, blk.cout, _lib.ptr(self.zero_bias), _lib.ptr(self.zero_bias),
+                                        _lib.ptr(self.zero_bias), _lib.ptr(self.zero_bias), 0.0, 0, 0,
+                                        _lib.ptr(self.scratch_sums),
+                                        ctypes.c_void_p(blk.gres.ptr) if blk.gres is not None else None,
+                                        blk.gres.cs if blk.gres is not None else 0, int(blk.gres_acc), None, st),
+                   "bn_act_bwd (weight_from)")
+        if blk.dil is None:
+            _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(blk.z), blk.zcs, blk.cout_pad, ctypes.c_void_p(blk.src.ptr), blk.src.cs,
+                                            blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.k, _lib.ptr(blk.dw), st),
+                       "wgrad (weight_from)")
+            gp = blk.gsrc.ptr
+            blk.ddesc.has_residual = int(blk.gsrc_acc)
+            _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(blk.z), _lib.ptr(blk.pwd),
+                                                 _lib.ptr(self.zero_bias), ctypes.c_void_p(gp) if blk.gsrc_acc else None,
+                                                 ctypes.c_void_p(gp), None, 0, st), "dgrad (weight_from)")
+            return
+        dh, dw = blk.dil
+        _lib.check(lib.ryolo_dilate_split(_lib.ptr(blk.z), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout, dh, dw,
+                                          _lib.ptr(blk.zp), blk.zcs, st), "dilate_split (dz)")
+        _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(blk.zp), blk.zcs, blk.cout_pad, _lib.ptr(blk.xp), blk.cin_pad,
+                                        blk.cin_pad, blk.nb, blk.hp, blk.wp, 3, _lib.ptr(blk.dw), st), "wgrad (dilated)")
+        _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(blk.zp), _lib.ptr(blk.pwd),
+                                             _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxp), None, 0, st),
+                   "dgrad (dilated)")
+        _lib.check(lib.ryolo_dilate_merge(_lib.ptr(blk.dxp), blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.cin, dh, dw,
+                                          None, 0, int(blk.gsrc_acc), ctypes.c_void_p(blk.gsrc.ptr), blk.gsrc.cs, st),
+                   "dilate_merge (dx)")
 
     def backward(self, grads):
         m = self.model

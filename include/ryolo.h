@@ -414,6 +414,10 @@ int ryolo_head_grad_to_padded(const float* g, int batch, int na, int no, int ny,
  * C <= 2048. */
 int ryolo_head_grad_nchw_to_padded(const float* g, int batch, int c, int ny, int nx, void* dst,
                                    int dst_cstride, float* bias_grad, void* stream);
+/* The bias gradient alone of the same cotangent: the per-channel sums of g are ADDED to bias_grad ([C] fp32), in the
+ * same order as ryolo_head_grad_nchw_to_padded takes them, so the same bits; g is read once and nothing else is written
+ * (training with the head convolution's weight and everything below it frozen); C <= 2048. */
+int ryolo_head_bias_grad(const float* g, int batch, int c, int ny, int nx, float* bias_grad, void* stream);
 /* Objectness term of compute_loss (reference model/loss.py:340-348: BCEWithLogitsLoss(pos_weight)(pi[..., 5], tobj)
  * over every cell of a head map).  x: logical [batch, na, ny, nx, no] fp32 tensor addressed through `strides` (5 element
  * strides, so both the contiguous tensor and the permuted view of the NCHW head buffer are read in place); ch = the

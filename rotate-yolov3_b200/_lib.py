@@ -82,6 +82,7 @@ SIGNATURES = {
     "ryolo_conv_first_s2d_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),
     "ryolo_head_grad_to_padded": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_head_grad_nchw_to_padded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp]),
+    "ryolo_head_bias_grad": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_loss_rows_gather": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
     "ryolo_loss_rows_scatter_add": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i,
                                          _vp, _vp, _vp]),

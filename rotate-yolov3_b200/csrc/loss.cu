@@ -163,6 +163,8 @@ __device__ __forceinline__ float warp_sum8(const float* v, int lane) {
   return c1;   // value index = 4 * (lane bit 4) + 2 * (lane bit 3) + (lane bit 2)
 }
 
+// STORE = false: the bias sums only (the same loads, warp sums and row partials, so the same bits), no dst traffic
+template <bool STORE>
 __global__ void __launch_bounds__(256) head_grad_nchw_kernel(const float* __restrict__ g, int c, int ny, int nx,
                                                              __nv_bfloat16* __restrict__ dst, int dcs,
                                                              float* __restrict__ bias_partials /*[blocks][c]*/,
@@ -172,7 +174,7 @@ __global__ void __launch_bounds__(256) head_grad_nchw_kernel(const float* __rest
   const int c8 = (c + 7) & ~7;
   const int cpad = c8 + ((c8 >> 3) & 1 ? 0 : 8);                      // pitch = odd multiple of 16 bytes
   __nv_bfloat16* tile = reinterpret_cast<__nv_bfloat16*>(hg_smem);   // [32][cpad]
-  float* s_bias = reinterpret_cast<float*>(hg_smem + (size_t)32 * cpad * 2);   // [c8]: channel ch is owned by one warp
+  float* s_bias = reinterpret_cast<float*>(hg_smem + (STORE ? (size_t)32 * cpad * 2 : 0));   // [c8]: one warp per channel
   const int b = blockIdx.y;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int i = threadIdx.x; i < c8; i += 256) s_bias[i] = 0.f;
@@ -188,15 +190,18 @@ __global__ void __launch_bounds__(256) head_grad_nchw_kernel(const float* __rest
         float v[8];
 #pragma unroll
         for (int e = 0; e < 8; e++) v[e] = (lane < npx && ch0 + e < c) ? __ldg(grow + (size_t)(ch0 + e) * plane + x0 + lane) : 0.f;
-        __nv_bfloat162 h[4];
+        if (STORE) {
+          __nv_bfloat162 h[4];
 #pragma unroll
-        for (int e = 0; e < 4; e++) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
-        *reinterpret_cast<uint4*>(tile + lane * cpad + ch0) = *reinterpret_cast<uint4*>(h);
+          for (int e = 0; e < 4; e++) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+          *reinterpret_cast<uint4*>(tile + lane * cpad + ch0) = *reinterpret_cast<uint4*>(h);
+        }
         if (bias_grad) {
           const float t = warp_sum8(v, lane);
           if ((lane & 3) == 0) s_bias[ch0 + (lane >> 2)] += t;
         }
       }
+      if (!STORE) continue;
       __syncthreads();
       const int chunks = c >> 3;
       for (int idx = threadIdx.x; idx < npx * chunks; idx += 256) {
@@ -212,6 +217,7 @@ __global__ void __launch_bounds__(256) head_grad_nchw_kernel(const float* __rest
       __syncthreads();
     }
   }
+  if (!STORE) __syncthreads();   // s_bias[ch] is written by one warp and read below by another thread
   if (bias_grad)   // this block's row of per-channel sums; ordered_rows_add_kernel adds the rows in a fixed order
     for (int i = threadIdx.x; i < c; i += 256)
       bias_partials[(size_t)(blockIdx.y * gridDim.x + blockIdx.x) * c + i] = s_bias[i];
@@ -384,15 +390,12 @@ extern "C" int ryolo_obj_focal_bwd(const float* x, const long long* strides, int
   return obj_bwd<true>(x, strides, batch, na, ny, nx, no, ch, tobj, pos_weight, gamma, scale_dev, grad, stream_);
 }
 
-extern "C" int ryolo_head_grad_nchw_to_padded(const float* g, int batch, int c, int ny, int nx, void* dst, int dst_cstride,
-                                              float* bias_grad, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  RYOLO_ARG_CHECK(g && dst && batch > 0 && c > 0 && ny > 0 && nx > 0);
-  RYOLO_ARG_CHECK(dst_cstride >= c && dst_cstride % 8 == 0 && batch <= 65535 && c <= 2048);
+// dst null: the bias sums only (head_grad_nchw_kernel<false>, no tile in shared memory); same grid, so the same bits
+static int head_grad_nchw(const float* g, int batch, int c, int ny, int nx, void* dst, int dst_cstride, float* bias_grad,
+                          cudaStream_t stream) {
   const int c8 = (c + 7) & ~7;
   const int cpad = c8 + ((c8 >> 3) & 1 ? 0 : 8);
-  const size_t smem = (size_t)32 * cpad * 2 + (size_t)c8 * sizeof(float);
-  RYOLO_SMEM_OPT_IN(head_grad_nchw_kernel, 160 * 1024);
+  const size_t smem = (dst ? (size_t)32 * cpad * 2 : 0) + (size_t)c8 * sizeof(float);
   // rows per block: keep ~2k blocks in the grid (one row of c bias partials per block)
   int rpb = (int)(((long long)ny * batch + 2047) / 2048);
   if (rpb < 1) rpb = 1;
@@ -403,14 +406,31 @@ extern "C" int ryolo_head_grad_nchw_to_padded(const float* g, int batch, int c, 
     partials = static_cast<float*>(stream_scratch(stream, SCRATCH_LOSS, (size_t)blocks * c * sizeof(float)));
     if (!partials) return RYOLO_E_CUDA;
   }
-  head_grad_nchw_kernel<<<grid, 256, smem, stream>>>(g, c, ny, nx, static_cast<__nv_bfloat16*>(dst), dst_cstride, partials,
-                                                      rpb);
+  if (dst) {
+    RYOLO_SMEM_OPT_IN(head_grad_nchw_kernel<true>, 160 * 1024);
+    head_grad_nchw_kernel<true><<<grid, 256, smem, stream>>>(g, c, ny, nx, static_cast<__nv_bfloat16*>(dst), dst_cstride,
+                                                             partials, rpb);
+  } else {
+    head_grad_nchw_kernel<false><<<grid, 256, smem, stream>>>(g, c, ny, nx, nullptr, 0, partials, rpb);
+  }
   RYOLO_LAUNCH_CHECK();
   if (bias_grad) {
     ordered_rows_add_kernel<<<(c + 31) / 32, 256, 0, stream>>>(partials, blocks, c, bias_grad);
     RYOLO_LAUNCH_CHECK();
   }
   return RYOLO_OK;
+}
+
+extern "C" int ryolo_head_grad_nchw_to_padded(const float* g, int batch, int c, int ny, int nx, void* dst, int dst_cstride,
+                                              float* bias_grad, void* stream_) {
+  RYOLO_ARG_CHECK(g && dst && batch > 0 && c > 0 && ny > 0 && nx > 0);
+  RYOLO_ARG_CHECK(dst_cstride >= c && dst_cstride % 8 == 0 && batch <= 65535 && c <= 2048);
+  return head_grad_nchw(g, batch, c, ny, nx, dst, dst_cstride, bias_grad, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ryolo_head_bias_grad(const float* g, int batch, int c, int ny, int nx, float* bias_grad, void* stream_) {
+  RYOLO_ARG_CHECK(g && bias_grad && batch > 0 && c > 0 && ny > 0 && nx > 0 && batch <= 65535 && c <= 2048);
+  return head_grad_nchw(g, batch, c, ny, nx, nullptr, 0, bias_grad, static_cast<cudaStream_t>(stream_));
 }
 
 static inline RowIdx mk_rows(const long long* b, const long long* a, const long long* gj, const long long* gi,

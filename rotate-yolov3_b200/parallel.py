@@ -58,20 +58,23 @@ class GradBuckets:
     arena ranges of at least ``bucket_bytes`` cut at block boundaries.  ``ready(offset)`` is called by backward when every
     gradient below ``offset`` has been produced: each bucket that became complete is all-reduced asynchronously on a side
     stream (NCCL) -- overlapping the rest of backward -- and ``finish()`` makes the caller's stream wait for all of them.
+    ``ranges`` (default: the whole arena) are the sorted, disjoint parts of the arena that hold trainable parameters'
+    gradients; buckets never leave them, so frozen parameters are not all-reduced (like torch DDP's reducer).
     Device-agnostic (gloo on CPU in the tests: streams are skipped there)."""
 
-    def __init__(self, arena, boundaries, bucket_bytes=32 << 20, group=None):
+    def __init__(self, arena, boundaries, bucket_bytes=32 << 20, group=None, ranges=None):
         self.arena, self.group = arena, group
         self.world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
         cap = max(1, bucket_bytes // arena.element_size())
         self.buckets = []                      # (lo, hi) element ranges
-        lo = 0
-        for b in boundaries:
-            if b - lo >= cap:
-                self.buckets.append((lo, b))
-                lo = b
-        if lo < arena.numel():
-            self.buckets.append((lo, arena.numel()))
+        for r_lo, r_hi in (ranges if ranges is not None else [(0, arena.numel())]):
+            lo = r_lo
+            for b in boundaries:
+                if lo < b < r_hi and b - lo >= cap:
+                    self.buckets.append((lo, b))
+                    lo = b
+            if lo < r_hi:
+                self.buckets.append((lo, r_hi))
         self.cuda = arena.is_cuda
         self.stream = torch.cuda.Stream(device=arena.device) if self.cuda else None
         self.reset()

@@ -11,7 +11,10 @@ through a zero-inserted copy of dz.  The first layer (3 channels) goes through a
 the same kernels.  Activations and activation gradients are bf16 (padded NHWC), parameter gradients fp32.
 
 The whole network is ONE autograd.Function: PyTorch's autograd sees the three head tensors on the outside (so the
-loss stays ordinary PyTorch, reference model/loss.py) and receives the parameter gradients in ``parameters()`` order."""
+loss stays ordinary PyTorch, reference model/loss.py) and receives the parameter gradients in ``parameters()`` order.
+Like stock autograd, the backward follows ``requires_grad``: each trainable mask gets a backward schedule of its own
+(``Schedule``) that runs only the launches whose results reach a trainable parameter (reference train.py:120-135 and
+:215-220 freeze all but the heads, or the backbone)."""
 import ctypes
 
 import torch
@@ -193,7 +196,8 @@ class TrainPlan:
             if blk.owner is not None:
                 blk.dw = blk.owner_blk.dw
         self._key_now = None
-        self._multi = None           # job tables of the multi-tensor pack / unpack launches (keyed on parameter storage)
+        self.schedules = {}          # trainable mask -> Schedule
+        self.sched = self._schedule((True,) * len(self.names))
         self.gen = 0                 # forward generation: backward must see the activations of ITS forward
         self.consumed = True
         self.graphs = None           # CUDA graphs of forward / backward segments (model.use_cuda_graph)
@@ -209,6 +213,7 @@ class TrainPlan:
         m = self.model
         off = 0
         self.param_slots = {}        # (block index, "Module.param") -> (offset, numel, shape)
+        self.pieces = []             # (lo, hi, slot keys): the arena cut into the units a trainable mask keeps or drops
         bounds = []
         for blk in reversed(self.blocks):
             seq = m.module_list[blk.i]
@@ -224,16 +229,19 @@ class TrainPlan:
                 self.param_slots[(se.i, "fc.0.weight")] = (se.gw1_off, n, (se.cr, se.c))
                 self.param_slots[(se.i, "fc.2.weight")] = (se.gw2_off, n, (se.c, se.cr))
                 off += 2 * L.round_up(n, 4)
+                self.pieces.append((se.gw1_off, off, [(se.i, "fc.0.weight"), (se.i, "fc.2.weight")]))
             wshape = tuple(seq.Conv2d.weight.shape)
             n = seq.Conv2d.weight.numel()
             blk.gw_off = off
             self.param_slots[(blk.i, "Conv2d.weight")] = (off, n, wshape)
             off += L.round_up(n, 4)
+            self.pieces.append((blk.gw_off, off, [(blk.i, "Conv2d.weight")]))
             if blk.is_head:
                 if seq.Conv2d.bias is not None:
                     blk.gb_off = off
                     self.param_slots[(blk.i, "Conv2d.bias")] = (off, blk.cout, (blk.cout,))
                     off += L.round_up(blk.cout, 4)
+                    self.pieces.append((blk.gb_off, off, [(blk.i, "Conv2d.bias")]))
             else:
                 blk.bs_off = off
                 if blk.has_bn:
@@ -244,6 +252,9 @@ class TrainPlan:
                 if blk.has_act:
                     self.param_slots[(blk.i, "activation.weight")] = (off + 2 * blk.cout, 1, (1,))
                 off += L.round_up(2 * blk.cout + 1, 4)
+                self.pieces.append((blk.bs_off, off, [k for k in ((blk.i, "BatchNorm2d.bias"), (blk.i, "BatchNorm2d.weight"),
+                                                                  (blk.i, "Conv2d.bias"), (blk.i, "activation.weight"))
+                                                      if k in self.param_slots]))
             bounds.append(off)
             blk.arena_end = off
         self.garena = torch.zeros(off, dtype=torch.float32, device=self.device)
@@ -259,22 +270,25 @@ class TrainPlan:
                 se, n = blk.se, blk.se.c * blk.se.cr
                 se.gw1 = self.garena[se.gw1_off:se.gw1_off + n]
                 se.gw2 = self.garena[se.gw2_off:se.gw2_off + n]
-        ddp = getattr(m, "_ddp", None)
-        from .parallel import GradBuckets
-        self.buckets = GradBuckets(self.garena, bounds, bucket_bytes=ddp["bucket_bytes"] if ddp else (1 << 62),
-                                   group=ddp["group"] if ddp else None) if ddp else None
-        # backward segments = runs of blocks whose gradients complete one bucket (one segment without DDP)
-        segs, cur = [], []
-        ends = set(hi for _, hi in self.buckets.buckets) if self.buckets else set()
-        for blk in reversed(self.blocks):
-            cur.append(blk)
-            if blk.arena_end in ends:
-                segs.append(cur)
-                cur = []
-        if cur:
-            segs.append(cur)
-        self.segments = segs
+        self.bounds = bounds
         self.names = [nm for nm, _ in m.named_parameters()]
+
+    @property
+    def buckets(self):
+        """the all-reduce buckets of the current step's schedule (None without DDP)"""
+        return self.sched.buckets
+
+    @property
+    def segments(self):
+        return self.sched.segments
+
+    def _schedule(self, mask):
+        """the Schedule of `mask` (requires_grad of every parameter, in parameters() order), derived once and cached:
+        changing requires_grad between steps selects another schedule and rebuilds nothing else"""
+        sch = self.schedules.get(mask)
+        if sch is None:
+            sch = self.schedules[mask] = Schedule(self, mask)
+        return sch
 
     # ------------------------------------------------------------------------------------------------------
     def _slopes(self):
@@ -296,6 +310,8 @@ class TrainPlan:
 
     # ---- multi-tensor pack / unpack (csrc/multi.cu): job tables in device memory, rebuilt when parameter storage moves ----
     def _job_table(self, jobs, cls):
+        if not jobs:
+            return None, None, 0, 0
         arr = (cls * len(jobs))(*jobs)
         raw = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.device)
         sizes = []
@@ -309,8 +325,9 @@ class TrainPlan:
 
     def _multi_tables(self):
         key = self._key_now if self._key_now is not None else self._param_key()
-        if self._multi is not None and self._multi["key"] == key:
-            return self._multi
+        sch = self.sched
+        if sch.multi is not None and sch.multi["key"] == key:
+            return sch.multi
         m = self.model
 
         def pads(cout, cin):
@@ -330,7 +347,7 @@ class TrainPlan:
             cp, kp = pads(cout, cin)
             assert blk.pw.numel() == ks * ks * cp * kp * 2, (blk.i, blk.pw.numel(), ks, cp, kp)
             pack.append(_lib.PackJob(w.data_ptr(), blk.pw.data_ptr(), cout, cin, ks, cp, kp, mode))
-            if blk.i > 0:                                                        # dgrad operand: mirrored taps, transposed
+            if blk.i in sch.pwd_used:                                            # dgrad operand: mirrored taps, transposed
                 if blk.s2d:
                     cout_d, cin_d, ks_d, mode_d = blk.cin_eff, blk.cout, 2, 3
                 else:
@@ -339,10 +356,10 @@ class TrainPlan:
                 assert blk.pwd.numel() == ks_d * ks_d * cpd * kpd * 2, (blk.i, blk.pwd.numel(), ks_d, cpd, kpd)
                 pack.append(_lib.PackJob(w.data_ptr(), blk.pwd.data_ptr(), cout_d, cin_d, ks_d, cpd, kpd, mode_d))
         unpack = []
-        for seg in self.segments:
+        for seg in sch.segments:
             jobs = []
             for blk in seg:
-                if blk.owner is not None:
+                if blk.owner is not None or "wgrad" not in sch.run[blk.i]:
                     continue
                 if blk.s2d:
                     jobs.append(_lib.UnpackJob(blk.dw.data_ptr(), blk.gw.data_ptr(), blk.cout_pad, blk.cin_pad, 2, blk.cout,
@@ -351,11 +368,12 @@ class TrainPlan:
                     jobs.append(_lib.UnpackJob(blk.dw.data_ptr(), blk.gw.data_ptr(), blk.cout_pad, blk.cin_pad, 0, blk.cout,
                                                blk.cin, blk.k_eff))
             unpack.append(self._job_table(jobs, _lib.UnpackJob))
-        self._multi = {"key": key, "pack": self._job_table(pack, _lib.PackJob), "unpack": unpack}
-        return self._multi
+        sch.multi = {"key": key, "pack": self._job_table(pack, _lib.PackJob), "unpack": unpack}
+        return sch.multi
 
     def _pack_all(self):
-        """every forward AND dgrad weight operand of the step in one launch (the weights are constant within a step)"""
+        """every forward and every running dgrad's weight operand of the step in one launch (the weights are constant
+        within a step)"""
         for b in self.blocks:
             if b.owner is None and self.model.module_list[b.i].Conv2d.weight.dtype != torch.float32:
                 raise RuntimeError("fp32 parameters required")
@@ -365,12 +383,14 @@ class TrainPlan:
 
     def _backward_segment(self, si):
         if si == 0:
-            self.dw_arena.zero_()
-        for blk in self.segments[si]:
+            for lo, hi in self.sched.dw_ranges:
+                self.dw_arena[lo:hi].zero_()
+        for blk in self.sched.segments[si]:
             self._backward_block(blk)
         raw, prefix, n, total = self._multi_tables()["unpack"][si]
-        _lib.check(_lib.lib.ryolo_conv_unpack_wgrad_multi(_lib.ptr(raw), n, _lib.ptr(prefix), total,
-                                                          _lib.stream_ptr(self.device)), "unpack_wgrad_multi")
+        if n:
+            _lib.check(_lib.lib.ryolo_conv_unpack_wgrad_multi(_lib.ptr(raw), n, _lib.ptr(prefix), total,
+                                                              _lib.stream_ptr(self.device)), "unpack_wgrad_multi")
 
     def _forward_body(self, x):
         m = self.model
@@ -440,8 +460,10 @@ class TrainPlan:
         # ([B, na, ny, nx, no] like model/models.py:190-192, without the .contiguous() copy of 0.5 GB per step)
         return [blk.out for blk in self.heads]
 
-    def forward(self, x):
+    def forward(self, x, mask=None):
+        """mask: requires_grad of every parameter in parameters() order (None: all); selects the backward schedule"""
         m = self.model
+        self.sched = self._schedule(tuple(mask) if mask is not None else (True,) * len(self.names))
         self.heads = [b for b in self.blocks if b.is_head]
         for blk, yi in zip(self.heads, m.yolo_layers):
             layer = m.module_list[yi]
@@ -461,7 +483,7 @@ class TrainPlan:
     # rank) is the host, not the GPU.  Inputs are copied into static buffers; outputs are static buffers that the next
     # step overwrites (standard CUDA-graph semantics).
     def _forward_graph(self, x):
-        key = self._key_now
+        key = (self._key_now, self.sched.mask)     # the pack table and the backward segments depend on the schedule
         if self.graphs is None or self.graphs["key"] != key:
             self.graphs = {"key": key, "pool": None}
             self.x_static = x.clone()
@@ -489,10 +511,17 @@ class TrainPlan:
         lib = _lib.lib
         st = _lib.stream_ptr(self.device)
         for blk, g in zip(self.heads, grads):
+            run = self.sched.run[blk.i]
+            if not run & {"head", "head_bias"}:
+                continue
             g = g.contiguous().float()
             gb = self.garena[blk.gb_off:blk.gb_off + blk.cout] if (blk.i, "Conv2d.bias") in self.param_slots else None
             if gb is not None:       # the bias gradient = per-channel sums of g, taken on the way by the same kernel
                 gb.zero_()
+            if "head_bias" in run:   # only the bias trains: its sums alone, the same bits
+                _lib.check(lib.ryolo_head_bias_grad(_lib.ptr(g), self.batch, blk.cout, blk.oh, blk.ow, _lib.ptr(gb), st),
+                           "head_bias_grad")
+                continue
             _lib.check(lib.ryolo_head_grad_nchw_to_padded(_lib.ptr(g), self.batch, blk.cout, blk.oh, blk.ow, _lib.ptr(blk.dz),
                                                           blk.zcs, _lib.ptr(gb) if gb is not None else None, st),
                        "head_grad_nchw_to_padded")
@@ -518,14 +547,17 @@ class TrainPlan:
         lib = _lib.lib
         st = _lib.stream_ptr(self.device)
         seq = m.module_list[blk.i]
+        run = self.sched.run[blk.i]
         if blk.owner is not None and not blk.is_head:
-            self._linear_bwd(blk, st)
+            self._linear_bwd(blk, run, st)
             return
         if blk.is_head:
             dz = blk.dz
         else:
-            if blk.se is not None:
+            if "se" in run:
                 self._se_bwd(blk.se, st)
+            if "bnact" not in run:
+                return
             src_c = getattr(blk, "dy_s2d", None)
             dy_ptr, dy_cs, dy_mode = (blk.gy.ptr, blk.gy.cs, int(blk.fuse_up)) if src_c is None else \
                 (src_c.dxs.data_ptr(), src_c.xs_cs, 2)
@@ -538,24 +570,30 @@ class TrainPlan:
                                             ctypes.c_void_p(blk.slope_dev), st),
                        "bn_act_bwd")
             dz = blk.z
+        wgrad, dgrad = "wgrad" in run, "dgrad" in run
         if blk.s2d:
-            _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(dz), blk.zcs, blk.cout_pad, _lib.ptr(blk.xs), blk.xs_cs,
-                                            blk.cin_pad, self.batch, blk.src.h // 2, blk.src.w // 2, 2, _lib.ptr(blk.dw),
-                                            st), "wgrad s2d")
-            _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
-                                                 _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxs), None, 0, st), "dgrad s2d")
-            if not blk.dxs_direct:
-                _lib.check(lib.ryolo_depth_to_space(_lib.ptr(blk.dxs), blk.xs_cs, self.batch, blk.src.h, blk.src.w, blk.src.c,
-                                                    ctypes.c_void_p(blk.gsrc.ptr), blk.gsrc.cs, int(blk.gsrc_acc), st), "d2s")
+            if wgrad:
+                _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(dz), blk.zcs, blk.cout_pad, _lib.ptr(blk.xs), blk.xs_cs,
+                                                blk.cin_pad, self.batch, blk.src.h // 2, blk.src.w // 2, 2, _lib.ptr(blk.dw),
+                                                st), "wgrad s2d")
+            if dgrad:
+                _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
+                                                     _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxs), None, 0, st),
+                           "dgrad s2d")
+                if not blk.dxs_direct:
+                    _lib.check(lib.ryolo_depth_to_space(_lib.ptr(blk.dxs), blk.xs_cs, self.batch, blk.src.h, blk.src.w,
+                                                        blk.src.c, ctypes.c_void_p(blk.gsrc.ptr), blk.gsrc.cs,
+                                                        int(blk.gsrc_acc), st), "d2s")
             return
-        if blk.stride == 2:
+        if blk.stride == 2 and (wgrad or dgrad):
             _lib.check(lib.ryolo_zero_insert2x(_lib.ptr(dz), blk.zcs, self.batch, blk.oh, blk.ow, blk.zcs,
                                                _lib.ptr(blk.dz_up), blk.zcs, blk.src.h, blk.src.w, st), "zero_insert")
             dz = blk.dz_up
-        _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(dz), blk.zcs, blk.cout_pad, ctypes.c_void_p(blk.src.ptr), blk.src.cs,
-                                        blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.k_eff, _lib.ptr(blk.dw), st),
-                   "wgrad")
-        if blk.i > 0:
+        if wgrad:
+            _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(dz), blk.zcs, blk.cout_pad, ctypes.c_void_p(blk.src.ptr), blk.src.cs,
+                                            blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.k_eff, _lib.ptr(blk.dw), st),
+                       "wgrad")
+        if dgrad:
             gp = blk.gsrc.ptr
             blk.ddesc.has_residual = int(blk.gsrc_acc)
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
@@ -610,8 +648,10 @@ class TrainPlan:
                                           blk.res.cs if blk.res is not None else 0, 0, ctypes.c_void_p(blk.y.ptr), blk.y.cs,
                                           st), "dilate_merge")
 
-    def _linear_bwd(self, blk, st):
+    def _linear_bwd(self, blk, run, st):
         lib = _lib.lib
+        if "bnact" not in run:
+            return
         _lib.check(lib.ryolo_bn_act_bwd(ctypes.c_void_p(blk.gy.ptr), blk.gy.cs, 0, _lib.ptr(blk.z), blk.zcs, self.batch,
                                         blk.oh, blk.ow, blk.cout, _lib.ptr(self.zero_bias), _lib.ptr(self.zero_bias),
                                         _lib.ptr(self.zero_bias), _lib.ptr(self.zero_bias), 0.0, 0, 0,
@@ -619,10 +659,14 @@ class TrainPlan:
                                         ctypes.c_void_p(blk.gres.ptr) if blk.gres is not None else None,
                                         blk.gres.cs if blk.gres is not None else 0, int(blk.gres_acc), None, st),
                    "bn_act_bwd (weight_from)")
+        wgrad, dgrad = "wgrad" in run, "dgrad" in run
         if blk.dil is None:
-            _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(blk.z), blk.zcs, blk.cout_pad, ctypes.c_void_p(blk.src.ptr), blk.src.cs,
-                                            blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.k, _lib.ptr(blk.dw), st),
-                       "wgrad (weight_from)")
+            if wgrad:
+                _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(blk.z), blk.zcs, blk.cout_pad, ctypes.c_void_p(blk.src.ptr),
+                                                blk.src.cs, blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.k,
+                                                _lib.ptr(blk.dw), st), "wgrad (weight_from)")
+            if not dgrad:
+                return
             gp = blk.gsrc.ptr
             blk.ddesc.has_residual = int(blk.gsrc_acc)
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(blk.z), _lib.ptr(blk.pwd),
@@ -630,10 +674,15 @@ class TrainPlan:
                                                  ctypes.c_void_p(gp), None, 0, st), "dgrad (weight_from)")
             return
         dh, dw = blk.dil
+        if not (wgrad or dgrad):
+            return
         _lib.check(lib.ryolo_dilate_split(_lib.ptr(blk.z), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout, dh, dw,
                                           _lib.ptr(blk.zp), blk.zcs, st), "dilate_split (dz)")
-        _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(blk.zp), blk.zcs, blk.cout_pad, _lib.ptr(blk.xp), blk.cin_pad,
-                                        blk.cin_pad, blk.nb, blk.hp, blk.wp, 3, _lib.ptr(blk.dw), st), "wgrad (dilated)")
+        if wgrad:
+            _lib.check(lib.ryolo_conv_wgrad(_lib.ptr(blk.zp), blk.zcs, blk.cout_pad, _lib.ptr(blk.xp), blk.cin_pad,
+                                            blk.cin_pad, blk.nb, blk.hp, blk.wp, 3, _lib.ptr(blk.dw), st), "wgrad (dilated)")
+        if not dgrad:
+            return
         _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(blk.zp), _lib.ptr(blk.pwd),
                                              _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxp), None, 0, st),
                    "dgrad (dilated)")
@@ -656,19 +705,24 @@ class TrainPlan:
 
     def _backward(self, grads):
         m = self.model
+        sch = self.sched
         self._head_grads(grads)
         use_graph = getattr(m, "use_cuda_graph", False) and self.graphs is not None and "fwd" in self.graphs
         if use_graph and "bwd" not in self.graphs:
             # first backward after capture of the forward: run eagerly once (warm-up), then capture every segment
-            for si, seg in enumerate(self.segments):
+            for si in range(len(sch.segments)):
                 self._backward_segment(si)
-                if self.buckets:
-                    self.buckets.ready(seg[-1].arena_end)
-            inv = self.buckets.finish() if self.buckets else 1.0
-            out_flat = self.garena * inv
+                if sch.buckets:
+                    sch.buckets.ready(sch.ready[si])
+            inv = sch.buckets.finish() if sch.buckets else 1.0
+            outs = [self.garena[lo:hi] * inv for lo, hi in sch.ranges]
             torch.cuda.synchronize(self.device)
             gs, gk = [], []
-            for si in range(len(self.segments)):
+            for si in range(len(sch.segments)):
+                if not sch.busy[si]:          # nothing to launch: no graph (an empty capture is an error)
+                    gs.append(None)
+                    gk.append(0)
+                    continue
                 g = torch.cuda.CUDAGraph()
                 c0 = _lib.lib.ryolo_launch_count()
                 with torch.cuda.graph(g, pool=self.graphs["pool"]):
@@ -679,29 +733,187 @@ class TrainPlan:
             self.graphs["bwd"] = gs
             # the capture passes did not execute; the eager pass above produced this step's gradients
         else:
-            for si, seg in enumerate(self.segments):
-                if use_graph:
+            for si in range(len(sch.segments)):
+                if not use_graph:
+                    self._backward_segment(si)
+                elif self.graphs["bwd"][si] is not None:
                     self.graphs["bwd"][si].replay()
                     self.replayed_kernels += self.graphs["bwd_kernels"][si]
-                else:
-                    self._backward_segment(si)
-                if self.buckets:
-                    self.buckets.ready(seg[-1].arena_end)     # NCCL all-reduce of the finished bucket on the side stream
+                if sch.buckets:
+                    sch.buckets.ready(sch.ready[si])     # NCCL all-reduce of the finished bucket on the side stream
             if self.time_comm:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
-            inv = self.buckets.finish() if self.buckets else 1.0
+            inv = sch.buckets.finish() if sch.buckets else 1.0
             if self.time_comm:
                 e1.record()
                 self._comm_ev = (e0, e1)
-            out_flat = self.garena * inv                       # fresh tensor: autograd may keep what it is given
+            # fresh tensors, trainable ranges only: autograd may keep what it is given
+            outs = [self.garena[lo:hi] * inv for lo, hi in sch.ranges]
         self.consumed = True
         out = []
         for name in self.names:
             parts = name.split(".")            # module_list.{i}.{Module}.{param} (SE: module_list.{i}.fc.{0|2}.weight)
-            slot = self.param_slots.get((int(parts[1]), ".".join(parts[2:])))
-            out.append(out_flat[slot[0]:slot[0] + slot[1]].view(slot[2]) if slot is not None else None)
+            key = (int(parts[1]), ".".join(parts[2:]))
+            slot = self.param_slots.get(key) if key in sch.trainable else None
+            if slot is None:
+                out.append(None)
+                continue
+            r = sch.range_of[key]
+            lo = slot[0] - sch.ranges[r][0]
+            out.append(outs[r][lo:lo + slot[1]].view(slot[2]))
         return out
+
+
+class Schedule:
+    """The backward of one trainable mask: which launches run, the arena ranges autograd and the all-reduce see, the
+    segments and buckets.  Derived over the data edges of the plan (concat views, shortcuts, the fused upsamples, SE
+    nodes and weight_from uses):
+
+      up(t)      the tensor t depends on a trainable parameter (a forward walk; a view reads every range it overlaps)
+      out(b)     = trainable(b) or up(b.src) or up(b.res): b's output gradient is needed, so bn_act_bwd runs
+      se_bwd     iff an fc weight trains or out(b) (its gu is needed)
+      wgrad      iff the conv weight trains (a weight_from block: its owner's weight, every use adds into the owner's dw)
+      dgrad      iff up(b.src) (with its zero-insert / depth_to_space / dilate merge; split and zero-insert also serve wgrad)
+      heads      dz iff the weight trains or up(src); otherwise the bias sums alone when the bias trains
+
+    A gradient range is needed iff up(its tensor): every writer of a needed range then runs, in the order of the full
+    plan, so the static accumulate flags stay right.  That is asserted, by the same first-writer walk that set them.  With
+    every parameter trainable the schedule is the full plan, launch for launch."""
+
+    def __init__(self, plan, mask):
+        if len(mask) != len(plan.names):
+            raise ValueError("trainable mask of %d entries for %d parameters" % (len(mask), len(plan.names)))
+        self.mask = mask
+        self.multi = None        # job tables of the multi-tensor pack / unpack launches (keyed on parameter storage)
+        tr = set()
+        for name, t in zip(plan.names, mask):
+            parts = name.split(".")
+            if t:
+                tr.add((int(parts[1]), ".".join(parts[2:])))
+        self.trainable = tr
+        blocks = plan.blocks
+        ups = {}                 # buffer id -> [(lo, hi, up)] of the ranges written by the forward so far
+
+        def up(v):
+            if v is None or v.buf is None:
+                return False
+            lo, hi = v.ch_off, v.ch_off + v.c
+            return any(u for a, b, u in ups.get(id(v.buf), []) if a < hi and lo < b)
+
+        def record(v, u):
+            ups.setdefault(id(v.buf), []).append((v.ch_off, v.ch_off + v.c, u))
+
+        run = self.run = {}
+        for b in blocks:
+            wi = b.owner if b.owner is not None else b.i
+            tw = (wi, "Conv2d.weight") in tr
+            up_src = b.i > 0 and up(b.src)
+            r = set()
+            if b.is_head:
+                if tw or up_src:
+                    r.add("head")
+                elif (b.i, "Conv2d.bias") in tr and (b.i, "Conv2d.bias") in plan.param_slots:
+                    r.add("head_bias")
+            else:
+                tp = b.owner is None and any((b.i, k) in tr for k in ("BatchNorm2d.bias", "BatchNorm2d.weight",
+                                                                     "Conv2d.bias", "activation.weight"))
+                out = tw or tp or up_src or (b.res is not None and up(b.res))
+                if out:
+                    r.add("bnact")
+                record(b.y, out)
+                if b.se is not None:
+                    up_u = out or any((b.se.i, k) in tr for k in ("fc.0.weight", "fc.2.weight"))
+                    if up_u:
+                        r.add("se")
+                    record(b.se.u, up_u)
+            if tw:
+                r.add("wgrad")
+            if up_src:
+                r.add("dgrad")
+            run[b.i] = frozenset(r)
+
+        # the invariant: every writer of a needed gradient range runs, and the first-writer walk over the writers that
+        # run gives each of them its full-plan accumulate flag
+        written = {}
+        for b in reversed(blocks):
+            r = run[b.i]
+            for kind, v, flag in (("se", b.se.gx if b.se is not None else None, getattr(b.se, "gx_acc", None)),
+                                  ("bnact", b.gres, b.gres_acc), ("dgrad", b.gsrc, b.gsrc_acc)):
+                if v is None:
+                    continue
+                assert kind in r or not up(v), ("writer of a needed gradient range pruned", kind, b.i)
+                if kind in r:
+                    acc = G.claim(written, v)
+                    assert acc == flag or not up(v), ("accumulate flag differs from the full plan", kind, b.i)
+            p_ = getattr(b, "dy_s2d", None)
+            assert p_ is None or "bnact" not in r or "dgrad" in run[p_.i], ("dy read from a pruned dgrad", b.i)
+        self.pwd_used = set()        # owners whose packed dgrad operand some running dgrad reads
+        for b in blocks:
+            if "dgrad" in run[b.i]:
+                self.pwd_used.add(b.owner if b.owner is not None else b.i)
+        self.dw_ranges = _merge([(b.dw_off, b.dw_off + L.round_up(b.dw.numel(), 64)) for b in blocks
+                                 if b.owner is None and "wgrad" in run[b.i]])
+
+        # arena ranges autograd receives and the all-reduce covers: the pieces holding a trainable parameter
+        self.ranges = _merge([(lo, hi) for lo, hi, keys in plan.pieces if any(k in tr for k in keys)])
+        self.range_of = {}
+        for lo, hi, keys in plan.pieces:
+            for k in keys:
+                if k in tr:
+                    self.range_of[k] = next(j for j, (a, b_) in enumerate(self.ranges) if a <= lo and hi <= b_)
+        ddp = getattr(plan.model, "_ddp", None)
+        from .parallel import GradBuckets
+        self.buckets = GradBuckets(plan.garena, plan.bounds, bucket_bytes=ddp["bucket_bytes"], group=ddp["group"],
+                                   ranges=self.ranges) if ddp else None
+        # backward segments = runs of blocks whose gradients complete one bucket (one segment without DDP); ready[s] is
+        # the arena offset below which every gradient is final after segment s
+        ends = sorted(hi for _, hi in self.buckets.buckets) if self.buckets else []
+        segs, cur, self.ready, k = [], [], [], 0
+        for b in reversed(blocks):
+            cur.append(b)
+            if b.arena_end is not None and k < len(ends) and ends[k] <= b.arena_end:
+                while k < len(ends) and ends[k] <= b.arena_end:
+                    k += 1
+                segs.append(cur)
+                self.ready.append(b.arena_end)
+                cur = []
+        if cur:
+            segs.append(cur)
+            self.ready.append(plan.garena.numel())
+        self.segments = segs
+        self.busy = [bool((si == 0 and self.dw_ranges) or any(run[b.i] - {"head", "head_bias"} for b in seg))
+                     for si, seg in enumerate(segs)]
+
+    def ops(self, plan):
+        """the launches of the backward in order, as (kind, layer, accumulate flag or None): what the tests compare"""
+        out = []
+        for b in plan.blocks:
+            if b.is_head:
+                out += [(k, b.i, None) for k in ("head", "head_bias") if k in self.run[b.i]]
+        for seg in self.segments:
+            for b in seg:
+                r = self.run[b.i]
+                if "se" in r:
+                    out.append(("se", b.se.i, b.se.gx_acc))
+                if "bnact" in r:
+                    out.append(("bnact", b.i, b.gres_acc if b.gres is not None else None))
+                if "wgrad" in r:
+                    out.append(("wgrad", b.i, None))
+                if "dgrad" in r:
+                    out.append(("dgrad", b.i, (b.gsrc_acc, b.dxs_direct)))
+        return out
+
+
+def _merge(ranges):
+    """sorted, touching ranges joined"""
+    out = []
+    for lo, hi in sorted(ranges):
+        if out and out[-1][1] == lo:
+            out[-1] = (out[-1][0], hi)
+        else:
+            out.append((lo, hi))
+    return out
 
 
 def _comm_wait_ms(self):
@@ -730,7 +942,7 @@ class DarknetTrainFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, plan, x, *params):
         ctx.plan = plan
-        outs = plan.forward(x)
+        outs = plan.forward(x, ctx.needs_input_grad[2:])
         ctx.gen = plan.gen
         return tuple(outs)
 

@@ -235,17 +235,15 @@ typedef struct ryolo_conv_desc {
 
 /* Pack reference-layout weights [cout, cin, k, k] fp32 (nn.Conv2d.weight), times an optional
  * per-filter scale (folded BN: gamma / sqrt(var + eps)), into the bf16 GEMM operand
- * [k*k][cout_pad][cin_pad] (zero padded).  Device pointers. */
-size_t ryolo_conv_packed_weight_bytes(const ryolo_conv_desc* d);
-int ryolo_conv_pack_weights(const ryolo_conv_desc* d, const float* weight, const float* scale,
-                            void* packed_out, void* stream);
-/* Same with the operand transform done in the packing kernel (no framework-side flips / transposes / gathers):
- * mode 0 = plain; 1 = dgrad operand of a plain conv (`weight` is the FORWARD weight, `d` the dgrad
- * descriptor: taps mirrored, matrix transposed); 2 = space-to-depth form of a 3x3/stride-2 conv
+ * [k*k][cout_pad][cin_pad] (zero padded).  Device pointers.  The operand transform is done in the
+ * packing kernel (no framework-side flips / transposes / gathers): mode 0 = plain; 1 = dgrad operand
+ * of a plain conv (`weight` is the FORWARD weight, `d` the dgrad descriptor: taps mirrored, matrix
+ * transposed); 2 = space-to-depth form of a 3x3/stride-2 conv
  * (`weight` [cout, C, 3, 3], d->cin = 4C, d->ksize = 2); 3 = dgrad operand of mode 2 (d->cout = 4C,
  * d->ksize = -2).  ryolo_conv_unpack_wgrad is the inverse gather for weight GRADIENTS: wgrad output
  * [taps][cout_pad][cin_pad] -> nn.Conv2d layout [cout][cin][k][k] (mode 0) or, from the
  * space-to-depth form, [cout][C][3][3] (mode 2, cin = C). */
+size_t ryolo_conv_packed_weight_bytes(const ryolo_conv_desc* d);
 int ryolo_conv_pack_weights_ex(const ryolo_conv_desc* d, const float* weight, const float* scale,
                                void* packed_out, int mode, void* stream);
 int ryolo_conv_unpack_wgrad(const float* dw, int cout_pad, int cin_pad, int mode, int cout, int cin,
@@ -270,11 +268,10 @@ int ryolo_conv_pack_weights_multi(const ryolo_pack_job* jobs_dev, int njobs, con
                                   long long total, void* stream);
 int ryolo_conv_unpack_wgrad_multi(const ryolo_unpack_job* jobs_dev, int njobs, const long long* prefix_dev,
                                   long long total, void* stream);
-/* y = act(conv(x, W') + bias) [+ residual].  bias: fp32 [cout_pad] (zero beyond cout). */
-size_t ryolo_conv_workspace_bytes(const ryolo_conv_desc* d);
+/* y = act(conv(x, W') + bias) [+ residual].  bias: fp32 [cout_pad] (zero beyond cout).  The implicit
+ * GEMM needs no scratch memory. */
 int ryolo_conv_bn_act_fwd(const ryolo_conv_desc* d, const void* x, const void* packed_w,
-                          const float* bias, const void* residual, void* y, void* workspace,
-                          size_t workspace_bytes, void* stream);
+                          const float* bias, const void* residual, void* y, void* stream);
 /* First layer (cin = 3, 3x3, stride 1; reference model/models.py:45-74 block 0): fp32 NCHW image
  * [B,3,H,W] -> bf16 padded NHWC with channel stride cout_stride (channels >= cout zero-filled).
  * weight [cout,3,3,3] fp32 with BN folded (rounded to bf16 in the kernel like every other layer's
@@ -303,22 +300,14 @@ int ryolo_conv_wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x
                      int cin_pad, int batch, int in_h, int in_w, int ksize, float* dw, void* stream);
 
 /* Per-channel batch statistics of a raw conv output z (padded NHWC bf16, interior pixels):
- * sums[0..c) = sum z, sums[c..2c) = sum z^2 (fp32; zeroed inside). */
-int ryolo_bn_stats(const void* z, int z_cstride, int batch, int h, int w, int c, float* sums,
-                   void* stream);
-/* sums -> per-channel mean, invstd, scale = gamma*invstd, shift = beta - mean*scale, and (when the
- * pointers are non-null) the nn.BatchNorm2d running statistics update with momentum and the
- * unbiased variance (reference model/models.py:62: momentum 0.1, eps 1e-5). */
-/* ryolo_bn_stats + ryolo_bn_finalize in one call: when z's rows are contiguous (z_cstride == c) the last CTA of the
- * statistics kernel to finish finalises (one launch per block instead of two); otherwise the two kernels run back to
- * back.  sums: [2*c + 1] fp32 scratch (zeroed by the call; the extra word is the CTA ticket). */
+ * sums[0..c) = sum z, sums[c..2c) = sum z^2 (fp32), and from them the per-channel mean, invstd,
+ * scale = gamma*invstd, shift = beta - mean*scale and (when the pointers are non-null) the
+ * nn.BatchNorm2d running statistics update with momentum and the unbiased variance (reference
+ * model/models.py:62: momentum 0.1, eps 1e-5).  The sums are reduced in a fixed order and the
+ * finalisation is fused into that reduction. */
 int ryolo_bn_stats_finalize(const void* z, int z_cstride, int batch, int h, int w, int c, float* sums, float eps,
                             float momentum, const float* gamma, const float* beta, float* mean, float* invstd,
                             float* scale, float* shift, float* running_mean, float* running_var, void* stream);
-int ryolo_bn_finalize(const float* sums, int c, float count, float eps, float momentum,
-                      const float* gamma, const float* beta, float* mean, float* invstd,
-                      float* scale, float* shift, float* running_mean, float* running_var,
-                      void* stream);
 /* y = prelu(z * scale + shift) [+ residual], scale/shift = folded batch-stat BN (gamma*invstd,
  * beta - mean*gamma*invstd); upsample2x writes every pixel to its 2x2 block of a 2h x 2w y. */
 int ryolo_bn_act_fwd(const void* z, int z_cstride, int batch, int h, int w, int c,
@@ -400,15 +389,8 @@ int ryolo_se_bwd(const void* gu, int gu_cstride, const void* x, int x_cstride, v
  * nn.ZeroPad2d((0,1,0,1)) + MaxPool2d(2, 1). */
 int ryolo_maxpool2x2(const void* x, int x_cstride, int batch, int in_h, int in_w, int c, int stride,
                      void* y, int y_cstride, void* stream);
-/* fp32 NCHW [B,C,H,W] -> bf16 padded NHWC interior, channels [0,C) (head gradients). */
-int ryolo_nchw_to_padded(const float* src, int batch, int c, int h, int w, void* dst,
-                         int dst_cstride, void* stream);
-/* Gradient of a YOLO head in the layout autograd delivers it, fp32 [B, na, ny, nx, no] (training-mode
- * head output, reference model/models.py:190-192), -> bf16 padded NHWC [B, ny+2, nx+2, dst_cstride]
- * with channel = a*no + k (the head conv's filter index); channels >= na*no are left untouched. */
-int ryolo_head_grad_to_padded(const float* g, int batch, int na, int no, int ny, int nx, void* dst,
-                              int dst_cstride, void* stream);
-/* Same, for the cotangent in the layout the head convolution WROTE its output in: fp32 NCHW [B, C = na*no, ny, nx]
+/* Gradient of a YOLO head -> bf16 padded NHWC [B, ny+2, nx+2, dst_cstride], channels >= C and the halo left
+ * untouched.  The cotangent is in the layout the head convolution WROTE its output in: fp32 NCHW [B, C = na*no, ny, nx]
  * (what arrives when the consumer differentiates the permuted VIEW of that buffer, e.g. the fused loss below).
  * bias_grad (nullable): [C] fp32, the per-channel sums of g are ADDED to it (the head convolution's bias gradient);
  * C <= 2048. */

@@ -71,16 +71,13 @@ SIGNATURES = {
     "ryolo_nms_filter": (_i, [_vp, _i, _i, _f, _f, _vp, _i, _vp, _vp, _sz, _vp]),
     "ryolo_yolo_decode": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _f, _f, _i, _vp, _i, _i, _vp, _vp]),
     "ryolo_conv_packed_weight_bytes": (_sz, [ctypes.POINTER(ConvDesc)]),
-    "ryolo_conv_pack_weights": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp]),
     "ryolo_conv_pack_weights_ex": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _i, _vp]),
     "ryolo_conv_unpack_wgrad": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_conv_pack_weights_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_conv_unpack_wgrad_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
-    "ryolo_conv_workspace_bytes": (_sz, [ctypes.POINTER(ConvDesc)]),
-    "ryolo_conv_bn_act_fwd": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "ryolo_conv_bn_act_fwd": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_conv_first_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),
     "ryolo_conv_first_s2d_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),
-    "ryolo_head_grad_to_padded": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_head_grad_nchw_to_padded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp]),
     "ryolo_head_bias_grad": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_loss_rows_gather": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
@@ -92,9 +89,7 @@ SIGNATURES = {
     "ryolo_obj_focal_fwd": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _i, _vp, _f, _f, _vp, _vp]),
     "ryolo_obj_focal_bwd": (_i, [_vp, ctypes.POINTER(ctypes.c_longlong), _i, _i, _i, _i, _i, _i, _vp, _f, _f, _vp, _vp, _vp]),
     "ryolo_conv_wgrad": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
-    "ryolo_bn_stats": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_bn_stats_finalize": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "ryolo_bn_finalize": (_i, [_vp, _i, _f, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_bn_act_fwd": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _f, _i, _vp, _i, _vp, _i, _i, _vp, _vp]),
     "ryolo_bn_act_fwd_s2d": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _f, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _vp]),
     "ryolo_bn_act_bwd": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _i, _vp, _vp, _i, _i, _vp, _vp]),
@@ -109,7 +104,6 @@ SIGNATURES = {
     "ryolo_se_bwd": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                           _vp, _sz, _vp]),
     "ryolo_maxpool2x2": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp]),
-    "ryolo_nchw_to_padded": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "ryolo_im2col_first": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "ryolo_px_packed_weight_bytes": (_sz, [_i, _i, _i, _i]),
     "ryolo_px_pack_weights": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),

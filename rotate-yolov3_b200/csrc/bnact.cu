@@ -8,10 +8,9 @@
 //   bn_act_fwd        y = prelu(z*scale + shift) [+ res], optional 2x2 replicated store      (1 read [+1], 1 write)
 //   bn_act_bwd_reduce dy, z -> per-channel sum(du), sum(du * zhat), scalar d(slope)            (2 reads)
 //   bn_act_bwd_apply  dz = scale*(du - mean(du) - zhat*mean(du*zhat)) written over z; dres (+)= dy   (2 reads, 1-2 writes)
-// plus the small layout kernels of the training graph (zero insertion for stride-2 adjoints, NCHW fp32 -> padded
-// NHWC bf16 for the head gradients, im2col of the 3-channel image so that the first layer runs on the same GEMMs).
+// plus the small layout kernels of the training graph (zero insertion for stride-2 adjoints, im2col of the 3-channel
+// image so that the first layer runs on the same GEMMs).
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "f32x2.cuh"
@@ -384,29 +383,6 @@ __global__ void __launch_bounds__(BNT) bn_act_bwd_apply_kernel(const __nv_bfloat
   }
 }
 
-// BN finalisation: sums -> mean, invstd, scale, shift, and the running statistics of nn.BatchNorm2d (momentum m, unbiased
-// variance), one thread per channel.  Replaces ~10 tiny framework launches per block.
-__global__ void bn_finalize_kernel(const float* __restrict__ sums, int c, float count, float eps, float momentum,
-                                   const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   float* __restrict__ mean_o, float* __restrict__ invstd_o, float* __restrict__ scale_o,
-                                   float* __restrict__ shift_o, float* __restrict__ running_mean,
-                                   float* __restrict__ running_var) {
-  const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-  if (ch >= c) return;
-  const float mean = sums[ch] / count;
-  const float var = fmaxf(sums[c + ch] / count - mean * mean, 0.f);
-  const float invstd = rsqrtf(var + eps);
-  const float sc = gamma[ch] * invstd;
-  mean_o[ch] = mean;
-  invstd_o[ch] = invstd;
-  scale_o[ch] = sc;
-  shift_o[ch] = beta[ch] - mean * sc;
-  if (running_mean) {
-    running_mean[ch] = (1.f - momentum) * running_mean[ch] + momentum * mean;
-    running_var[ch] = (1.f - momentum) * running_var[ch] + momentum * var * (count / fmaxf(count - 1.f, 1.f));
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // adjoint of "keep the even pixels" (stride-2 conv): small grid gradient placed on the even interior pixels of the
 // (pre-zeroed, never otherwise written) input-resolution buffer
@@ -519,63 +495,6 @@ __global__ void __launch_bounds__(256) maxpool2x2_kernel(const __nv_bfloat16* __
   *reinterpret_cast<uint4*>(y + pad_off(b, oy, ox, g.h, g.w, ycs) + cg * 8) = *reinterpret_cast<uint4*>(m);
 }
 
-// fp32 NCHW [B, C, H, W] -> bf16 padded NHWC (interior, channels [0, C)).  Thread = (pixel x, 8-channel group):
-// consecutive threads read consecutive x of the same channel plane (coalesced) and write 16 bytes each.
-__global__ void __launch_bounds__(256) nchw_to_padded_kernel(const float* __restrict__ src, int batch, int c, int h, int w,
-                                                             __nv_bfloat16* __restrict__ dst, int dcs) {
-  const int cgs = (c + 7) >> 3;
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t total = (size_t)batch * cgs * h * w;
-  if (i >= total) return;
-  const int x = (int)(i % w);
-  const int y = (int)((i / w) % h);
-  const int cg = (int)((i / ((size_t)w * h)) % cgs);
-  const int b = (int)(i / ((size_t)w * h * cgs));
-  const size_t plane = (size_t)h * w;
-  const float* s = src + ((size_t)b * c + cg * 8) * plane + (size_t)y * w + x;
-  float f[8];
-#pragma unroll
-  for (int e = 0; e < 8; e++) f[e] = (cg * 8 + e < c) ? __ldg(s + e * plane) : 0.f;
-  __nv_bfloat16* o = dst + pad_off(b, y, x, h, w, dcs) + cg * 8;
-  if (cg * 8 + 8 <= dcs) {
-    *reinterpret_cast<uint4*>(o) = pack8(f);
-  } else {
-    for (int e = 0; e < 8 && cg * 8 + e < dcs; e++) o[e] = __float2bfloat16_rn(f[e]);
-  }
-}
-
-// Gradient of a YOLO head as autograd delivers it, fp32 [B, na, ny, nx, no] (the layout of the training-mode output,
-// model/models.py:190-192), -> bf16 padded NHWC with channel = a * no + k (the head conv's filter index).  One block =
-// 32 consecutive x of one image row: coalesced reads of the 32*no contiguous floats of every anchor, transposed through
-// shared memory, 16-byte stores of each pixel's na*no contiguous channels.
-__global__ void __launch_bounds__(256) head_grad_to_padded_kernel(const float* __restrict__ g, int na, int no, int ny, int nx,
-                                                                  __nv_bfloat16* __restrict__ dst, int dcs) {
-  extern __shared__ __align__(16) unsigned char hg_smem[];
-  __nv_bfloat16* tile = reinterpret_cast<__nv_bfloat16*>(hg_smem);   // [32][cpad]
-  const int c = na * no, cpad = (c + 7) & ~7;
-  const int x0 = blockIdx.x * 32, y = blockIdx.y, b = blockIdx.z;
-  const int npx = min(32, nx - x0);
-  const int run = npx * no;                                            // contiguous floats per anchor
-  for (int idx = threadIdx.x; idx < na * run; idx += 256) {
-    const int a = idx / run, r = idx - a * run;
-    const int px = r / no, k = r - px * no;
-    const float v = __ldg(g + (((size_t)b * na + a) * ny + y) * (size_t)nx * no + (size_t)x0 * no + r);
-    tile[px * cpad + a * no + k] = __float2bfloat16_rn(v);
-  }
-  __syncthreads();
-  const int chunks = c >> 3;                                           // whole 16-byte chunks per pixel
-  for (int idx = threadIdx.x; idx < npx * chunks; idx += 256) {
-    const int px = idx / chunks, ch = idx - px * chunks;
-    *reinterpret_cast<uint4*>(dst + pad_off(b, y, x0 + px, ny, nx, dcs) + ch * 8) =
-        *reinterpret_cast<const uint4*>(tile + px * cpad + ch * 8);
-  }
-  const int tail = c & 7;
-  for (int idx = threadIdx.x; idx < npx * tail; idx += 256) {
-    const int px = idx / tail, e = (c & ~7) + idx % tail;
-    dst[pad_off(b, y, x0 + px, ny, nx, dcs) + e] = tile[px * cpad + e];
-  }
-}
-
 // im2col of the 3-channel image for the first 3x3/stride-1/pad-1 conv: column index = c*9 + kh*3 + kw (the flattening
 // of nn.Conv2d.weight[co]), 27 real + zero padding to 64 channels, bf16 padded NHWC.  A thread builds one pixel's
 // 128-byte row in shared memory; the block then stores its rows as 16-byte chunks in address order, so a warp writes
@@ -626,14 +545,10 @@ static inline Geo mk_geo(int batch, int h, int w, int c) {
 static inline size_t n_items(const Geo& g) { return (size_t)g.batch * g.h * g.w * (g.c >> 3); }
 // rows per CTA so that a CTA streams ~16k 16-byte items and the grid still has >= ~4 CTAs per SM
 static inline int rows_per_block(const Geo& g) {
+  constexpr long long kItemsPerCta = 16384;
   const int cgs = g.c >> 3;
   long long per_row = (long long)g.w * cgs;
-  static int target = -1;
-  if (target < 0) {
-    const char* e = getenv("RYOLO_BN_ITEMS");     // measurement knob: 16-byte items per CTA
-    target = e ? atoi(e) : 16384;
-  }
-  int r = (int)((target + per_row - 1) / per_row);
+  int r = (int)((kItemsPerCta + per_row - 1) / per_row);
   const int nrows = g.batch * g.h;
   const int max_r = (nrows + 591) / 592;
   if (r > max_r) r = max_r;
@@ -671,11 +586,11 @@ static int bn_stats_impl(const void* z, int z_cstride, const Geo& g, float* sums
   const int c = g.c;
   int grid;
   PieceGeo pg;
-  const bool piped = pipe_ok(g, z_cstride, PIPE_STATS);
+  const bool piped = pipe_ok(g, z_cstride);
   const int rpb = rows_per_block(g);
   if (piped) {
     pg = mk_pieces(g, &grid);
-    pg.rev = bn_reverse_mode() & 1;
+    pg.rev = 1;   // descending: it starts in the tail the conv just wrote
   } else {
     grid = (g.batch * g.h + rpb - 1) / rpb;
   }
@@ -692,15 +607,6 @@ static int bn_stats_impl(const void* z, int z_cstride, const Geo& g, float* sums
   return bn_sums_reduce(partials, grid, c, 0, sums, fin, stream);
 }
 
-extern "C" int ryolo_bn_stats(const void* z, int z_cstride, int batch, int h, int w, int c, float* sums, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  RYOLO_ARG_CHECK(z && sums);
-  GEO_CHECK();
-  const Geo g = mk_geo(batch, h, w, c);
-  GEO_CHECK_P2();
-  return bn_stats_impl(z, z_cstride, g, sums, BnFinalize{}, stream);
-}
-
 static int bn_act_fwd_impl(const void* z, int z_cstride, int batch, int h, int w, int c, const float* scale,
                            const float* shift, float slope, int has_act, const void* residual, int res_cstride, void* y,
                            int y_cstride, int upsample2x, const float* slope_dev, void* xs, int xs_cstride, void* stream_) {
@@ -711,17 +617,6 @@ static int bn_act_fwd_impl(const void* z, int z_cstride, int batch, int h, int w
   RYOLO_ARG_CHECK(!xs || (!upsample2x && h % 2 == 0 && w % 2 == 0 && xs_cstride >= 4 * c && xs_cstride % 8 == 0));
   GEO_CHECK_P2();
   const Geo g = mk_geo(batch, h, w, c);
-  if (pipe_ok(g, z_cstride, PIPE_FWD)) {
-    int grid;
-    const PieceGeo pg = mk_pieces(g, &grid);
-    RYOLO_SMEM_OPT_IN(bn_act_fwd_pipe_kernel, (RowPipe<1, 4>::smem_bytes()));
-    bn_act_fwd_pipe_kernel<<<grid, BNT, RowPipe<1, 4>::smem_bytes(), stream>>>(
-        static_cast<const __nv_bfloat16*>(z), g, pg, scale, shift, slope, has_act, static_cast<const __nv_bfloat16*>(residual),
-        res_cstride, static_cast<__nv_bfloat16*>(y), y_cstride, upsample2x, slope_dev, static_cast<__nv_bfloat16*>(xs),
-        xs_cstride);
-    RYOLO_LAUNCH_CHECK();
-    return RYOLO_OK;
-  }
   const int rpb = rows_per_block(g);
   bn_act_fwd_kernel<<<(unsigned)((batch * h + rpb - 1) / rpb), BNT, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(z), z_cstride, g, scale, shift, slope, has_act,
@@ -759,7 +654,7 @@ extern "C" int ryolo_bn_act_bwd(const void* dy, int dy_cstride, int upsample2x, 
   GEO_CHECK_P2();
   const Geo g = mk_geo(batch, h, w, c);
   const float inv_cnt = 1.0f / ((float)batch * h * w);
-  if (pipe_ok(g, z_cstride, PIPE_BWD)) {
+  if (pipe_ok(g, z_cstride)) {
     // how dy reaches the kernels: 1 = plain tensor on the pipe, 2 = space-to-depth dgrad output on the pipe (row pairs),
     // 0 = direct loads (upsample adjoint, concat buffers)
     const int dyp = (upsample2x == 0 && dy_cstride == c) ? 1
@@ -775,7 +670,7 @@ extern "C" int ryolo_bn_act_bwd(const void* dy, int dy_cstride, int upsample2x, 
     float* partials = bn_partials(stream, (size_t)grid * (2 * c + 1));
     if (!partials) return RYOLO_E_CUDA;
     PieceGeo pg_red = pg;                       // the reduction walks descending (it starts in the tail dgrad just wrote),
-    pg_red.rev = (bn_reverse_mode() >> 1) & 1;   // the apply pass ascending (it starts where the reduction ended)
+    pg_red.rev = 1;                             // the apply pass ascending (it starts where the reduction ended)
 #define RYOLO_BWD_PIPE(D)                                                                                                  \
   do {                                                                                                                   \
     RYOLO_SMEM_OPT_IN(bn_act_bwd_reduce_pipe_kernel<D>, kMax);                                                           \
@@ -813,9 +708,6 @@ extern "C" int ryolo_bn_act_bwd(const void* dy, int dy_cstride, int upsample2x, 
   return RYOLO_OK;
 }
 
-extern "C" int ryolo_bn_finalize(const float* sums, int c, float count, float eps, float momentum, const float* gamma,
-                                 const float* beta, float* mean, float* invstd, float* scale, float* shift,
-                                 float* running_mean, float* running_var, void* stream_);
 extern "C" int ryolo_bn_stats_finalize(const void* z, int z_cstride, int batch, int h, int w, int c, float* sums, float eps,
                                        float momentum, const float* gamma, const float* beta, float* mean, float* invstd,
                                        float* scale, float* shift, float* running_mean, float* running_var, void* stream_) {
@@ -830,18 +722,6 @@ extern "C" int ryolo_bn_stats_finalize(const void* z, int z_cstride, int batch, 
   fin.gamma = gamma; fin.beta = beta; fin.mean = mean; fin.invstd = invstd; fin.scale = scale; fin.shift = shift;
   fin.running_mean = running_mean; fin.running_var = running_var; fin.count = count; fin.eps = eps; fin.momentum = momentum;
   return bn_stats_impl(z, z_cstride, g, sums, fin, stream);
-}
-
-extern "C" int ryolo_bn_finalize(const float* sums, int c, float count, float eps, float momentum, const float* gamma,
-                                 const float* beta, float* mean, float* invstd, float* scale, float* shift,
-                                 float* running_mean, float* running_var, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  RYOLO_ARG_CHECK(sums && gamma && beta && mean && invstd && scale && shift && c > 0 && count > 0.f);
-  RYOLO_ARG_CHECK((running_mean == nullptr) == (running_var == nullptr));
-  bn_finalize_kernel<<<(c + 127) / 128, 128, 0, stream>>>(sums, c, count, eps, momentum, gamma, beta, mean, invstd, scale,
-                                                          shift, running_mean, running_var);
-  RYOLO_LAUNCH_CHECK();
-  return RYOLO_OK;
 }
 
 extern "C" int ryolo_zero_insert2x(const void* src, int src_cstride, int batch, int h, int w, int c, void* dst,
@@ -936,33 +816,6 @@ extern "C" int ryolo_maxpool2x2(const void* x, int x_cstride, int batch, int in_
   maxpool2x2_kernel<<<(unsigned)((items + 255) / 256), 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(x), x_cstride, in_h,
                                                                         in_w, g, stride, static_cast<__nv_bfloat16*>(y),
                                                                         y_cstride);
-  RYOLO_LAUNCH_CHECK();
-  return RYOLO_OK;
-}
-
-extern "C" int ryolo_nchw_to_padded(const float* src, int batch, int c, int h, int w, void* dst, int dst_cstride,
-                                    void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  RYOLO_ARG_CHECK(src && dst && batch > 0 && c > 0 && h > 0 && w > 0 && dst_cstride >= c);
-  RYOLO_ARG_CHECK(dst_cstride % 8 == 0);
-  const size_t total = (size_t)batch * ((c + 7) / 8) * h * w;
-  nchw_to_padded_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(src, batch, c, h, w,
-                                                                            static_cast<__nv_bfloat16*>(dst), dst_cstride);
-  RYOLO_LAUNCH_CHECK();
-  return RYOLO_OK;
-}
-
-extern "C" int ryolo_head_grad_to_padded(const float* g, int batch, int na, int no, int ny, int nx, void* dst,
-                                         int dst_cstride, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  RYOLO_ARG_CHECK(g && dst && batch > 0 && na > 0 && no > 0 && ny > 0 && nx > 0);
-  RYOLO_ARG_CHECK(dst_cstride >= na * no && dst_cstride % 8 == 0 && batch <= 65535 && ny <= 65535);
-  const int cpad = (na * no + 7) & ~7;
-  const size_t smem = (size_t)32 * cpad * 2;
-  RYOLO_ARG_CHECK(smem <= 160 * 1024);
-  RYOLO_SMEM_OPT_IN(head_grad_to_padded_kernel, 160 * 1024);   // upper bound checked above; per device
-  dim3 grid((unsigned)((nx + 31) / 32), (unsigned)ny, (unsigned)batch);
-  head_grad_to_padded_kernel<<<grid, 256, smem, stream>>>(g, na, no, ny, nx, static_cast<__nv_bfloat16*>(dst), dst_cstride);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }

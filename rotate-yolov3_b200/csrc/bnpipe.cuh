@@ -1,4 +1,5 @@
-// TMA-fed versions of the four BN / PReLU passes (included by bnact.cu; same arithmetic, same results).
+// TMA-fed versions of the three read-limited BN / PReLU passes: statistics, backward reduce, backward apply (included by
+// bnact.cu; same arithmetic, same results).
 //
 // Work split: the grid of <= 2 x SMs persistent CTAs strides over the row pieces together (piece = blockIdx + k * gridDim), so
 // the whole grid reads one moving front of the tensor.
@@ -206,60 +207,6 @@ __global__ void __launch_bounds__(BNT, 2) bn_stats_pipe_kernel(const __nv_bfloat
     f2unpack(p2[e], s2[2 * e], s2[2 * e + 1]);
   }
   block_partials(rs, g.c, s1, s2, 0.f, false, s_acc, partials);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(BNT, 2) bn_act_fwd_pipe_kernel(const __nv_bfloat16* __restrict__ z, Geo g, PieceGeo pg,
-                                                                 const float* __restrict__ scale,
-                                                                 const float* __restrict__ shift, float slope, int has_act,
-                                                                 const __nv_bfloat16* __restrict__ res, int rcs,
-                                                                 __nv_bfloat16* __restrict__ y, int ycs, int up,
-                                                                 const float* __restrict__ slope_dev,
-                                                                 __nv_bfloat16* __restrict__ xs, int xcs) {
-  extern __shared__ __align__(128) unsigned char dsm[];
-  using Pipe = RowPipe<1, 4>;
-  Pipe pipe;
-  pipe.init(dsm, pg);
-  __syncthreads();
-  const __nv_bfloat16* src[1] = {z};
-  pipe.prologue(g, pg, src);
-  if (slope_dev) slope = __ldg(slope_dev);
-  const RowSpan rs = row_span(g);
-  float sc[8], sh[8];
-  load8(scale, rs.cg, sc);
-  load8(shift, rs.cg, sh);
-  for (int p = pipe.p_begin; p < pipe.p_end; p++) {
-    const Piece q = piece_at(g, pg, pipe.phys(p));
-    const int b = q.b, yy = q.y;
-    const __nv_bfloat16* rr = res ? res + pad_off(b, yy, 0, g.h, g.w, rcs) + rs.cg * 8 : nullptr;
-    const uint4* st = pipe.wait(p, 0);
-    const int items = q.npx << rs.cgs_log2;
-    for (int i = threadIdx.x; i < items; i += BNT) {
-      const int x = q.x0 + (i >> rs.cgs_log2);
-      float f[8], r[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      unpack8(st[i], f);
-      if (rr) unpack8(*reinterpret_cast<const uint4*>(rr + (size_t)x * rcs), r);
-#pragma unroll
-      for (int e = 0; e < 8; e++) {
-        float u = fmaf(f[e], sc[e], sh[e]);
-        if (has_act) u = u > 0.f ? u : slope * u;
-        f[e] = u + r[e];
-      }
-      const uint4 o = pack8(f);
-      if (!up) {
-        *reinterpret_cast<uint4*>(y + pad_off(b, yy, x, g.h, g.w, ycs) + rs.cg * 8) = o;
-        if (xs) *reinterpret_cast<uint4*>(xs + pad_off(b, yy >> 1, x >> 1, g.h >> 1, g.w >> 1, xcs) +
-                                          ((yy & 1) * 2 + (x & 1)) * g.c + rs.cg * 8) = o;
-      } else {
-#pragma unroll
-        for (int ry = 0; ry < 2; ry++)
-#pragma unroll
-          for (int rx = 0; rx < 2; rx++)
-            *reinterpret_cast<uint4*>(y + pad_off(b, 2 * yy + ry, 2 * x + rx, 2 * g.h, 2 * g.w, ycs) + rs.cg * 8) = o;
-      }
-    }
-    pipe.release(g, pg, p, src);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -513,31 +460,10 @@ __global__ void __launch_bounds__(BNT, 2) bn_act_bwd_apply_pipe_kernel(
 }
 
 // host side ------------------------------------------------------------------------------------------------------
-// measurement knob RYOLO_BN_PIPE = bit mask of the passes that take the pipe: 1 stats, 2 forward, 4 backward.  Default 5:
-// the forward pass is write-limited, so its direct version gains nothing from the pipe; statistics and the backward pair
-// are read-limited and do.
-constexpr int PIPE_STATS = 1, PIPE_FWD = 2, PIPE_BWD = 4;
-static inline int bn_pipe_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("RYOLO_BN_PIPE");
-    mode = e ? atoi(e) : (PIPE_STATS | PIPE_BWD);
-  }
-  return mode;
-}
-// measurement knob RYOLO_BN_REVERSE: bit 0 statistics, bit 1 backward reduce walk their ranges descending (default 3)
-static inline int bn_reverse_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("RYOLO_BN_REVERSE");
-    mode = e ? atoi(e) : 3;
-  }
-  return mode;
-}
-// the pipe needs the rows of the tensor to be contiguous (channel stride == c) and 256 threads to tile the channel groups
-static inline bool pipe_ok(const Geo& g, int cstride, int pass) {
-  return (bn_pipe_mode() & pass) != 0 && cstride == g.c && (g.c >> 3) <= BNT;
-}
+// The pipe needs the rows of the tensor to be contiguous (channel stride == c) and 256 threads to tile the channel groups.
+// Only the read-limited passes (statistics, the backward pair) take it: the forward pass is write-limited, so its direct
+// version gains nothing from the pipe.
+static inline bool pipe_ok(const Geo& g, int cstride) { return cstride == g.c && (g.c >> 3) <= BNT; }
 // rows_per_piece = 2: row pairs with even piece boundaries and half-size z pieces (BwdPipe<2>)
 static inline PieceGeo mk_pieces(const Geo& g, int* grid, int rows_per_piece = 1) {
   PieceGeo pg;

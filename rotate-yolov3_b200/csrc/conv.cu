@@ -537,14 +537,6 @@ extern "C" size_t ryolo_conv_packed_weight_bytes(const ryolo_conv_desc* d) {
   return (size_t)g.taps * g.cout_pad * g.cin_pad * 2;
 }
 
-extern "C" int ryolo_conv_pack_weights_ex(const ryolo_conv_desc* d, const float* weight, const float* scale,
-                                          void* packed_out, int mode, void* stream_);
-
-extern "C" int ryolo_conv_pack_weights(const ryolo_conv_desc* d, const float* weight, const float* scale, void* packed_out,
-                                       void* stream_) {
-  return ryolo_conv_pack_weights_ex(d, weight, scale, packed_out, 0, stream_);
-}
-
 extern "C" int ryolo_conv_unpack_wgrad(const float* dw, int cout_pad, int cin_pad, int mode, int cout, int cin, int ksize,
                                        float* grad, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -573,16 +565,8 @@ extern "C" int ryolo_conv_pack_weights_ex(const ryolo_conv_desc* d, const float*
   return RYOLO_OK;
 }
 
-extern "C" size_t ryolo_conv_workspace_bytes(const ryolo_conv_desc* d) {
-  (void)d;
-  return 0;  // the implicit GEMM needs no scratch (no im2col buffer)
-}
-
 extern "C" int ryolo_conv_bn_act_fwd(const ryolo_conv_desc* d, const void* x, const void* packed_w, const float* bias,
-                                     const void* residual, void* y, void* workspace, size_t workspace_bytes,
-                                     void* stream_) {
-  (void)workspace;
-  (void)workspace_bytes;
+                                     const void* residual, void* y, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RYOLO_ARG_CHECK(d && x && packed_w && bias && y);
   RYOLO_ARG_CHECK(d->batch > 0 && d->in_h > 0 && d->in_w > 0 && d->cin > 0 && d->cout > 0);

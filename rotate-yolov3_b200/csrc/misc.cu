@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(256) yolo_decode_kernel(const float* __restric
 
 using namespace ryolo;
 
-extern "C" int ryolo_abi_version(void) { return 1; }
+extern "C" int ryolo_abi_version(void) { return 2; }
 extern "C" const char* ryolo_last_error(void) { return err_buf(); }
 extern "C" uint64_t ryolo_launch_count(void) { return g_launches.load(); }
 

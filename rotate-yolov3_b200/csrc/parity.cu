@@ -349,7 +349,7 @@ __global__ void __launch_bounds__(256) px_to_nchw_kernel(const float* __restrict
   out[i] = v;
 }
 
-// head gradient fp32 [B, na, ny, nx, no] -> split planes, channel = a*no + k (cf. head_grad_to_padded_kernel)
+// head gradient fp32 [B, na, ny, nx, no] -> split planes, channel = a*no + k (the head conv's filter index)
 __global__ void __launch_bounds__(256) px_head_grad_kernel(const float* __restrict__ g, int batch, int na, int no, int ny,
                                                            int nx, __nv_bfloat16* __restrict__ dst, int dcs, int dlo, int np) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

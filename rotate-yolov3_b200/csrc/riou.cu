@@ -20,8 +20,6 @@
 // Stage A2: separating-axis test on queue 1 with converged warps -> queue 2 (~12 % of all pairs).  Stage B: clamp
 // integral on queue 2.  The output tile lives in shared memory (pre-zeroed) and is written back with 128-bit
 // streaming stores, so HBM sees exactly one coalesced write of the matrix.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "f32x2.cuh"
 #include "riou_area.cuh"
@@ -204,7 +202,6 @@ __device__ __forceinline__ void store_row(RiouSmem& sm, int t, const float4& d0,
   rr[2] = -d0.z;
 }
 
-template <int STORE>   // 0: streaming (st.global.cs), 1: plain, 2: write-through (st.global.wt)
 __global__ void __launch_bounds__(RIOU_THREADS, 4) riou_pairwise_kernel(const float* __restrict__ a, int n, int sa,
                                                                         const float* __restrict__ b, int m, int sb,
                                                                         int mode, float* __restrict__ out) {
@@ -361,10 +358,7 @@ __global__ void __launch_bounds__(RIOU_THREADS, 4) riou_pairwise_kernel(const fl
         if ((tid >> 5) + k * (RIOU_THREADS / 32) < rows) {
           const float4 v = src[k * RIOU_THREADS];
           src[k * RIOU_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
-          float4* d = dst + k * dstep;
-          if (STORE == 0) __stcs(d, v);        // streaming: the matrix is written once and not re-read by this kernel
-          else if (STORE == 1) *d = v;
-          else __stwt(d, v);
+          __stcs(dst + k * dstep, v);        // streaming: the matrix is written once and not re-read by this kernel
         }
       }
     } else {
@@ -404,15 +398,7 @@ extern "C" int ryolo_riou_pairwise(const float* a, int n, int stride_a, const fl
   RYOLO_ARG_CHECK(a && b && out);
   dim3 grid((m + CT - 1) / CT, ((n + RT - 1) / RT + ROW_TILES - 1) / ROW_TILES);
   RYOLO_ARG_CHECK(grid.y <= 65535);
-  static int store_mode = -1;
-  if (store_mode < 0) {   // measurement knob: RYOLO_RIOU_STORE=0|1|2, default streaming stores
-    const char* e = getenv("RYOLO_RIOU_STORE");
-    store_mode = e ? atoi(e) : 0;
-    if (store_mode < 0 || store_mode > 2) store_mode = 0;
-  }
-  if (store_mode == 1) riou_pairwise_kernel<1><<<grid, RIOU_THREADS, 0, stream>>>(a, n, stride_a, b, m, stride_b, mode, out);
-  else if (store_mode == 2) riou_pairwise_kernel<2><<<grid, RIOU_THREADS, 0, stream>>>(a, n, stride_a, b, m, stride_b, mode, out);
-  else riou_pairwise_kernel<0><<<grid, RIOU_THREADS, 0, stream>>>(a, n, stride_a, b, m, stride_b, mode, out);
+  riou_pairwise_kernel<<<grid, RIOU_THREADS, 0, stream>>>(a, n, stride_a, b, m, stride_b, mode, out);
   RYOLO_LAUNCH_CHECK();
   return RYOLO_OK;
 }

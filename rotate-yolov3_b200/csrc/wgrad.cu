@@ -20,8 +20,6 @@
 // and over the thousands of updates of one pixel range its error is biased towards zero.  As in conv_parity.cu, the MMA
 // warp groups then restart the accumulator every WG_SEG k-steps (32 MMA updates) and fold it into a second register set
 // with round-to-nearest fp32 adds; the split-K reduction and the store are unchanged.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "sm90.cuh"
 
@@ -360,29 +358,18 @@ static int wgrad(const void* dz, int dz_cstride, int cout_pad, const void* x, in
   p.ksteps_total = (p.np + WG_BK - 1) / WG_BK;
   const int num_sms = gemm_sm_count();
   // taps per CTA: the kernel row (3 or 2 taps) when the accumulators fit the registers (TG * bn <= 256) and the layer
-  // is thin enough to be operand-stream bound; RYOLO_WGRAD_TG=1 forces one tap per CTA (measurement knob)
-  static int force_tg = -1;
-  if (force_tg < 0) {
-    const char* e = getenv("RYOLO_WGRAD_TG");
-    force_tg = e ? atoi(e) : 0;
-  }
+  // is thin enough to be operand-stream bound
   int tg = 1;
-  if (bn <= 128 && force_tg != 1) tg = p.taps == 9 ? 3 : (p.taps == 4 ? 2 : 1);
+  if (bn <= 128) tg = p.taps == 9 ? 3 : (p.taps == 4 ? 2 : 1);
   if (tg * bn > (seg ? 128 : 256)) tg = 1;
   p.tap_groups = p.taps / tg;
   const int tiles = p.tap_groups * p.m_tiles * p.n_tiles;
   // split-K: every (tile, split) CTA ends with tile-size fp32 stores and cannot overlap them with its MMAs, so use the
   // FEWEST waves that still fill the SMs (>= 90 % of the last wave), not a fixed multiple
-  static int force_waves = -1;
-  if (force_waves < 0) {
-    const char* e = getenv("RYOLO_WGRAD_WAVES");   // measurement knob
-    force_waves = e ? atoi(e) : 0;
-  }
   int ksplit = 1;
   {
     double best_eff = 0.0;
     for (int waves = 1; waves <= 4; waves++) {
-      if (force_waves > 0 && waves != force_waves) continue;
       int ks = waves * num_sms / tiles;
       if (ks < 1) ks = 1;
       const int ctas = tiles * ks;

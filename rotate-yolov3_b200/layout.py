@@ -88,5 +88,5 @@ def s2d_weight_grad(dw2, c):
 def conv_fwd(desc, x_ptr, packed_w, bias, y_ptr, residual_ptr=None, device=None):
     st = _lib.lib.ryolo_conv_bn_act_fwd(ctypes.byref(desc), ctypes.c_void_p(x_ptr), _lib.ptr(packed_w), _lib.ptr(bias),
                                         ctypes.c_void_p(residual_ptr) if residual_ptr else None,
-                                        ctypes.c_void_p(y_ptr), None, 0, _lib.stream_ptr(device))
+                                        ctypes.c_void_p(y_ptr), _lib.stream_ptr(device))
     _lib.check(st, "ryolo_conv_bn_act_fwd")

@@ -503,7 +503,7 @@ class Darknet(nn.Module):
             else:
                 st = lib.ryolo_conv_bn_act_fwd(ctypes.byref(a["desc"]), ctypes.c_void_p(a["x"]), _lib.ptr(a["w"]),
                                                _lib.ptr(a["b"]), ctypes.c_void_p(a["r"]) if a["r"] else None,
-                                               ctypes.c_void_p(a["y"]), None, 0, stream)
+                                               ctypes.c_void_p(a["y"]), stream)
                 _lib.check(st, "ryolo_conv_bn_act_fwd")
         if not self.yolo_layers:      # trunk graph without YOLO layers: the raw head maps [B, filters, ny, nx]
             return [head for _, head in plan["heads"]]

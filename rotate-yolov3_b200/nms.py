@@ -42,34 +42,6 @@ def r_nms(dets, threshold):
         return keep[:k]
 
 
-def r_nms_async(dets, threshold):
-    """Same computation as r_nms without the host synchronisation: returns (keep [N] int64, num_keep [1] int32) device
-    tensors; keep[:num_keep] are the kept original indices, ascending.  dets must be [N>0, 6] float32 CUDA contiguous.
-    Used to overlap several images' NMS on different streams (bench.py detect workload)."""
-    n = dets.shape[0]
-    ws_bytes = _lib.lib.ryolo_rnms_workspace_bytes(n)
-    ws = _workspace(ws_bytes, dets.device)
-    keep = torch.empty((n,), dtype=torch.long, device=dets.device)
-    num = torch.empty((1,), dtype=torch.int32, device=dets.device)
-    st = _lib.lib.ryolo_rnms(_lib.ptr(dets), n, float(threshold), _lib.ptr(keep), _lib.ptr(num), _lib.ptr(ws), ws_bytes,
-                             _lib.stream_ptr(dets.device))
-    _lib.check(st, "ryolo_rnms")
-    return keep, num, ws
-
-
-def nms_filter_async(pred, conf_thres, min_wh, capacity):
-    """nms_filter without the host synchronisation: returns (out [capacity, 8] pre-filled with conf = -1, num [1])."""
-    p, no = pred.shape
-    out = torch.full((capacity, 8), -1.0, dtype=torch.float32, device=pred.device)
-    num = torch.empty((1,), dtype=torch.int32, device=pred.device)
-    ws_bytes = _lib.lib.ryolo_nms_filter_workspace_bytes(p)
-    ws = _workspace(ws_bytes, pred.device)
-    st = _lib.lib.ryolo_nms_filter(_lib.ptr(pred), p, no - 6, float(conf_thres), float(min_wh), _lib.ptr(out), capacity,
-                                   _lib.ptr(num), _lib.ptr(ws), ws_bytes, _lib.stream_ptr(pred.device))
-    _lib.check(st, "ryolo_nms_filter")
-    return out, num
-
-
 def rnms_debug(dets, threshold):
     """Test hook: run r_nms and also return (sorted_boxes [N,6], order [N] int32, mask [N, ceil(N/64)] int64 view)."""
     d = dets[:, :6].to(torch.float32).contiguous()

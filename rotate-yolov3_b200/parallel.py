@@ -126,10 +126,7 @@ class DistributedDataParallel(torch.nn.Module):
         super().__init__()
         self.module = module
         # reserved_sms: SMs the backward GEMMs leave to the concurrent NCCL kernels.  The default leaves every SM to the
-        # GEMMs; the knob is for rank counts where the all-reduce competes with them
-        import os
-        reserved_sms = int(os.environ.get("RYOLO_DDP_RESERVED_SMS", reserved_sms))     # measurement knobs
-        bucket_mb = float(os.environ.get("RYOLO_DDP_BUCKET_MB", bucket_mb))
+        # GEMMs; the argument is for rank counts where the all-reduce competes with them
         module._ddp = {"bucket_bytes": int(bucket_mb * (1 << 20)), "group": process_group, "reserved_sms": int(reserved_sms)}
         module._tplan = None          # the plan builds its buckets at construction
         module._pplan = None

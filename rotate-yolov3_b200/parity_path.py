@@ -49,10 +49,6 @@ def _f32_buf(batch, h, w, cs, device):
     return torch.zeros((batch, h + 2, w + 2, cs), dtype=torch.float32, device=device)
 
 
-class _Blk:
-    pass
-
-
 class ParityPlan:
     def __init__(self, model, batch, height, width, device, train):
         self.model, self.batch, self.h, self.w, self.device, self.train = model, batch, height, width, device, train

@@ -422,10 +422,10 @@ class TrainPlan:
                 if seq.Conv2d.bias is not None and blk.owner is None:     # a weight_from head runs without bias
                     blk.bias_pad[:blk.cout].copy_(seq.Conv2d.bias.detach())
                 _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), ctypes.c_void_p(x_ptr), _lib.ptr(blk.pw),
-                                                     _lib.ptr(blk.bias_pad), None, _lib.ptr(blk.out), None, 0, st), "conv head")
+                                                     _lib.ptr(blk.bias_pad), None, _lib.ptr(blk.out), st), "conv head")
                 continue
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), ctypes.c_void_p(x_ptr), _lib.ptr(blk.pw),
-                                                 _lib.ptr(self.zero_bias), None, _lib.ptr(blk.z), None, 0, st), "conv")
+                                                 _lib.ptr(self.zero_bias), None, _lib.ptr(blk.z), st), "conv")
             cnt = n_per_pixel * blk.oh * blk.ow
             if blk.has_bn:
                 bn = seq.BatchNorm2d
@@ -578,7 +578,7 @@ class TrainPlan:
                                                 st), "wgrad s2d")
             if dgrad:
                 _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
-                                                     _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxs), None, 0, st),
+                                                     _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxs), st),
                            "dgrad s2d")
                 if not blk.dxs_direct:
                     _lib.check(lib.ryolo_depth_to_space(_lib.ptr(blk.dxs), blk.xs_cs, self.batch, blk.src.h, blk.src.w,
@@ -598,7 +598,7 @@ class TrainPlan:
             blk.ddesc.has_residual = int(blk.gsrc_acc)
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
                                                  _lib.ptr(self.zero_bias), ctypes.c_void_p(gp) if blk.gsrc_acc else None,
-                                                 ctypes.c_void_p(gp), None, 0, st), "dgrad")
+                                                 ctypes.c_void_p(gp), st), "dgrad")
 
     # ---- weight_from blocks (reference models.py:255-265): a linear conv with the owner's weight, no bias / BN / activation.
     # The forward writes y directly (the conv epilogue, or for a dilated conv the merge, adds the shortcut that follows).
@@ -636,13 +636,13 @@ class TrainPlan:
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), ctypes.c_void_p(blk.src.ptr), _lib.ptr(blk.pw),
                                                  _lib.ptr(self.zero_bias),
                                                  ctypes.c_void_p(blk.res.ptr) if blk.res is not None else None,
-                                                 ctypes.c_void_p(blk.y.ptr), None, 0, st), "conv (weight_from)")
+                                                 ctypes.c_void_p(blk.y.ptr), st), "conv (weight_from)")
             return
         dh, dw = blk.dil
         _lib.check(lib.ryolo_dilate_split(ctypes.c_void_p(blk.src.ptr), blk.src.cs, self.batch, blk.src.h, blk.src.w,
                                           blk.cin, dh, dw, _lib.ptr(blk.xp), blk.cin_pad, st), "dilate_split")
         _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.fdesc), _lib.ptr(blk.xp), _lib.ptr(blk.pw),
-                                             _lib.ptr(self.zero_bias), None, _lib.ptr(blk.zp), None, 0, st), "conv (dilated)")
+                                             _lib.ptr(self.zero_bias), None, _lib.ptr(blk.zp), st), "conv (dilated)")
         _lib.check(lib.ryolo_dilate_merge(_lib.ptr(blk.zp), blk.zcs, self.batch, blk.oh, blk.ow, blk.cout, dh, dw,
                                           ctypes.c_void_p(blk.res.ptr) if blk.res is not None else None,
                                           blk.res.cs if blk.res is not None else 0, 0, ctypes.c_void_p(blk.y.ptr), blk.y.cs,
@@ -671,7 +671,7 @@ class TrainPlan:
             blk.ddesc.has_residual = int(blk.gsrc_acc)
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(blk.z), _lib.ptr(blk.pwd),
                                                  _lib.ptr(self.zero_bias), ctypes.c_void_p(gp) if blk.gsrc_acc else None,
-                                                 ctypes.c_void_p(gp), None, 0, st), "dgrad (weight_from)")
+                                                 ctypes.c_void_p(gp), st), "dgrad (weight_from)")
             return
         dh, dw = blk.dil
         if not (wgrad or dgrad):
@@ -684,7 +684,7 @@ class TrainPlan:
         if not dgrad:
             return
         _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(blk.zp), _lib.ptr(blk.pwd),
-                                             _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxp), None, 0, st),
+                                             _lib.ptr(self.zero_bias), None, _lib.ptr(blk.dxp), st),
                    "dgrad (dilated)")
         _lib.check(lib.ryolo_dilate_merge(_lib.ptr(blk.dxp), blk.cin_pad, self.batch, blk.src.h, blk.src.w, blk.cin, dh, dw,
                                           None, 0, int(blk.gsrc_acc), ctypes.c_void_p(blk.gsrc.ptr), blk.gsrc.cs, st),

@@ -15,7 +15,7 @@ def _declared():
     return sorted(set(re.findall(r"\b(ryolo_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_header_symbols_exported():
+def test_header_symbols_exported_abi_v2():
     import rotate_yolov3_b200 as pkg
     names = _declared()
     assert len(names) >= 10
@@ -23,7 +23,7 @@ def test_header_symbols_exported():
         assert hasattr(pkg._lib.lib, n), "libryolo.so does not export %s" % n
         assert n in pkg._lib.SIGNATURES, "ctypes binding missing for %s" % n
     assert set(pkg._lib.SIGNATURES) == set(names)
-    assert pkg._lib.lib.ryolo_abi_version() == 1
+    assert pkg._lib.lib.ryolo_abi_version() == 2
 
 
 def test_workspace_queries_need_no_gpu():
@@ -66,3 +66,19 @@ def test_no_oracle_in_product():
             if f.endswith((".py", ".cu", ".cuh", ".h")):
                 txt = open(os.path.join(root, f), errors="ignore").read()
                 assert "librbox_oracle" not in txt and "oracle/_ref" not in txt.replace("oracle/_ref (", ""), f
+
+
+def test_no_environment_knobs():
+    """Nothing the library or the package computes depends on the environment: no getenv in the CUDA sources, and the
+    only environment read in the package is the build's NVCC lookup."""
+    pkg_dir = os.path.join(REPO, "rotate-yolov3_b200")
+    for root, _, files in os.walk(os.path.join(pkg_dir, "csrc")):
+        for f in files:
+            assert "getenv(" not in open(os.path.join(root, f), errors="ignore").read(), f
+    for root, _, files in os.walk(pkg_dir):
+        for f in files:
+            if f.endswith(".py"):
+                txt = open(os.path.join(root, f)).read()
+                if f == "build.py":
+                    txt = txt.replace('os.environ.get("NVCC")', "", 1)
+                assert not re.search(r"os\.environ|os\.getenv", txt), f

@@ -21,7 +21,7 @@ def _bf(t):
                                             (64, 200, 200, 4, True, False), (128, 8, 6, 2, False, 2),
                                             (64, 200, 200, 3, False, 2), (32, 8, 8, 2, False, 2), (1024, 19, 19, 8, True, False),
                                             (64, 120, 200, 2, False, True)])
-def test_bn_prelu_fwd_bwd_vs_autograd(c, h, w, b, res, up):
+def test_bn_stats_finalize_prelu_fwd_bwd_vs_autograd(c, h, w, b, res, up):
     import rotate_yolov3_b200 as pkg
     from rotate_yolov3_b200 import layout as L
     lib = pkg._lib.lib
@@ -50,24 +50,22 @@ def test_bn_prelu_fwd_bwd_vs_autograd(c, h, w, b, res, up):
     # ---- kernels ----
     cs = L.round_up(c, 64)
     zb = L.to_padded_nhwc(z, cs)
-    sums = torch.zeros(2 * c, device=dev)
     pt = pkg._lib.ptr
     stream = pkg._lib.stream_ptr(dev)
-    assert lib.ryolo_bn_stats(pt(zb), cs, b, h, w, c, pt(sums), stream) == 0
+    # statistics + finalisation in ONE call (the reduction of the per-CTA partial rows finalises each channel) ==
+    # nn.BatchNorm2d's bookkeeping
+    sums = torch.full((2 * c + 1,), 3.0, device=dev)       # sums[0, 2c) are overwritten, whatever they held
+    f_mean, f_inv, f_sc, f_sh = (torch.empty(c, device=dev) for _ in range(4))
+    rm, rv = torch.full((c,), 0.25, device=dev), torch.full((c,), 2.0, device=dev)
+    assert lib.ryolo_bn_stats_finalize(pt(zb), cs, b, h, w, c, pt(sums), 1e-5, 0.1, pt(gamma), pt(beta), pt(f_mean), pt(f_inv),
+                                       pt(f_sc), pt(f_sh), pt(rm), pt(rv), stream) == 0
     n = b * h * w
     mean = sums[:c] / n
-    var = (sums[c:] / n - mean * mean).clamp_(min=0)
+    var = (sums[c:2 * c] / n - mean * mean).clamp_(min=0)
     assert torch.allclose(mean, z.mean((0, 2, 3)), atol=1e-4) and torch.allclose(var, z.var((0, 2, 3), unbiased=False), rtol=1e-3, atol=1e-4)
     invstd = torch.rsqrt(var + 1e-5)
     scale = (gamma * invstd).contiguous()
     shift = (beta - mean * scale).contiguous()
-    # statistics + finalisation in ONE call (the reduction of the per-CTA partial rows finalises each channel) ==
-    # nn.BatchNorm2d's bookkeeping
-    f_sums = torch.full((2 * c + 1,), 3.0, device=dev)       # sums[0, 2c) are overwritten, whatever they held
-    f_mean, f_inv, f_sc, f_sh = (torch.empty(c, device=dev) for _ in range(4))
-    rm, rv = torch.full((c,), 0.25, device=dev), torch.full((c,), 2.0, device=dev)
-    assert lib.ryolo_bn_stats_finalize(pt(zb), cs, b, h, w, c, pt(f_sums), 1e-5, 0.1, pt(gamma), pt(beta), pt(f_mean), pt(f_inv),
-                                       pt(f_sc), pt(f_sh), pt(rm), pt(rv), stream) == 0
     assert torch.allclose(f_mean, mean, atol=1e-5) and torch.allclose(f_inv, invstd, rtol=1e-4)
     assert torch.allclose(f_sc, scale, rtol=1e-4, atol=1e-6) and torch.allclose(f_sh, shift, rtol=1e-4, atol=1e-5)
     assert torch.allclose(rm, 0.9 * 0.25 + 0.1 * mean, atol=1e-5)
@@ -138,25 +136,3 @@ def test_dgrad_via_forward_kernel_vs_autograd(cin, cout, k, stride, h, w):
     sc = float(want.abs().max())
     assert float((got - want).abs().max()) <= 2.0 ** -7 * sc, (float((got - want).abs().max()), sc)
 
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("shape", [(2, 3, 7, 5, 9), (3, 72, 7, 19, 19), (1, 4, 6, 40, 33)])
-def test_head_grad_to_padded(shape):
-    """autograd's head gradient [B, na, ny, nx, no] fp32 -> bf16 padded NHWC with channel = a*no + k (exact bf16 rounding
-    of the same values as the permute + nchw_to_padded path); channels beyond na*no and the halo stay untouched"""
-    import rotate_yolov3_b200 as pkg
-    from rotate_yolov3_b200 import layout as L
-    dev = torch.device("cuda")
-    b, na, no, ny, nx = shape
-    g = torch.randn(b, na, ny, nx, no, generator=torch.Generator().manual_seed(7)).to(dev)
-    c = na * no
-    cs = L.round_up(c, 32)
-    dst = L.alloc_padded(b, ny, nx, cs, dev)
-    dst[..., c:] = 3.0
-    st = pkg._lib.lib.ryolo_head_grad_to_padded(pkg._lib.ptr(g), b, na, no, ny, nx, pkg._lib.ptr(dst), cs,
-                                                pkg._lib.stream_ptr(dev))
-    assert st == 0, pkg._lib.last_error()
-    want = g.permute(0, 2, 3, 1, 4).reshape(b, ny, nx, c).to(torch.bfloat16)
-    assert torch.equal(dst[:, 1:-1, 1:-1, :c], want)
-    assert float((dst[:, 1:-1, 1:-1, c:] - 3.0).abs().max() if cs > c else 0.0) == 0.0
-    assert float(dst[:, 0, :, :c].abs().max()) == 0 and float(dst[:, :, 0, :c].abs().max()) == 0

@@ -80,7 +80,7 @@ def gemm_sm_count():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# BN geometry mirror (csrc/bnact.cu rows_per_block, csrc/bnpipe.cuh mk_pieces / pipe_ok with the default pass mask)
+# BN geometry mirror (csrc/bnact.cu rows_per_block, csrc/bnpipe.cuh mk_pieces / pipe_ok)
 def bn_geometry(b, h, w, c, cs, sms):
     cgs = c // 8
     pstep = 256 // cgs

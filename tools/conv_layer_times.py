@@ -168,7 +168,7 @@ def main():
 
         def run_fwd(a=fwd):
             _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(a[0]), ctypes.c_void_p(a[1]), _lib.ptr(a[2]), _lib.ptr(a[3]),
-                                                 None, _lib.ptr(a[4]), None, 0, st), "conv")
+                                                 None, _lib.ptr(a[4]), st), "conv")
         r["fwd_us"] = event_time_us(run_fwd, args.iters)
         r["fwd_mma_gflop"] = mma_f / 1e9
         r["fwd_matmul_tflops"], r["fwd_matmul_mnk"] = matmul_rate(B * blk.oh * blk.ow, blk.cout,
@@ -197,7 +197,7 @@ def main():
             if blk.s2d:
                 def run_dgrad(blk=blk, dz=dz):
                     _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
-                                                         _lib.ptr(plan.zero_bias), None, _lib.ptr(blk.dxs), None, 0, st),
+                                                         _lib.ptr(plan.zero_bias), None, _lib.ptr(blk.dxs), st),
                                "dgrad s2d")
             else:
                 def run_dgrad(blk=blk, dz=dz):
@@ -206,7 +206,7 @@ def main():
                     _lib.check(lib.ryolo_conv_bn_act_fwd(ctypes.byref(blk.ddesc), _lib.ptr(dz), _lib.ptr(blk.pwd),
                                                          _lib.ptr(plan.zero_bias),
                                                          ctypes.c_void_p(gp) if blk.gsrc_acc else None,
-                                                         ctypes.c_void_p(gp), None, 0, st), "dgrad")
+                                                         ctypes.c_void_p(gp), st), "dgrad")
             r["dgrad_us"] = event_time_us(run_dgrad, args.iters)
             r["dgrad_matmul_tflops"], r["dgrad_matmul_mnk"] = matmul_rate(B * h * w, blk.cin, blk.cout * blk.k * blk.k,
                                                                           args.iters)

@@ -268,6 +268,16 @@ int ryolo_conv_pack_weights_multi(const ryolo_pack_job* jobs_dev, int njobs, con
                                   long long total, void* stream);
 int ryolo_conv_unpack_wgrad_multi(const ryolo_unpack_job* jobs_dev, int njobs, const long long* prefix_dev,
                                   long long total, void* stream);
+/* Zero invariants of padded-NHWC bf16 buffers [batch, h+2, w+2, c_stride] that share storage with buffers of other
+ * shapes (the activation pool of a Darknet model): one launch zeroes, for every job of the table (device memory), the
+ * 1-pixel halo ring (all channels) and channels [c_real, c_stride) of the interior pixels; interior channels below
+ * c_real keep their bytes.  c_real = 0 zeroes the whole buffer.  ptr 16-byte aligned, c_stride % 8 == 0,
+ * 0 <= c_real <= c_stride; njobs <= 65535. */
+typedef struct ryolo_halo_job {
+  void* ptr;
+  int32_t batch, h, w, c_real, c_stride, reserved;
+} ryolo_halo_job;
+int ryolo_zero_halo_multi(const ryolo_halo_job* jobs_dev, int njobs, void* stream);
 /* y = act(conv(x, W') + bias) [+ residual].  bias: fp32 [cout_pad] (zero beyond cout).  The implicit
  * GEMM needs no scratch memory. */
 int ryolo_conv_bn_act_fwd(const ryolo_conv_desc* d, const void* x, const void* packed_w,

@@ -46,6 +46,12 @@ class UnpackJob(ctypes.Structure):
                 ("mode", ctypes.c_int32), ("cout", ctypes.c_int32), ("cin", ctypes.c_int32), ("ks", ctypes.c_int32)]
 
 
+class HaloJob(ctypes.Structure):
+    """mirror of ryolo_halo_job"""
+    _fields_ = [("ptr", ctypes.c_void_p), ("batch", ctypes.c_int32), ("h", ctypes.c_int32), ("w", ctypes.c_int32),
+                ("c_real", ctypes.c_int32), ("c_stride", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
 # name -> (restype, argtypes); must list every symbol include/ryolo.h declares (tests/test_abi.py checks it)
 SIGNATURES = {
     "ryolo_abi_version": (_i, []),
@@ -74,6 +80,7 @@ SIGNATURES = {
     "ryolo_conv_pack_weights_ex": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _i, _vp]),
     "ryolo_conv_unpack_wgrad": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_conv_pack_weights_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
+    "ryolo_zero_halo_multi": (_i, [_vp, _i, _vp]),
     "ryolo_conv_unpack_wgrad_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_conv_bn_act_fwd": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_conv_first_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),

@@ -137,20 +137,28 @@ class Graph:
 class Buffers:
     """the output view of every materialised layer and, where the plan trains, its gradient twin.  alloc(h, w, cs)
     returns (buffer, gradient buffer or None) with channel stride cs; a layer outside any concat gets buffers of its own
-    with cs rounded up to `round_to`."""
+    with cs rounded up to `round_to`.  channels: id of every buffer -> the channels its views cover (the rest of cs is
+    padding no producer writes)."""
 
     def __init__(self, graph, alloc, round_to):
         self.graph, self.alloc, self.round_to = graph, alloc, round_to
         self.views, self.gviews = [None] * len(graph.shape), [None] * len(graph.shape)
         self.place = {}          # concat source -> (buffer, gradient buffer, channel offset)
+        self.channels = {}
         for i, ls in graph.concats.items():
             c, h, w = graph.shape[i]
             buf, gbuf = alloc(h, w, L.round_up(c, 64))
+            self._real(buf, gbuf, c)
             off = 0
             for l in ls:
                 self.place[l] = (buf, gbuf, off)
                 off += graph.shape[l][0]
             self.views[i], self.gviews[i] = self._pair(buf, gbuf, 0, c, h, w)
+
+    def _real(self, buf, gbuf, c):
+        for b in (buf, gbuf):
+            if b is not None:
+                self.channels[id(b)] = c
 
     @staticmethod
     def _pair(buf, gbuf, off, c, h, w):
@@ -163,6 +171,7 @@ class Buffers:
             buf, gbuf, off = self.place[layer]
         else:
             (buf, gbuf), off = self.alloc(h, w, L.round_up(c, self.round_to)), 0
+            self._real(buf, gbuf, c)
         self.views[layer], self.gviews[layer] = self._pair(buf, gbuf, off, c, h, w)
         return self.views[layer], self.gviews[layer]
 

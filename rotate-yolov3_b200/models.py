@@ -24,6 +24,7 @@ from . import _lib
 from . import graph as G
 from . import layout as L
 from .parse_config import parse_model_cfg
+from .pool import ActivationPool
 
 
 class SELayer(nn.Module):
@@ -69,7 +70,13 @@ class YOLOLayer(nn.Module):
         self.ng = torch.Tensor(ng).to(device)
         self.nx = nx
         self.ny = ny
-        self._anchors_dev = self.anchors.to(device=device, dtype=torch.float32).contiguous()
+        a = self.anchors.to(device=device, dtype=torch.float32).contiguous()
+        old = getattr(self, "_anchors_dev", None)
+        if old is not None and old.device == a.device and old.shape == a.shape:
+            # in place: the CUDA graphs of the eval plans of other shapes hold this address in their decode launches
+            old.copy_(a)
+        else:
+            self._anchors_dev = a
 
     def decode_into(self, p, img_size, io, rows_total, row_offset):
         """p: [B, na*(nc+6), ny, nx] fp32 NCHW head output -> writes rows of io, returns the permuted raw view."""
@@ -206,41 +213,94 @@ class Darknet(nn.Module):
         self.arc = arc
         self.version = np.array([0, 2, 5], dtype=np.int32)
         self.seen = np.array([0], dtype=np.int64)
-        self._plan = None
-        self._plan_key = None
+        # Plans are cached per shape, (batch, h, w, device), and per mode; the shape-sized storage of all training plans
+        # is one ActivationPool (pool.py), that of the eval plans one per batch size, so the plans of the reference's
+        # multi-scale loops stay resident at the cost of the largest shape.  Eval plans hold weights packed at one parameter version (_plans_ver): a version change
+        # drops them all.  _tshared / _eshared: the parameter-sized device state the plans of every shape share.
+        self._plans, self._tplans, self._pools = {}, {}, {}
+        self._plans_ver = None
+        self._tshared, self._eshared = {}, {}
+        self._plan_cur = self._tplan_cur = None
         self._ver_tensors = None
-        self._tplan = None
-        self._tplan_key = None
         # opt-in: replay the eval forward as ONE CUDA graph (78 launches -> 1).  The returned tensors are then static
         # buffers that the next forward overwrites (standard CUDA-graph semantics), hence not the default.
         self.use_cuda_graph = False
-        self._graph = None
+        self._graph = self._x_static = self._graph_out = self._graph_kernels = None
         self.replayed_kernels = 0
+
+    # the plans of the last forward in each mode; assigning None drops the whole cache of that mode
+    @property
+    def _plan(self):
+        return self._plan_cur
+
+    @_plan.setter
+    def _plan(self, value):
+        if value is not None:
+            raise ValueError("only None (drop the eval plans) can be assigned")
+        self._drop_eval()
+        self._eshared.clear()
+
+    @property
+    def _tplan(self):
+        return self._tplan_cur
+
+    @_tplan.setter
+    def _tplan(self, value):           # `model._tplan = None`, the spelling bench.py uses
+        if value is not None:
+            raise ValueError("only None (drop the training plans) can be assigned")
+        self.drop_training_plans()
+
+    def drop_training_plans(self):
+        """forget every training plan and the parameter-sized state they share (packed weights, gradient arenas,
+        all-reduce buckets); the next training forward builds its plan afresh in the pool"""
+        self._drop_train()
+        self._tshared.clear()
+
+    def _drop_eval(self, batch=None):
+        """the eval plans (with their CUDA graphs) of one batch size, or all; the packed weights stay"""
+        for key in [k for k in self._plans if batch is None or k[0] == batch]:
+            del self._plans[key]
+        if self._plan_cur is not None and self._plan_cur not in self._plans.values():
+            self._plan_cur = None
+            self._graph = self._x_static = self._graph_out = self._graph_kernels = None
+
+    def _drop_train(self):
+        self._tplans.clear()
+        self._tplan_cur = None
+
+    def _pool(self, mode, device):
+        if (mode, device) not in self._pools:
+            self._pools[(mode, device)] = ActivationPool(device)
+        return self._pools[(mode, device)]
 
     # ------------------------------------------------------------------------------------------------------
     def fuse(self):
         """reference models.py:300-313 folds BN into the convs module-by-module; here folding happens when the
         GEMM operands are packed (every eval forward uses folded weights), so this only drops the cache."""
         self._plan = None
-        self._graph = None
 
     def train(self, mode=True):
         self._plan = None
-        self._graph = None
         return super().train(mode)
 
     def load_state_dict(self, *a, **k):
         self._plan = None
-        self._graph = None
         return super().load_state_dict(*a, **k)
 
     def _apply(self, fn, *a, **k):      # .to() / .cuda() / .half() / .float(): storage changes without a version bump
         self._plan = None
-        self._graph = None
         self._tplan = None
+        self._pools = {}
         self._pplan = None
         self._ver_tensors = None
         return super()._apply(fn, *a, **k)
+
+    def _packed(self, key, desc, wt, scale=None):
+        """packed weight operand, shared by the eval plans of every shape until the parameters change"""
+        k = key + (desc.cin, desc.cout, desc.ksize)
+        if k not in self._eshared:
+            self._eshared[k] = L.pack_weights(desc, wt, scale)
+        return self._eshared[k]
 
     # ------------------------------------------------------------------------------------------------------
     def _folded(self, i, device):
@@ -261,19 +321,23 @@ class Darknet(nn.Module):
         slope = float(seq.activation.weight.detach().float().item()) if hasattr(seq, "activation") else None
         return w, scale, bias, slope
 
-    def _build_plan(self, batch, height, width, device):
+    def _build_plan(self, batch, height, width, device, pool):
+        """the eval forward at one shape: its shape-sized storage from `pool` (every zero-initialised buffer is rewritten
+        by every forward before it is read or restored by the pool when the plan takes the storage over, as each
+        allocation says), the packed weights from _packed"""
         g = G.Graph(self, height, width, ("se", "maxpool", "d-convolutional"), "block type %r has no sm_90a kernel yet")
-        bufs = G.Buffers(g, lambda h, w, cs: (L.alloc_padded(batch, h, w, cs, device), None), 32)
+        # producers write the real channels of the interior; halo and padding channels are restored
+        bufs = G.Buffers(g, lambda h, w, cs: (pool.padded(batch, h, w, cs, None), None), 32)
         steps = []
         heads = []
         first_xs = None
         raw = {}          # owner block -> its RAW packed weight, shared by every `weight_from` use
         phase = {}        # (role, shape) -> phase-layout scratch of the dilated convs (the steps run in order)
 
-        def phase_buf(role, nb, h, w, cs):
+        def phase_buf(role, nb, h, w, cs, c):
             key = (role, nb, h, w, cs)
             if key not in phase:
-                phase[key] = L.alloc_padded(nb, h, w, cs, device)
+                phase[key] = pool.padded(nb, h, w, cs, c)     # split / conv write channels < c; the rest is restored
             return phase[key]
 
         for t, i in g.ops:
@@ -292,11 +356,11 @@ class Darknet(nn.Module):
                     # the shortcut that follows it is added by the merge
                     dh, dw = cv.dil
                     nb, hp, wp = batch * dh * dw, -(-src.h // dh), -(-src.w // dw)
-                    xp = phase_buf("x", nb, hp, wp, L.round_up(src.c, 64))
-                    yp = phase_buf("y", nb, hp, wp, L.round_up(cout, 32))
+                    xp = phase_buf("x", nb, hp, wp, L.round_up(src.c, 64), src.c)
+                    yp = phase_buf("y", nb, hp, wp, L.round_up(cout, 32), cout)
                     desc = L.make_desc(nb, hp, wp, src.c, xp.shape[-1], cout, yp.shape[-1], 3, 1, False, 0.0)
                     if cv.owner not in raw:
-                        raw[cv.owner] = L.pack_weights(desc, wt)
+                        raw[cv.owner] = self._packed(("raw", cv.owner), desc, wt)
                     out = bufs.out(cv.mat)[0]
                     res = bufs.view(cv.shortcut) if cv.fuse_res else None
                     steps.append(("dsplit", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c, dh=dh, dw=dw, xp=xp,
@@ -316,7 +380,7 @@ class Darknet(nn.Module):
                     if first_s2d:
                         # layer 0 feeds only the stride-2 layer 1: write its output directly in that layer's
                         # space-to-depth layout (no [B, H+2, W+2, 32] tensor, no s2d pass over it)
-                        first_xs = L.alloc_padded(batch, height // 2, width // 2, L.round_up(4 * cout, 64), device)
+                        first_xs = pool.padded(batch, height // 2, width // 2, L.round_up(4 * cout, 64), 4 * cout)
                         v = bufs.views[0] = G.View(None, 0, cout, height, width)
                     else:
                         v = bufs.out(0)[0]
@@ -332,7 +396,7 @@ class Darknet(nn.Module):
                     if i == 1 and first_xs is not None:
                         xs = first_xs                      # already written by the first-layer kernel
                     else:
-                        xs = L.alloc_padded(batch, src.h // 2, src.w // 2, L.round_up(4 * src.c, 64), device)
+                        xs = pool.padded(batch, src.h // 2, src.w // 2, L.round_up(4 * src.c, 64), 4 * src.c)
                         steps.append(("s2d", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c, xs=xs, keep=src)))
                     desc = L.make_desc(batch, src.h // 2, src.w // 2, 4 * src.c, xs.shape[-1], cout, 0, 2, 1,
                                        slope is not None, slope if slope is not None else 0.0, fuse_res, 0, fuse_up, is_head)
@@ -343,7 +407,7 @@ class Darknet(nn.Module):
                                        slope if slope is not None else 0.0, fuse_res, 0, fuse_up, is_head)
                 res = None
                 if is_head:
-                    out = torch.empty((batch, cout, oh, ow), dtype=torch.float32, device=device)
+                    out = pool.take((batch, cout, oh, ow), torch.float32)      # every element written by the head conv
                     out_ptr = out.data_ptr()
                     heads.append((i, out))
                 else:
@@ -355,10 +419,10 @@ class Darknet(nn.Module):
                         desc.res_stride = res.cs
                 if cv.owner is not None:
                     if cv.owner not in raw:
-                        raw[cv.owner] = L.pack_weights(desc, wt)
+                        raw[cv.owner] = self._packed(("raw", cv.owner), desc, wt)
                     pw = raw[cv.owner]
                 else:
-                    pw = L.pack_weights(desc, wt, scale)
+                    pw = self._packed(("folded", i), desc, wt, scale)
                 pb = L.padded_bias(desc, bias)
                 steps.append(("conv", dict(desc=desc, x=x_ptr, w=pw, b=pb, y=out_ptr,
                                            r=res.ptr if res is not None else None, keep=(src, res, out))))
@@ -375,27 +439,30 @@ class Darknet(nn.Module):
                     steps.append(("se_fwd", dict(x=src.ptr, xcs=src.cs, u=v.ptr, ucs=v.cs, h=src.h, w=src.w, c=src.c,
                                                  w1=fc[0].weight.detach().float().contiguous(),
                                                  w2=fc[2].weight.detach().float().contiguous(), cr=cr,
-                                                 m=torch.zeros(batch * src.c, dtype=torch.float32, device=device),
-                                                 p=torch.zeros(batch * cr, dtype=torch.float32, device=device),
-                                                 s=torch.zeros(batch * src.c, dtype=torch.float32, device=device),
-                                                 ws=torch.empty(_lib.lib.ryolo_se_workspace_bytes(batch, src.h, src.w,
-                                                                                                  src.c, cr),
-                                                                dtype=torch.uint8, device=device), keep=(src, v))))
+                                                 # outputs of ryolo_se_fwd and its workspace: written every forward
+                                                 m=pool.take((batch * src.c,), torch.float32),
+                                                 p=pool.take((batch * cr,), torch.float32),
+                                                 s=pool.take((batch * src.c,), torch.float32),
+                                                 ws=pool.take((_lib.lib.ryolo_se_workspace_bytes(batch, src.h, src.w,
+                                                                                                 src.c, cr),), torch.uint8),
+                                                 keep=(src, v))))
                     continue
                 # otherwise the scale is applied IN PLACE: nothing else reads the unscaled tensor
                 steps.append(("se", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c,
                                          w1=fc[0].weight.detach().float().contiguous(),
                                          w2=fc[2].weight.detach().float().contiguous(), cr=fc[0].weight.shape[0],
-                                         sums=torch.zeros(batch * src.c, dtype=torch.float32, device=device),
-                                         scale=torch.zeros(batch * src.c, dtype=torch.float32, device=device), keep=src)))
+                                         # ryolo_se_block zeroes sums and writes scale every forward
+                                         sums=pool.take((batch * src.c,), torch.float32),
+                                         scale=pool.take((batch * src.c,), torch.float32), keep=src)))
                 bufs.views[i] = src
             else:                                        # maxpool
                 src = bufs.view(i - 1)
                 v = bufs.out(i)[0]
                 steps.append(("maxpool", dict(x=src.ptr, xcs=src.cs, h=src.h, w=src.w, c=src.c,
                                               stride=int(g.defs[i]["stride"]), y=v.ptr, ycs=v.cs, keep=(src, v))))
+        pool.channels(bufs.channels)
         rows = [self.module_list[j].na * g.shape[j][1] * g.shape[j][2] for j in self.yolo_layers]
-        return dict(steps=steps, heads=heads, rows=rows, img=(height, width))
+        return dict(steps=steps, heads=heads, rows=rows, img=(height, width), graph=None)
 
     # ------------------------------------------------------------------------------------------------------
     def forward(self, x, var=None):
@@ -423,10 +490,15 @@ class Darknet(nn.Module):
             # reference models.py:192-194, 290-292: list of raw [B, na, ny, nx, nc+6] tensors; differentiable
             from .train_path import DarknetTrainFn, TrainPlan
             with torch.cuda.device(x.device):
-                if self._tplan is None or self._tplan_key != key:
-                    self._tplan = TrainPlan(self, b, h, w, x.device)
-                    self._tplan_key = key
-                raw = DarknetTrainFn.apply(self._tplan, x, *list(self.parameters()))     # fp32 NCHW head buffers
+                plan = self._tplans.get(key)
+                if plan is None:
+                    pool = self._pool("train", x.device)
+                    plan, halo = pool.build(lambda: TrainPlan(self, b, h, w, x.device, pool, self._tshared),
+                                            self._drop_train)
+                    plan.halo = halo
+                    self._tplans[key] = plan
+                self._tplan_cur = plan
+                raw = DarknetTrainFn.apply(plan, x, *list(self.parameters()))     # fp32 NCHW head buffers
                 outs = []
                 for t, yi in zip(raw, self.yolo_layers):
                     layer = self.module_list[yi]
@@ -438,23 +510,37 @@ class Darknet(nn.Module):
             # modified in place since (optimizer step, manual edits); train()/eval()/load_state_dict drop it explicitly
             if self._ver_tensors is None:      # walking the module tree costs ~1 ms; the tensor objects are stable
                 self._ver_tensors = list(self.parameters()) + list(self.buffers())
-            key = key + (sum(t._version for t in self._ver_tensors),)
-            if self._plan is None or self._plan_key != key:
-                self._plan = self._build_plan(b, h, w, x.device)
-                self._plan_key = key
-                self._graph = None
+            ver = sum(t._version for t in self._ver_tensors)
+            if ver != self._plans_ver:
+                self._plan = None
+                self._plans_ver = ver
+            # one eval pool per batch size: a caller may keep the heads of one batch while it runs single images
+            # (detect.py --multi-scale: batch 1 at changing sizes, one pool)
+            pool = self._pool(("eval", b), x.device)
+            plan = self._plans.get(key)
+            if plan is None:
+                plan, halo = pool.build(lambda: self._build_plan(b, h, w, x.device, pool), lambda: self._drop_eval(b))
+                plan["halo"] = halo
+                self._plans[key] = plan
+            self._plan_cur = plan
+            pool.activate(plan["halo"], _lib.stream_ptr(x.device))
             if self.use_cuda_graph:
-                if self._graph is None:
-                    self._x_static = x.clone()
-                    self._run_eval(self._x_static, b, h, w)          # warm-up (attribute calls, lazy inits) outside capture
+                if plan["graph"] is None:
+                    # the CUDA-graph input, copied before every replay; outside the pool: only plans that capture need it
+                    plan["x_static"] = x.clone()
+                    xs = plan["x_static"]
+                    self._run_eval(xs, b, h, w)          # warm-up (attribute calls, lazy inits) outside capture
                     torch.cuda.synchronize()
                     g = torch.cuda.CUDAGraph()
                     c0 = _lib.lib.ryolo_launch_count()
                     with torch.cuda.graph(g):
-                        self._graph_out = self._run_eval(self._x_static, b, h, w)
-                    self._graph = g
-                    self._graph_kernels = int(_lib.lib.ryolo_launch_count() - c0)
-                self._x_static.copy_(x)
+                        plan["graph_out"] = self._run_eval(xs, b, h, w)
+                    plan["graph"] = g
+                    plan["graph_kernels"] = int(_lib.lib.ryolo_launch_count() - c0)
+                xs = plan["x_static"]
+                self._graph, self._x_static = plan["graph"], xs
+                self._graph_out, self._graph_kernels = plan["graph_out"], plan["graph_kernels"]
+                xs.copy_(x)
                 self._graph.replay()
                 self.replayed_kernels += self._graph_kernels     # this library's kernels executed by the replay
                 return self._graph_out

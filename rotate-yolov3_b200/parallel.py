@@ -128,7 +128,7 @@ class DistributedDataParallel(torch.nn.Module):
         # reserved_sms: SMs the backward GEMMs leave to the concurrent NCCL kernels.  The default leaves every SM to the
         # GEMMs; the argument is for rank counts where the all-reduce competes with them
         module._ddp = {"bucket_bytes": int(bucket_mb * (1 << 20)), "group": process_group, "reserved_sms": int(reserved_sms)}
-        module._tplan = None          # the plan builds its buckets at construction
+        module.drop_training_plans()  # the plans build their buckets at construction
         module._pplan = None
 
     def forward(self, *a, **k):

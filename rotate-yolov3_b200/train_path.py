@@ -16,12 +16,14 @@ Like stock autograd, the backward follows ``requires_grad``: each trainable mask
 (``Schedule``) that runs only the launches whose results reach a trainable parameter (reference train.py:120-135 and
 :215-220 freeze all but the heads, or the backbone)."""
 import ctypes
+import weakref
 
 import torch
 
 from . import _lib
 from . import graph as G
 from . import layout as L
+from .pool import ActivationPool
 
 _EPS = 1e-5
 
@@ -31,18 +33,31 @@ class _Block:
 
 
 class TrainPlan:
-    def __init__(self, model, batch, height, width, device):
+    """The training step at one (batch, height, width).  Its shape-sized storage comes from `pool` (the model's training
+    ActivationPool, shared with the plans of its other shapes; None: zeroed tensors of its own), its parameter-sized
+    device state -- packed weights, gradient arena, split-K weight-gradient arena, all-reduce buckets -- from `shared`, a
+    dict the model keeps once for the plans of every shape.
+
+    Every zero-initialised buffer is either rewritten by every step before it is read, or restored by the pool when the
+    plan takes the storage over (``ActivationPool.padded``: the halo and the channels no kernel writes); each
+    allocation below says which."""
+
+    def __init__(self, model, batch, height, width, device, pool=None, shared=None):
         self.model, self.batch, self.h, self.w, self.device = model, batch, height, width, device
+        self.pool = pool if pool is not None else ActivationPool(device)
+        self.shared = shared if shared is not None else {}
+        self.halo = None             # the pool's restore table of this plan (set by the model)
+        P = self.pool
         g = G.Graph(model, height, width, ("se", "d-convolutional"), "block type %r has no training kernel")
         if not model.yolo_layers and any(cv.is_head for cv in g.convs.values()):
             # the head bookkeeping (create_grids, the gradients autograd hands back) zips the heads with yolo_layers
             raise NotImplementedError("training needs the YOLO layers of the graph; YOLO-less trunks run in eval only")
-        # activation buffers (y) and their gradient twins; concat groups share one buffer
-        bufs = G.Buffers(g, lambda hh, ww, cs: (L.alloc_padded(batch, hh, ww, cs, device),
-                                                L.alloc_padded(batch, hh, ww, cs, device)), 32)
+        # activation buffers (y) and their gradient twins; concat groups share one buffer.  Interior real channels: the
+        # producer (y) / the first backward writer (gy) writes them every step; halo and padding channels are restored
+        bufs = G.Buffers(g, lambda hh, ww, cs: (P.padded(batch, hh, ww, cs, None), P.padded(batch, hh, ww, cs, None)), 32)
 
-        # first layer input: im2col of the image (27 real channels in a 64-channel padded NHWC buffer)
-        self.col = L.alloc_padded(batch, height, width, 64, device)
+        # first layer input: im2col of the image (27 real channels in a 64-channel padded NHWC buffer); restored beyond 27
+        self.col = P.padded(batch, height, width, 64, 27)
         blocks = []
         self.phase = {}          # (role, shape) -> phase-layout scratch of the dilated convs (blocks run one at a time)
         for t, i in g.ops:
@@ -64,11 +79,14 @@ class TrainPlan:
                 blk.cin = blk.src.c
                 blk.cin_pad = L.round_up(blk.cin, 64)
                 if blk.is_head:
-                    blk.out = torch.empty((batch, blk.cout, blk.oh, blk.ow), dtype=torch.float32, device=device)
-                    blk.dz = L.alloc_padded(batch, blk.oh, blk.ow, blk.zcs, device)   # gradient of the head output
+                    # fp32 NCHW head output: every element written by the head conv every step
+                    blk.out = P.take((batch, blk.cout, blk.oh, blk.ow), torch.float32)
+                    # gradient of the head output: ryolo_head_grad_nchw_to_padded writes channels < cout; rest restored
+                    blk.dz = P.padded(batch, blk.oh, blk.ow, blk.zcs, blk.cout)
                     blk.res = blk.gres = None
                 else:
-                    blk.z = L.alloc_padded(batch, blk.oh, blk.ow, blk.zcs, device)     # raw conv output / dz
+                    # raw conv output / dz: the conv (or the weight_from block's bn_act_bwd) writes channels < cout
+                    blk.z = P.padded(batch, blk.oh, blk.ow, blk.zcs, blk.cout)
                     blk.y, blk.gy = bufs.out(blk.mat)
                     if blk.fuse_res:
                         blk.res, blk.gres = bufs.view(blk.shortcut), bufs.gview(blk.shortcut)
@@ -81,8 +99,9 @@ class TrainPlan:
                 if blk.s2d:
                     # 3x3/stride-2 block on the space-to-depth copy of its input: 2x2 taps, 4C channels, stride 1
                     blk.xs_cs = L.round_up(4 * blk.src.c, 64)
-                    blk.xs = L.alloc_padded(batch, blk.src.h // 2, blk.src.w // 2, blk.xs_cs, device)
-                    blk.dxs = L.alloc_padded(batch, blk.src.h // 2, blk.src.w // 2, blk.xs_cs, device)
+                    # space-to-depth input and its dgrad output: channels < 4C written every step, the rest restored
+                    blk.xs = P.padded(batch, blk.src.h // 2, blk.src.w // 2, blk.xs_cs, 4 * blk.src.c)
+                    blk.dxs = P.padded(batch, blk.src.h // 2, blk.src.w // 2, blk.xs_cs, 4 * blk.src.c)
                     blk.k_eff = 2
                     blk.cin_eff, blk.cin_pad = 4 * blk.src.c, blk.xs_cs
                     blk.fdesc = L.make_desc(batch, blk.src.h // 2, blk.src.w // 2, blk.cin_eff, blk.xs_cs, blk.cout,
@@ -92,7 +111,8 @@ class TrainPlan:
                 else:
                     blk.cin_eff = blk.cin
                     if blk.stride == 2:
-                        blk.dz_up = L.alloc_padded(batch, blk.src.h, blk.src.w, blk.zcs, device)  # zero-inserted dz
+                        # zero-inserted dz: ryolo_zero_insert2x writes the even pixels only, the whole buffer is restored
+                        blk.dz_up = P.padded(batch, blk.src.h, blk.src.w, blk.zcs, 0)
                     # forward descriptor: raw conv (no bias / activation); heads keep their bias and write fp32 NCHW
                     blk.fdesc = L.make_desc(batch, blk.src.h, blk.src.w, blk.cin, blk.src.cs, blk.cout,
                                             0 if blk.is_head else blk.zcs, blk.k_eff, blk.stride, False, 0.0, False, 0,
@@ -107,11 +127,11 @@ class TrainPlan:
                 if blk.owner is not None:
                     blocks.append(blk)           # shares the owner's pw / pwd / dw (set below)
                     continue
-                blk.pw = torch.empty(_lib.lib.ryolo_conv_packed_weight_bytes(ctypes.byref(blk.fdesc)), dtype=torch.uint8,
-                                     device=device)
+                # packed weight operands: repacked by every forward (_pack_all), shared by the plans of every shape
+                blk.pw = self._shared_bytes(("pw", i), _lib.lib.ryolo_conv_packed_weight_bytes(ctypes.byref(blk.fdesc)))
                 if i > 0:
-                    blk.pwd = torch.empty(_lib.lib.ryolo_conv_packed_weight_bytes(ctypes.byref(blk.ddesc)), dtype=torch.uint8,
-                                          device=device)
+                    blk.pwd = self._shared_bytes(("pwd", i),
+                                                 _lib.lib.ryolo_conv_packed_weight_bytes(ctypes.byref(blk.ddesc)))
                 blocks.append(blk)
             else:
                 # out of place: u = x * s gets a buffer pair of its own and views[i]; views[i - 1] stays x, so that the
@@ -125,10 +145,12 @@ class TrainPlan:
                 se.i, se.x, se.gx, se.c, se.h, se.w = i, x, gx, x.c, x.h, x.w
                 se.cr = model.module_list[i].fc[0].weight.shape[0]
                 se.u, se.gu = bufs.out(i)
-                se.m, se.s, se.ds, se.dm = (torch.zeros(batch * x.c, dtype=torch.float32, device=device) for _ in range(4))
-                se.p = torch.zeros(batch * se.cr, dtype=torch.float32, device=device)
+                # SE scratch: outputs of ryolo_se_fwd (m, p, s) and ryolo_se_bwd (ds, dm), written every step
+                se.m, se.s, se.ds, se.dm = (P.take((batch * x.c,), torch.float32) for _ in range(4))
+                se.p = P.take((batch * se.cr,), torch.float32)
                 prod[0].se = se
         self.blocks = blocks
+        P.channels(bufs.channels)
         by_index = {b.i: b for b in blocks}
         for b in blocks:
             if b.owner is not None:
@@ -146,8 +168,9 @@ class TrainPlan:
                 b.invstd.fill_(1.0)
         self.scratch_sums = torch.zeros(2 * 2048 + 1, dtype=torch.float32, device=device)
         ses = [b.se for b in blocks if b.se is not None]
-        self.se_ws = torch.empty(max([_lib.lib.ryolo_se_workspace_bytes(batch, se.h, se.w, se.c, se.cr) for se in ses] + [0]),
-                                 dtype=torch.uint8, device=device)
+        # SE workspace: written before it is read within each launch
+        self.se_ws = P.take((max([_lib.lib.ryolo_se_workspace_bytes(batch, se.h, se.w, se.c, se.cr) for se in ses] + [0]),),
+                            torch.uint8)
         # a block whose output feeds a space-to-depth (3x3 / stride 2) block writes the s2d copy itself (bn_act_fwd_s2d)
         for c_ in blocks:
             c_.xs_from_producer = False
@@ -187,7 +210,8 @@ class TrainPlan:
             if blk.owner is None:
                 blk.dw_off = off
                 off += L.round_up(blk.dw_shape[0] * blk.dw_shape[1] * blk.dw_shape[2], 64)
-        self.dw_arena = torch.zeros(off, dtype=torch.float32, device=device)
+        # its used ranges are zeroed at the start of every backward (_backward_segment)
+        self.dw_arena = self._shared_zeros("dw_arena", off)
         for blk in blocks:
             if blk.owner is None:
                 n_ = blk.dw_shape[0] * blk.dw_shape[1] * blk.dw_shape[2]
@@ -198,8 +222,6 @@ class TrainPlan:
         self._key_now = None
         self.schedules = {}          # trainable mask -> Schedule
         self.sched = self._schedule((True,) * len(self.names))
-        self.gen = 0                 # forward generation: backward must see the activations of ITS forward
-        self.consumed = True
         self.graphs = None           # CUDA graphs of forward / backward segments (model.use_cuda_graph)
         self.replayed_kernels = 0    # kernels of this library executed through CUDA-graph replays (bench.py gpu_launches)
         self.time_comm = False       # bench.py: record events around the wait for the all-reduces (exposed time)
@@ -257,7 +279,8 @@ class TrainPlan:
                                                       if k in self.param_slots]))
             bounds.append(off)
             blk.arena_end = off
-        self.garena = torch.zeros(off, dtype=torch.float32, device=self.device)
+        # every gradient the backward hands out is written by that backward before it is copied out
+        self.garena = self._shared_zeros("garena", off)
         for blk in self.blocks:
             if blk.owner is not None:
                 continue
@@ -272,6 +295,19 @@ class TrainPlan:
                 se.gw2 = self.garena[se.gw2_off:se.gw2_off + n]
         self.bounds = bounds
         self.names = [nm for nm, _ in m.named_parameters()]
+
+    def _shared_bytes(self, key, nbytes):
+        """parameter-sized uint8 device state of the model, one per (key, size) for the plans of every shape"""
+        k = key + (nbytes,)
+        if k not in self.shared:
+            self.shared[k] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return self.shared[k]
+
+    def _shared_zeros(self, key, n):
+        k = (key, n)
+        if k not in self.shared:
+            self.shared[k] = torch.zeros(n, dtype=torch.float32, device=self.device)
+        return self.shared[k]
 
     @property
     def buckets(self):
@@ -470,12 +506,14 @@ class TrainPlan:
             if (layer.nx, layer.ny) != (blk.ow, blk.oh):
                 layer.create_grids((self.h, self.w), (blk.ow, blk.oh), self.device, torch.float32)
         self._key_now = self._param_key()      # once per step: storage identity of parameters / buffers
+        if self.halo is not None:              # the pool served another plan since this plan's last step
+            self.pool.activate(self.halo, _lib.stream_ptr(self.device))
         if getattr(m, "use_cuda_graph", False):
             outs = self._forward_graph(x)
         else:
             outs = self._forward_body(x)
-        self.gen += 1
-        self.consumed = False
+        self.pool.gen += 1
+        self.pool.consumed = False
         return outs
 
     # ---- CUDA-graph form (opt-in, model.use_cuda_graph): the ~1100 launches of a forward and the ~1300 of a backward are
@@ -486,7 +524,7 @@ class TrainPlan:
         key = (self._key_now, self.sched.mask)     # the pack table and the backward segments depend on the schedule
         if self.graphs is None or self.graphs["key"] != key:
             self.graphs = {"key": key, "pool": None}
-            self.x_static = x.clone()
+            self.x_static = x.clone()          # outside the pool: only plans that capture need it
             eager = self._forward_body(self.x_static)         # this call's forward, eagerly (also the capture warm-up)
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
@@ -606,10 +644,11 @@ class TrainPlan:
     # into the owner's dw and the dgrad runs on the owner's pwd.  A dilated 3x3 conv (dh, dw) is an ordinary 3x3 conv on
     # the dh*dw phase images of its input (ryolo_dilate_split); the merge is the split's adjoint, so the backward splits
     # dz, runs wgrad / dgrad on the phase images and merges dx into the source gradient.
-    def _phase_buf(self, role, nb, h, w, cs):
+    def _phase_buf(self, role, nb, h, w, cs, blk_c):
         key = (role, nb, h, w, cs)
         if key not in self.phase:
-            self.phase[key] = L.alloc_padded(nb, h, w, cs, self.device)
+            # z / dx phase images: the split / the dgrad writes channels < the real count, the rest is restored
+            self.phase[key] = self.pool.padded(nb, h, w, cs, blk_c)
         return self.phase[key]
 
     def _linear_block(self, blk, batch, device):
@@ -624,9 +663,10 @@ class TrainPlan:
             return
         dh, dw = blk.dil
         blk.nb, blk.hp, blk.wp = batch * dh * dw, -(-blk.src.h // dh), -(-blk.src.w // dw)
-        blk.xp = L.alloc_padded(blk.nb, blk.hp, blk.wp, blk.cin_pad, device)       # kept for the wgrad
-        blk.zp = self._phase_buf("z", blk.nb, blk.hp, blk.wp, blk.zcs)
-        blk.dxp = self._phase_buf("dx", blk.nb, blk.hp, blk.wp, blk.cin_pad)
+        # kept for the wgrad; the split writes channels < cin of the interior (zero fill included), the rest is restored
+        blk.xp = self.pool.padded(blk.nb, blk.hp, blk.wp, blk.cin_pad, blk.cin)
+        blk.zp = self._phase_buf("z", blk.nb, blk.hp, blk.wp, blk.zcs, blk.cout)
+        blk.dxp = self._phase_buf("dx", blk.nb, blk.hp, blk.wp, blk.cin_pad, blk.cin)
         blk.fdesc = L.make_desc(blk.nb, blk.hp, blk.wp, blk.cin, blk.cin_pad, blk.cout, blk.zcs, 3, 1, False, 0.0)
         blk.ddesc = L.make_desc(blk.nb, blk.hp, blk.wp, blk.cout, blk.zcs, blk.cin, blk.cin_pad, 3, 1, False, 0.0)
 
@@ -750,7 +790,7 @@ class TrainPlan:
                 self._comm_ev = (e0, e1)
             # fresh tensors, trainable ranges only: autograd may keep what it is given
             outs = [self.garena[lo:hi] * inv for lo, hi in sch.ranges]
-        self.consumed = True
+        self.pool.consumed = True
         out = []
         for name in self.names:
             parts = name.split(".")            # module_list.{i}.{Module}.{param} (SE: module_list.{i}.fc.{0|2}.weight)
@@ -864,8 +904,13 @@ class Schedule:
                     self.range_of[k] = next(j for j, (a, b_) in enumerate(self.ranges) if a <= lo and hi <= b_)
         ddp = getattr(plan.model, "_ddp", None)
         from .parallel import GradBuckets
-        self.buckets = GradBuckets(plan.garena, plan.bounds, bucket_bytes=ddp["bucket_bytes"], group=ddp["group"],
-                                   ranges=self.ranges) if ddp else None
+        self.buckets = None
+        if ddp:              # one set per mask for the plans of every shape (they share the gradient arena)
+            bk = ("buckets", mask, plan.garena.numel())
+            if bk not in plan.shared:
+                plan.shared[bk] = GradBuckets(plan.garena, plan.bounds, bucket_bytes=ddp["bucket_bytes"],
+                                              group=ddp["group"], ranges=self.ranges)
+            self.buckets = plan.shared[bk]
         # backward segments = runs of blocks whose gradients complete one bucket (one segment without DDP); ready[s] is
         # the arena offset below which every gradient is final after segment s
         ends = sorted(hi for _, hi in self.buckets.buckets) if self.buckets else []
@@ -941,15 +986,20 @@ def check_activations(plan, gen):
 class DarknetTrainFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, plan, x, *params):
-        ctx.plan = plan
+        # weak: the head buffers returned below are the plan's own and carry this node as grad_fn, so a strong reference
+        # would keep every plan alive (and its pool storage, which growth must free) through that cycle
+        ctx.plan = weakref.ref(plan)
         outs = plan.forward(x, ctx.needs_input_grad[2:])
-        ctx.gen = plan.gen
+        ctx.gen = plan.pool.gen
         return tuple(outs)
 
     @staticmethod
     def backward(ctx, *grads):
-        plan = ctx.plan
-        check_activations(plan, ctx.gen)
+        plan = ctx.plan()
+        if plan is None:
+            raise RuntimeError("Darknet training plan: the plan of this forward was dropped (a larger shape grew the "
+                               "activation pool, or the model moved) before its backward")
+        plan.pool.check(ctx.gen)
         gl = []
         for g, blk, yi in zip(grads, plan.heads, plan.model.yolo_layers):
             if g is None:

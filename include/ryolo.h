@@ -515,6 +515,37 @@ int ryolo_px_depth_to_space(const float* dxs, int dxs_cstride, int batch, int h,
 int ryolo_px_split_from_nchw(const float* src, int batch, int c, int h, int w, void* dst,
                              int dst_cstride, int dst_lo, int nplanes, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Letterbox <- letterbox()                               utils/datasets.py:512-546
+ *              LoadImages / LoadImagesAndLabels normalisation   utils/datasets.py:112-117, 498-500
+ * One launch letterboxes a batch of uint8 HWC BGR images of any sizes into out [njobs, 3, out_h, out_w]
+ * (RGB, value/255 by IEEE division, fp32 or fp16; border pixels 128/255), byte for byte what
+ * cv2.resize(INTER_AREA) + copyMakeBorder + the reference's normalisation compute.  jobs_dev and tables_dev
+ * are device memory built from shapes alone (rotate-yolov3_b200/preprocess.py).  A job's per-axis table at
+ * word offset xtab / ytab of tables_dev holds, per output index d, three int32 {start, count, woff}: the taps
+ * are source indices start + t (t < count; clipped to the image for RYOLO_LB_LINEAR) with weights at word
+ * offset xtab + woff (float32 for RYOLO_LB_AREA, int32 for RYOLO_LB_LINEAR, none for RYOLO_LB_AREA_INT).
+ * No resize is RYOLO_LB_AREA with one unit tap per pixel.  Requires top + dst_h <= out_h,
+ * left + dst_w <= out_w; njobs <= 65535.  Allocates nothing; capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+#define RYOLO_DT_F16 2
+#define RYOLO_LB_AREA 0     /* float32 area weights (non-integer downscale, or a copy)          */
+#define RYOLO_LB_AREA_INT 1 /* integer factors kx x ky: integer sums                             */
+#define RYOLO_LB_LINEAR 2   /* an axis upscales: 2-tap linear, 11-bit fixed-point weights        */
+typedef struct ryolo_letterbox_job {
+  const uint8_t* src;  /* [src_h, src_w, 3] BGR, pixels contiguous                            */
+  int64_t src_stride;  /* bytes between source rows                                           */
+  int32_t src_h, src_w;
+  int32_t dst_h, dst_w; /* resized (unpadded) size                                            */
+  int32_t top, left;    /* border above / left of the resized image                            */
+  int32_t kind;         /* RYOLO_LB_*                                                          */
+  int32_t kx, ky;       /* RYOLO_LB_AREA_INT factors                                           */
+  int32_t xtab, ytab;   /* word offsets of the per-axis tables in tables_dev                   */
+  int32_t reserved;
+} ryolo_letterbox_job;
+int ryolo_letterbox(const ryolo_letterbox_job* jobs_dev, int njobs, const int32_t* tables_dev, void* out,
+                    int out_h, int out_w, int out_dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

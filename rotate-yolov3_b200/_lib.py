@@ -14,6 +14,7 @@ IOU_MODE_IOU = 0
 IOU_MODE_GIOU = 1
 DT_BF16 = 0
 DT_F32 = 1
+DT_F16 = 2
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
@@ -52,6 +53,14 @@ class HaloJob(ctypes.Structure):
                 ("c_real", ctypes.c_int32), ("c_stride", ctypes.c_int32), ("reserved", ctypes.c_int32)]
 
 
+class LetterboxJob(ctypes.Structure):
+    """mirror of ryolo_letterbox_job"""
+    _fields_ = [("src", ctypes.c_void_p), ("src_stride", ctypes.c_int64), ("src_h", ctypes.c_int32),
+                ("src_w", ctypes.c_int32), ("dst_h", ctypes.c_int32), ("dst_w", ctypes.c_int32), ("top", ctypes.c_int32),
+                ("left", ctypes.c_int32), ("kind", ctypes.c_int32), ("kx", ctypes.c_int32), ("ky", ctypes.c_int32),
+                ("xtab", ctypes.c_int32), ("ytab", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
 # name -> (restype, argtypes); must list every symbol include/ryolo.h declares (tests/test_abi.py checks it)
 SIGNATURES = {
     "ryolo_abi_version": (_i, []),
@@ -81,6 +90,7 @@ SIGNATURES = {
     "ryolo_conv_unpack_wgrad": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_conv_pack_weights_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_zero_halo_multi": (_i, [_vp, _i, _vp]),
+    "ryolo_letterbox": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "ryolo_conv_unpack_wgrad_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_conv_bn_act_fwd": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_conv_first_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),

@@ -387,7 +387,8 @@ def dy_of(plan, blk, shift=0):
 
 # ---------------------------------------------------------------------------------------------------------------
 class Step:
-    pass
+    """one checked training step; batch, h, w default to the module's 608 step"""
+    batch, h, w = BATCH, SIZE, SIZE
 
 
 def _bn_of(model, blk):
@@ -407,12 +408,14 @@ def forward_checks(st):
     L = _layout()
     out = {}
     # im2col of the image: bit for bit, columns 27..63 and the halo zero
-    want_col = F.unfold(st.x, 3, padding=1).view(BATCH, 27, SIZE, SIZE).permute(0, 2, 3, 1).to(BF16)
+    want_col = F.unfold(st.x, 3, padding=1).view(st.batch, 27, st.h, st.w).permute(0, 2, 3, 1).to(BF16)
     st.im2col = dict(bits=bitwise(interior(plan.col, 0, 27), want_col),
                      pad_zero=bool((interior(plan.col, 27, 37) == 0).all()), halo=halo_zero(plan.col))
     # the multi-tensor pack against the single-operand pack into fresh buffers
     packs = []
     for blk in plan.blocks:
+        if blk.owner is not None:          # a weight_from block runs its owner's packed operands
+            continue
         w = _weight(model, blk)
         wf = w.reshape(blk.cout, 27, 1, 1).contiguous() if blk.i == 0 else w
         packs.append((blk.i, "fwd", torch.equal(blk.pw, L.pack_weights(blk.fdesc, wf, mode=2 if blk.s2d else 0))))
@@ -422,6 +425,8 @@ def forward_checks(st):
     ratios = []
     st.rv_biased = {}
     for blk in plan.blocks:
+        if blk.owner is not None:          # weight_from blocks: their own launches (test_dilated_train_f64_gpu.py)
+            continue
         r = {}
         w = _weight(model, blk)
         want, mag = fwd_ref(plan, blk, w)
@@ -438,18 +443,23 @@ def forward_checks(st):
         if blk.i in st.keep_fwd:
             st.stash[("z", blk.i)] = dict(want=want.clone(), mag=mag.clone(), n=n, got=z.clone())
         del want, mag
-        bn = _bn_of(model, blk)
-        rs, ratio = stats_check(z, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale, blk.shift, st.rm0[blk.i], st.rv0[blk.i],
-                                bn.running_mean, bn.running_var, bn.weight.detach(), bn.bias.detach(), bn.eps, bn.momentum,
-                                bn_chain(BATCH, blk.oh, blk.ow, blk.cout)["sums"])
-        r.update(rs)
-        r["mean_over_std"] = ratio
-        # the same check with the running variance taken as biased (n instead of n - 1): kept for the bound self-test
-        rb_, _ = stats_check(z, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale, blk.shift, st.rm0[blk.i], st.rv0[blk.i],
-                             bn.running_mean, bn.running_var, bn.weight.detach(), bn.bias.detach(), bn.eps, bn.momentum,
-                             bn_chain(BATCH, blk.oh, blk.ow, blk.cout)["sums"], unbiased=False)
-        st.rv_biased[blk.i] = max(rb_["running"], rb_["finalize"])
-        ratios.append(ratio)
+        if blk.has_bn:
+            bn = _bn_of(model, blk)
+            rs, ratio = stats_check(z, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale, blk.shift, st.rm0[blk.i],
+                                    st.rv0[blk.i], bn.running_mean, bn.running_var, bn.weight.detach(), bn.bias.detach(),
+                                    bn.eps, bn.momentum, bn_chain(st.batch, blk.oh, blk.ow, blk.cout)["sums"])
+            r.update(rs)
+            r["mean_over_std"] = ratio
+            # the same check with the running variance taken as biased (n instead of n - 1): kept for the bound self-test
+            rb_, _ = stats_check(z, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale, blk.shift, st.rm0[blk.i],
+                                 st.rv0[blk.i], bn.running_mean, bn.running_var, bn.weight.detach(), bn.bias.detach(),
+                                 bn.eps, bn.momentum, bn_chain(st.batch, blk.oh, blk.ow, blk.cout)["sums"], unbiased=False)
+            st.rv_biased[blk.i] = max(rb_["running"], rb_["finalize"])
+            ratios.append(ratio)
+        else:
+            # a bias (+ PReLU) conv without BatchNorm: fixed statistics, scale 1 and shift = the conv bias, bit for bit
+            bias = model.module_list[blk.i].Conv2d.bias.detach()
+            r["fixed_stats"] = bool((blk.scale == 1).all()) and torch.equal(blk.shift, bias)
         # bn_act_fwd
         res = vint(blk.res) if blk.res is not None else None
         want_y, t = bn_act_fwd_ref(z, blk.scale, blk.shift, _slope_of(model, blk), res)
@@ -509,17 +519,17 @@ def check_block_bwd(st, blk, orig):
     return r
 
 
-def _bwd_checks(st, blk, snap, r):
-    plan, model = st.plan, st.model
-    w = _weight(model, blk)
-    w64 = w.to(BF16).double()
+def dz_checks(st, blk, snap, r):
+    """the head cotangent's dz bit for bit, or bn_act_bwd of a BatchNorm block (dz, d beta, d gamma, d slope, the shortcut
+    gradient); returns dz"""
+    model = st.model
     if blk.is_head:
         dz = interior(blk.dz, 0, blk.cout)
         r["dz_bits"] = bitwise(dz, st.g_nhwc[blk.i].to(BF16))
         r["dz_pad_zero"] = bool((blk.dz[..., blk.cout:] == 0).all()) and halo_zero(blk.dz)
     else:
         dz = interior(blk.z, 0, blk.cout)
-        chain = bn_chain(BATCH, blk.oh, blk.ow, blk.cout, 2 if r["dy_mode"] == 2 and blk.cout // 8 * 2 <= 640 else 1)
+        chain = bn_chain(st.batch, blk.oh, blk.ow, blk.cout, 2 if r["dy_mode"] == 2 and blk.cout // 8 * 2 <= 640 else 1)
         rb, near = bn_bwd_check(snap["z"], snap["dy"], dz, blk.bsums, blk.mean, blk.invstd, blk.scale, blk.shift,
                                 _slope_of(model, blk), chain)
         r["dz"], r["dz_bias"] = rb["max"], rb["bias"]
@@ -537,6 +547,14 @@ def _bwd_checks(st, blk, snap, r):
             want = (snap["gres_prior"].float() + d).to(BF16) if blk.gres_acc else d.to(BF16)
             r["gres_bits"] = bitwise(vint(blk.gres), want)
         r["dz_halo"] = halo_zero(blk.z)
+    return dz
+
+
+def _bwd_checks(st, blk, snap, r):
+    plan, model = st.plan, st.model
+    w = _weight(model, blk)
+    w64 = w.to(BF16).double()
+    dz = dz_checks(st, blk, snap, r)
     # weight gradient (split-K layout) and its gather
     if blk.i == 0:
         x, offs, cin = interior(plan.col, 0, 27), [(0, 0)], 27
@@ -549,7 +567,7 @@ def _bwd_checks(st, blk, snap, r):
         offs = [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)]
     gh, gw_ = x.shape[1], x.shape[2]
     wr, wm = wgrad_ref(x, dz, offs)
-    plan_w = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, BATCH, gh, gw_, wgrad_test.gemm_sms())
+    plan_w = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, st.batch, gh, gw_, wgrad_test.gemm_sms())
     got = blk.dw[:, :blk.cout, :cin]
     # test_wgrad's random-walk bound (KAPPA sqrt(n_add) 2^-24 A) is reported, not required: on the step's operands the
     # accumulator's truncations do not cancel

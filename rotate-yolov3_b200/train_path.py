@@ -26,6 +26,9 @@ from . import layout as L
 from .pool import ActivationPool
 
 _EPS = 1e-5
+# the widest head the training backward takes: ryolo_head_grad_nchw_to_padded / ryolo_head_bias_grad reject c > 2048
+# (csrc/loss.cu); 72 anchors per head allow up to 22 classes
+HEAD_GRAD_MAX_CHANNELS = 2048
 
 
 class _Block:
@@ -52,6 +55,12 @@ class TrainPlan:
         if not model.yolo_layers and any(cv.is_head for cv in g.convs.values()):
             # the head bookkeeping (create_grids, the gradients autograd hands back) zips the heads with yolo_layers
             raise NotImplementedError("training needs the YOLO layers of the graph; YOLO-less trunks run in eval only")
+        wide = [(i, cv.cout) for i, cv in sorted(g.convs.items()) if cv.is_head and cv.cout > HEAD_GRAD_MAX_CHANNELS]
+        if wide:
+            # refused here, before any launch: the head cotangent's transpose would reject it in the middle of a backward
+            raise NotImplementedError("training heads are limited to %d channels (ryolo_head_grad_nchw_to_padded); "
+                                      "head conv(s) %s have more (anchors per head * (classes + 6)); such a model "
+                                      "runs in eval only" % (HEAD_GRAD_MAX_CHANNELS, wide))
         # activation buffers (y) and their gradient twins; concat groups share one buffer.  Interior real channels: the
         # producer (y) / the first backward writer (gy) writes them every step; halo and padding channels are restored
         bufs = G.Buffers(g, lambda hh, ww, cs: (P.padded(batch, hh, ww, cs, None), P.padded(batch, hh, ww, cs, None)), 32)

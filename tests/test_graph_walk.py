@@ -127,3 +127,20 @@ def test_plans_refuse_what_they_cannot_run():
         TrainPlan(m, 1, 32, 32, CPU)
     with pytest.raises(NotImplementedError, match="shortcut at block 3"):
         ParityPlan(m, 1, 32, 32, CPU, True)
+
+
+def test_training_refuses_heads_wider_than_the_head_gradient():
+    """72 anchors per head: 22 classes give 2016-channel heads (trains), 23 give 2088 (refused at plan build, naming
+    the limit, before any buffer or launch; eval still runs them, test_multiclass_f64_gpu.py)"""
+    import rotate_yolov3_b200 as pkg
+    from rotate_yolov3_b200 import cfgs
+    from rotate_yolov3_b200.train_path import HEAD_GRAD_MAX_CHANNELS, TrainPlan
+    assert HEAD_GRAD_MAX_CHANNELS == 2048
+    for nc, ok in ((22, True), (23, False)):
+        m = pkg.Darknet(cfgs.yolov3_cfg(width=64, height=64, classes=nc), {"context_factor": 1.0}, arc="default")
+        if ok:
+            plan = TrainPlan(m, 1, 64, 64, CPU)
+            assert [b.cout for b in plan.blocks if b.is_head] == [2016] * 3
+        else:
+            with pytest.raises(NotImplementedError, match=r"limited to 2048 channels.*\(81, 2088\), \(93, 2088\)"):
+                TrainPlan(m, 1, 64, 64, CPU)

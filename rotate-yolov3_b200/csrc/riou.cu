@@ -105,12 +105,14 @@ __device__ __forceinline__ float clamp_integral_area(const RBox& a, const RBox& 
   return fmaxf(0.5f * acc, 0.f);
 }
 
-// axis-aligned envelope of the 8 corners (mode 'giou', utils/utils.py:682-685)
+// axis-aligned envelope of the 8 corners (mode 'giou', utils/utils.py:682-685), taken relative to a's centre: at 1e5 px
+// cx +- extent rounds by up to 4e-3 px, which put the envelope of a 100 x 10 px pair 4e-4 off
 __device__ __forceinline__ float envelope_area(const RBox& a, const RBox& b) {
   const float ax = fabsf(a.c) * a.hw + fabsf(a.s) * a.hh, ay = fabsf(a.s) * a.hw + fabsf(a.c) * a.hh;
   const float bx = fabsf(b.c) * b.hw + fabsf(b.s) * b.hh, by = fabsf(b.s) * b.hw + fabsf(b.c) * b.hh;
-  const float x0 = fminf(a.cx - ax, b.cx - bx), x1 = fmaxf(a.cx + ax, b.cx + bx);
-  const float y0 = fminf(a.cy - ay, b.cy - by), y1 = fmaxf(a.cy + ay, b.cy + by);
+  const float dx = b.cx - a.cx, dy = b.cy - a.cy;
+  const float x0 = fminf(-ax, dx - bx), x1 = fmaxf(ax, dx + bx);
+  const float y0 = fminf(-ay, dy - by), y1 = fmaxf(ay, dy + by);
   return (x1 - x0) * (y1 - y0);
 }
 
@@ -175,12 +177,15 @@ struct RiouSmem {
 
 constexpr float FAR_AWAY = 1e18f;
 
+// row boxes (far > 0) are the frame of the clamp integral: canonical_frame, once per box.  SAT and envelope only see the
+// same rectangle.
 __device__ __forceinline__ void derive_box(const float* __restrict__ p, bool in_range, float far, float4& d0, float4& d1) {
   RBox bx;
   bool live = false;
   if (in_range) {
     bx = make_rbox(p);
     live = bx.rad >= 0.f;
+    if (far > 0.f) canonical_frame(bx.c, bx.s, bx.hw, bx.hh);
   }
   if (live) {
     d0 = make_float4(bx.cx, bx.cy, bx.rad * 1.0001f, bx.area);

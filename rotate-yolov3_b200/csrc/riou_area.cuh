@@ -55,7 +55,24 @@ RY_HD float clamp_edge_xdy(float ax, float ay, float ex, float ey, float rx, flo
   return ey * in;     // twice the contribution
 }
 
-// a: centre (acx, acy), cos/sin (ac, as), half extents (ahw, ahh); b likewise.  Returns area(a ∩ b) >= 0.
+// The frame box a should have its long side along y (canonical_frame): b's edges enter the integral weighted by ey, and each
+// breakpoint's rounding (~u in t) moves an edge's dY by ~u |ey|, multiplied by X in [0, 1].  With a thin box along x
+// crossed at a steep angle, |ey| reaches ~50 (b's length over a's height): two aspect-50 boxes crossing at 75 degrees put
+// the IoU 1e-6 off, past the 1e-4 relative + 1e-6 contract.  With a's long side along y, |ey| is at most b's length over
+// a's long side.
+RY_HD void canonical_frame(float& c, float& s, float& hw, float& hh) {
+  if (hw > hh) {   // the same rectangle turned by +90 degrees: exact (a swap and a negation)
+    const float t = c;
+    c = -s;
+    s = t;
+    const float h = hw;
+    hw = hh;
+    hh = h;
+  }
+}
+
+// a: centre (acx, acy), cos/sin (ac, as), half extents (ahw, ahh) in canonical_frame; b likewise (any frame).  Returns
+// area(a ∩ b) >= 0.
 RY_HD float clamp_integral_area2(float acx, float acy, float ac, float as, float ahw, float ahh, float bcx, float bcy,
                                  float bc, float bs, float bhw, float bhh) {
   const float dx = bcx - acx, dy = bcy - acy;

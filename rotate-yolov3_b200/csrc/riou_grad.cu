@@ -85,6 +85,18 @@ __device__ __forceinline__ void edge_terms(const GBox& in, const GBox& out, floa
   g[4] = gt;
 }
 
+// separated on one of the four box axes by more than the fp32 rounding of the projections (8 u of their scale)
+__device__ __forceinline__ bool separated(const GBox& a, const GBox& b) {
+  const float dx = b.cx - a.cx, dy = b.cy - a.cy;
+  const float C = fabsf(a.c * b.c + a.s * b.s), S = fabsf(a.c * b.s - a.s * b.c);
+  const float ha = 0.5f * a.w, ka = 0.5f * a.h, hb = 0.5f * b.w, kb = 0.5f * b.h;
+  const float slack = 4.76837158e-7f * (fabsf(dx) + fabsf(dy) + ha + ka + hb + kb);   // 8 * 2^-24
+  return fabsf(dx * a.c + dy * a.s) - (ha + hb * C + kb * S) > slack ||
+         fabsf(dy * a.c - dx * a.s) - (ka + hb * S + kb * C) > slack ||
+         fabsf(dx * b.c + dy * b.s) - (hb + ha * C + ka * S) > slack ||
+         fabsf(dy * b.c - dx * b.s) - (kb + ha * S + ka * C) > slack;
+}
+
 __global__ void __launch_bounds__(128) riou_grad_kernel(const float* __restrict__ a, const float* __restrict__ b, int n,
                                                         int sa, int sb, const float* __restrict__ gout,
                                                         float* __restrict__ iou_out, float* __restrict__ ga,
@@ -102,18 +114,30 @@ __global__ void __launch_bounds__(128) riou_grad_kernel(const float* __restrict_
   // 2 I = w_a I_wa + h_a I_ha + w_b I_wb + h_b I_hb + (c_b − c_a)·∇_{c_b} I), but that sum counts a run where an edge of a
   // lies ON an edge of b twice (once in each box's terms) -- exactly the axis-aligned, equal-height boxes detection data is
   // full of; there the gradient is one-sided anyway, the value must still be right.
-  float I = clamp_integral_area2(A.cx, A.cy, A.c, A.s, 0.5f * A.w, 0.5f * A.h, B.cx, B.cy, B.c, B.s, 0.5f * B.w, 0.5f * B.h);
+  float fc = A.c, fs = A.s, fhw = 0.5f * A.w, fhh = 0.5f * A.h;
+  canonical_frame(fc, fs, fhw, fhh);
+  float I = clamp_integral_area2(A.cx, A.cy, fc, fs, fhw, fhh, B.cx, B.cy, B.c, B.s, 0.5f * B.w, 0.5f * B.h);
   const float Aa = A.w * A.h, Ab = B.w * B.h;
   const bool finite = isfinite(pa[0]) && isfinite(pa[1]) && isfinite(pa[2]) && isfinite(pa[3]) && isfinite(pa[4]) &&
                       isfinite(pb[0]) && isfinite(pb[1]) && isfinite(pb[2]) && isfinite(pb[3]) && isfinite(pb[4]);
   I = fminf(fmaxf(I, 0.f), fminf(Aa, Ab));
   const float U = Aa + Ab - I;
-  const bool live = finite && Aa > 0.f && Ab > 0.f && U > 0.f;
+  // Separated boxes have IoU 0 and zero gradients, whatever rounding residue the clamp integral leaves for them (a few
+  // 1e-7 of the areas): that residue would otherwise turn into a w / h gradient through the union.
+  const bool live = finite && Aa > 0.f && Ab > 0.f && U > 0.f && !separated(A, B);
   const float iou = live ? I / U : 0.f;
   if (iou_out) iou_out[i] = iou;
+  if (!live) {   // disjoint, zero-area or invalid: the edge terms may hold inf or NaN, so no 0 * dI here
+#pragma unroll
+    for (int k = 0; k < 5; k++) {
+      if (ga) ga[(size_t)i * 5 + k] = 0.f;
+      if (gb) gb[(size_t)i * 5 + k] = 0.f;
+    }
+    return;
+  }
   const float go = gout ? gout[i] : 1.f;
-  const float k1 = live ? go * (U + I) / (U * U) : 0.f;     // multiplies dI
-  const float k2 = live ? go * I / (U * U) : 0.f;           // multiplies dA
+  const float k1 = go * (U + I) / (U * U);     // multiplies dI
+  const float k2 = go * I / (U * U);           // multiplies dA
   // sign of w, h: the box uses |w|, |h|
   const float swa = pa[2] < 0.f ? -1.f : 1.f, sha = pa[3] < 0.f ? -1.f : 1.f;
   const float swb = pb[2] < 0.f ? -1.f : 1.f, shb = pb[3] < 0.f ? -1.f : 1.f;

@@ -52,6 +52,12 @@ def rotated_iou_matrix(a, b, GIoU=False, out=None):
     n, m = a.shape[0], b.shape[0]
     if out is None:
         out = torch.empty((n, m), dtype=torch.float32, device=a.device)
+    elif (out.dtype != torch.float32 or tuple(out.shape) != (n, m) or out.device != a.device
+          or not out.is_contiguous()):
+        # the kernel writes out as a dense row-major fp32 [n, m] block
+        raise ValueError("rotated_iou_matrix: out must be a contiguous float32 [%d, %d] tensor on %s, got %s %s %s%s"
+                         % (n, m, a.device, out.dtype, tuple(out.shape), out.device,
+                            "" if out.is_contiguous() else " (not contiguous)"))
     if n == 0 or m == 0:
         return out
     sa = a.stride(0) if n > 1 else a.shape[1]
@@ -69,6 +75,7 @@ class _RotatedIoU(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, a, b):
+        ctx.in_meta = ((a.shape, a.dtype), (b.shape, b.dtype))
         a = a[:, :5].contiguous().float()
         b = b[:, :5].contiguous().float()
         n = a.shape[0]
@@ -92,11 +99,21 @@ class _RotatedIoU(torch.autograd.Function):
                                                  _lib.ptr(ga) if ga is not None else None,
                                                  _lib.ptr(gb) if gb is not None else None, _lib.stream_ptr(a.device))
         _lib.check(st, "ryolo_riou_paired_grad")
-        return ga, gb
+        return _widen(ga, *ctx.in_meta[0]), _widen(gb, *ctx.in_meta[1])
+
+
+def _widen(g, shape, dtype):
+    """[N, 5] fp32 gradient -> the input's shape and dtype; the columns beyond the box get zero"""
+    if g is None or (g.shape == shape and g.dtype == dtype):
+        return g
+    full = torch.zeros(shape, dtype=dtype, device=g.device)
+    full[:, :5] = g
+    return full
 
 
 def rotated_iou(box1, box2):
-    """differentiable IoU of paired rotated boxes: box1, box2 [N, >=5] (cx, cy, w, h, theta) CUDA -> [N]"""
+    """differentiable IoU of paired rotated boxes: box1, box2 [N, >=5] (cx, cy, w, h, theta, ...) CUDA -> [N]; the
+    gradients have the inputs' shapes and dtypes (zero beyond column 5)"""
     if not (box1.is_cuda and box2.is_cuda):
         raise RuntimeError("rotated_iou needs CUDA tensors (sm_90a kernels, no CPU fallback)")
     return _RotatedIoU.apply(box1, box2)
@@ -104,7 +121,7 @@ def rotated_iou(box1, box2):
 
 def riou_loss(pred, target, reduction="mean"):
     """rotated-IoU regression loss 1 - IoU(pred, target) (the README's 'riou loss'; the reference's compute_loss uses
-    SmoothL1 + a horizontal wh_iou instead, SURVEY.md D1).  pred, target [N, 5]; gradients flow to both."""
+    SmoothL1 + a horizontal wh_iou instead, SURVEY.md D1).  pred, target [N, >=5] rows; gradients flow to both."""
     loss = 1.0 - rotated_iou(pred, target)
     if reduction == "mean":
         return loss.mean() if loss.numel() else loss.sum()

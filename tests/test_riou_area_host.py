@@ -27,7 +27,9 @@ static void gen(double* b, double canvas, int kind) {
   if (kind == 2) { b[4] = (rand() % 4) * M_PI / 2 - M_PI / 2; }
 }
 static float iou32(const float* a, const float* b) {
-  float inter = ryolo::clamp_integral_area2(a[0], a[1], cosf(a[4]), sinf(a[4]), 0.5f * a[2], 0.5f * a[3], b[0], b[1],
+  float c = cosf(a[4]), s = sinf(a[4]), hw = 0.5f * a[2], hh = 0.5f * a[3];
+  ryolo::canonical_frame(c, s, hw, hh);
+  float inter = ryolo::clamp_integral_area2(a[0], a[1], c, s, hw, hh, b[0], b[1],
                                             cosf(b[4]), sinf(b[4]), 0.5f * b[2], 0.5f * b[3]);
   const float aa = a[2] * a[3], ab = b[2] * b[3];
   inter = fminf(inter, fminf(aa, ab));

@@ -527,8 +527,11 @@ int ryolo_px_split_from_nchw(const float* src, int batch, int c, int h, int w, v
  * offset xtab + woff (float32 for RYOLO_LB_AREA, int32 for RYOLO_LB_LINEAR, none for RYOLO_LB_AREA_INT).
  * No resize is RYOLO_LB_AREA with one unit tap per pixel.  Requires top + dst_h <= out_h,
  * left + dst_w <= out_w; njobs <= 65535.  Allocates nothing; capturable in a CUDA graph.
+ * out_dtype RYOLO_DT_U8 writes the letterboxed uint8 image instead: out [njobs, out_h, out_w, 3] BGR, border 128
+ * (the training augmentation's intermediate; with top = left = 0 it is a plain batched resize).
  * ------------------------------------------------------------------------------------------ */
 #define RYOLO_DT_F16 2
+#define RYOLO_DT_U8 3
 #define RYOLO_LB_AREA 0     /* float32 area weights (non-integer downscale, or a copy)          */
 #define RYOLO_LB_AREA_INT 1 /* integer factors kx x ky: integer sums                             */
 #define RYOLO_LB_LINEAR 2   /* an axis upscales: 2-tap linear, 11-bit fixed-point weights        */
@@ -545,6 +548,45 @@ typedef struct ryolo_letterbox_job {
 } ryolo_letterbox_job;
 int ryolo_letterbox(const ryolo_letterbox_job* jobs_dev, int njobs, const int32_t* tables_dev, void* out,
                     int out_h, int out_w, int out_dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Training augmentation <- utils/augment.py random_affine, Gamma, HSV, HorizontalFlip, VerticalFlip
+ *                          and the LoadImagesAndLabels normalisation   utils/datasets.py:470-500
+ * Both launches run over a batch of letterboxed uint8 [h, w, 3] BGR images (ryolo_letterbox with RYOLO_DT_U8).
+ *
+ * ryolo_augment_warp: one job per image that is warped or whose maximum gamma needs.  warp = 1:
+ *   cv2.warpAffine(src, M, (w, h), INTER_LINEAR, border 128) into dst [h, w, 3] (rows of 3 * w bytes), given m,
+ *   the inverse of M as cv2 inverts it; cv2's fixed-point remap (10-bit AB, 5-bit INTER fractions, 15-bit
+ *   weights).  rowmax[image * h + y] = max over row y of dst (warp = 1) or of src (warp = 0, dst unused).
+ * ryolo_augment_finish: one job per image, job b writes out[b] [3, h, w] (RGB, /255, fp32 or fp16) from src
+ *   (the warped or letterboxed image): gamma uint8(pow(v / M, gamma) * M) with M = max of rowmax[b * h ..
+ *   b * h + h) (0 when M = 0), then cv2's 8-bit BGR2HSV, S and V scaled by the float32 factors and truncated,
+ *   8-bit HSV2BGR, then the flips, each when its flag is set.
+ * njobs <= 65535.  Allocate nothing; capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+#define RYOLO_AUG_GAMMA 1
+#define RYOLO_AUG_HSV 2
+#define RYOLO_AUG_HFLIP 4
+#define RYOLO_AUG_VFLIP 8
+typedef struct ryolo_warp_job {
+  const uint8_t* src;  /* [h, w, 3] BGR, rows of src_stride bytes                                */
+  uint8_t* dst;        /* [h, w, 3] BGR, rows of 3 * w bytes (warp = 1)                          */
+  int64_t src_stride;
+  double m[6];         /* dst -> src affine map, row major 2 x 3                                 */
+  int32_t warp;        /* 1: warp into dst and take its row maxima; 0: row maxima of src only   */
+  int32_t image;       /* row block of rowmax                                                    */
+} ryolo_warp_job;
+typedef struct ryolo_finish_job {
+  const uint8_t* src;  /* [h, w, 3] BGR, rows of src_stride bytes                                */
+  int64_t src_stride;
+  double gamma;        /* RYOLO_AUG_GAMMA exponent                                               */
+  float hsv_s, hsv_v;  /* RYOLO_AUG_HSV factors, >= 0                                            */
+  int32_t flags;       /* RYOLO_AUG_*                                                            */
+  int32_t reserved;
+} ryolo_finish_job;
+int ryolo_augment_warp(const ryolo_warp_job* jobs_dev, int njobs, uint8_t* rowmax, int h, int w, void* stream);
+int ryolo_augment_finish(const ryolo_finish_job* jobs_dev, int njobs, const uint8_t* rowmax, void* out, int h, int w,
+                         int out_dtype, void* stream);
 
 #ifdef __cplusplus
 }

@@ -9,6 +9,7 @@ from .iou import rotated_iou_matrix, skew_bbox_iou  # noqa: F401
 from .nms import nms_filter, non_max_suppression, r_nms  # noqa: F401
 from .models import Darknet, YOLOLayer  # noqa: F401
 from .preprocess import letterbox, letterbox_labels, scale_coords  # noqa: F401
+from .augment import train_batch  # noqa: F401
 
 __all__ = ["r_nms", "non_max_suppression", "nms_filter", "skew_bbox_iou", "rotated_iou_matrix", "Darknet", "YOLOLayer",
-           "letterbox", "letterbox_labels", "scale_coords"]
+           "letterbox", "letterbox_labels", "scale_coords", "train_batch"]

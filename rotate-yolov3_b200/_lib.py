@@ -15,6 +15,7 @@ IOU_MODE_GIOU = 1
 DT_BF16 = 0
 DT_F32 = 1
 DT_F16 = 2
+DT_U8 = 3
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
@@ -61,6 +62,19 @@ class LetterboxJob(ctypes.Structure):
                 ("xtab", ctypes.c_int32), ("ytab", ctypes.c_int32), ("reserved", ctypes.c_int32)]
 
 
+class WarpJob(ctypes.Structure):
+    """mirror of ryolo_warp_job"""
+    _fields_ = [("src", ctypes.c_void_p), ("dst", ctypes.c_void_p), ("src_stride", ctypes.c_int64),
+                ("m", ctypes.c_double * 6), ("warp", ctypes.c_int32), ("image", ctypes.c_int32)]
+
+
+class FinishJob(ctypes.Structure):
+    """mirror of ryolo_finish_job"""
+    _fields_ = [("src", ctypes.c_void_p), ("src_stride", ctypes.c_int64), ("gamma", ctypes.c_double),
+                ("hsv_s", ctypes.c_float), ("hsv_v", ctypes.c_float), ("flags", ctypes.c_int32),
+                ("reserved", ctypes.c_int32)]
+
+
 # name -> (restype, argtypes); must list every symbol include/ryolo.h declares (tests/test_abi.py checks it)
 SIGNATURES = {
     "ryolo_abi_version": (_i, []),
@@ -91,6 +105,8 @@ SIGNATURES = {
     "ryolo_conv_pack_weights_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_zero_halo_multi": (_i, [_vp, _i, _vp]),
     "ryolo_letterbox": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _vp]),
+    "ryolo_augment_warp": (_i, [_vp, _i, _vp, _i, _i, _vp]),
+    "ryolo_augment_finish": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "ryolo_conv_unpack_wgrad_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_conv_bn_act_fwd": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_conv_first_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),

@@ -13,6 +13,9 @@
 // The value v in [0, 255] becomes v / 255.f by IEEE division (numpy's float32 `/= 255.0`), and for fp16 that float32
 // quotient rounded to half (numpy's float16 `/=` computes in float32 and rounds once to half).
 //
+// RYOLO_DT_U8 writes the letterboxed uint8 image itself, [B, H, W, 3] BGR with border 128, for the training
+// augmentation that runs on it (csrc/augment.cu); the float outputs are untouched by that mode.
+//
 // One CTA per output row of one job (grid.y = job).  Consecutive threads take consecutive output pixels, so a warp
 // reads one contiguous span of each source row it needs and writes 32 consecutive elements of each output plane.
 #include <cuda_fp16.h>
@@ -130,6 +133,31 @@ __global__ void __launch_bounds__(kLbThreads)
   }
 }
 
+// the same pixels into a uint8 HWC BGR image per job: out [njobs, out_h, out_w, 3], border 128
+__global__ void __launch_bounds__(kLbThreads)
+    letterbox_u8_kernel(const ryolo_letterbox_job* __restrict__ jobs, const int* __restrict__ tab,
+                        uint8_t* __restrict__ out, int out_h, int out_w) {
+  const ryolo_letterbox_job jb = jobs[blockIdx.y];
+  const int y = blockIdx.x;
+  uint8_t* o = out + ((size_t)blockIdx.y * out_h + y) * out_w * 3;
+  const int yy = y - jb.top;
+  const bool row_in = yy >= 0 && yy < jb.dst_h;
+  for (int x = threadIdx.x; x < out_w; x += kLbThreads) {
+    const int xx = x - jb.left;
+    int v[3] = {128, 128, 128};
+    if (row_in && xx >= 0 && xx < jb.dst_w) {
+      if (jb.kind == RYOLO_LB_AREA) {
+        area_px(jb, tab, yy, xx, v);
+      } else if (jb.kind == RYOLO_LB_AREA_INT) {
+        area_int_px(jb, yy, xx, v);
+      } else {
+        linear_px(jb, tab, yy, xx, v);
+      }
+    }
+    o[3 * x] = (uint8_t)v[0], o[3 * x + 1] = (uint8_t)v[1], o[3 * x + 2] = (uint8_t)v[2];
+  }
+}
+
 }  // namespace ryolo
 
 using namespace ryolo;
@@ -138,9 +166,12 @@ extern "C" int ryolo_letterbox(const ryolo_letterbox_job* jobs_dev, int njobs, c
                                int out_h, int out_w, int out_dtype, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RYOLO_ARG_CHECK(jobs_dev && tables_dev && out && njobs > 0 && njobs <= 65535 && out_h > 0 && out_w > 0);
-  RYOLO_ARG_CHECK(out_dtype == RYOLO_DT_F32 || out_dtype == RYOLO_DT_F16);
+  RYOLO_ARG_CHECK(out_dtype == RYOLO_DT_F32 || out_dtype == RYOLO_DT_F16 || out_dtype == RYOLO_DT_U8);
   const dim3 grid(out_h, njobs);
-  if (out_dtype == RYOLO_DT_F32) {
+  if (out_dtype == RYOLO_DT_U8) {
+    letterbox_u8_kernel<<<grid, kLbThreads, 0, stream>>>(jobs_dev, tables_dev, static_cast<uint8_t*>(out), out_h,
+                                                         out_w);
+  } else if (out_dtype == RYOLO_DT_F32) {
     letterbox_kernel<float><<<grid, kLbThreads, 0, stream>>>(jobs_dev, tables_dev, static_cast<float*>(out), out_h,
                                                               out_w);
   } else {

@@ -94,6 +94,41 @@ def _linear_axis(ssize, dsize, scale, inv_scale, clamp_last):
     return starts, weights
 
 
+def _linear_resize_axis(ssize, dsize, scale):
+    """cv2.resize(INTER_LINEAR)'s coefficients for one axis: fx = float32((d + 0.5) * scale - 0.5), sx = floor(fx),
+    clamped to the image at both ends (fx = 0 there), and the 11-bit weights rint((1 - f) * 2048), rint(f * 2048)"""
+    starts, weights = [], []
+    for d in range(dsize):
+        fx = np.float32((d + 0.5) * scale - 0.5)
+        s = math.floor(fx)
+        f = np.float32(fx - np.float32(s))
+        if s < 0:
+            f, s = np.float32(0), 0
+        if s >= ssize - 1:
+            f, s = np.float32(0), ssize - 1
+        a0 = int(np.rint(np.float32(np.float32(1) - f) * np.float32(COEF_SCALE)))
+        a1 = int(np.rint(f * np.float32(COEF_SCALE)))
+        starts.append(s)
+        weights.append((a0, a1))
+    return starts, weights
+
+
+def linear_resize_tables(src_hw, dst_hw):
+    """The arithmetic path cv2.resize(INTER_LINEAR) takes for this pair of shapes, in resample_tables' format: an
+    exact 2x downscale on both axes runs as INTER_AREA's 2x2 block mean (AREA_INT), every other pair as LINEAR."""
+    (sh, sw), (dh, dw) = src_hw, dst_hw
+    sx, sy = 1.0 / (dw / sw), 1.0 / (dh / sh)
+    if (sh, sw) == (dh, dw):
+        return resample_tables(src_hw, dst_hw)
+    ix, iy = int(np.rint(sx)), int(np.rint(sy))
+    if ix == 2 and iy == 2 and abs(sx - ix) < DBL_EPSILON and abs(sy - iy) < DBL_EPSILON:
+        xs = ([2 * d for d in range(dw)], [2] * dw, None)
+        return AREA_INT, (2, 2), xs, ([2 * d for d in range(dh)], [2] * dh, None)
+    xs0, xw = _linear_resize_axis(sw, dw, sx)
+    ys0, yw = _linear_resize_axis(sh, dh, sy)
+    return LINEAR, (0, 0), (xs0, [2] * dw, xw), (ys0, [2] * dh, yw)
+
+
 def resample_tables(src_hw, dst_hw):
     """The arithmetic path cv2.resize(INTER_AREA) takes for this pair of shapes, and its per-axis tables.
 
@@ -138,8 +173,8 @@ def _pack_axis(tab, kind):
 
 
 @functools.lru_cache(maxsize=256)
-def _packed(src_hw, dst_hw):
-    kind, (kx, ky), xt, yt = resample_tables(src_hw, dst_hw)
+def _packed(src_hw, dst_hw, linear=False):
+    kind, (kx, ky), xt, yt = (linear_resize_tables if linear else resample_tables)(src_hw, dst_hw)
     return kind, kx, ky, _pack_axis(xt, kind), _pack_axis(yt, kind)
 
 

@@ -47,3 +47,19 @@ def darknet_case():
     x = torch.rand(4, 3, 128, 160, generator=torch.Generator().manual_seed(11))
     _, targets, hyp = base_inputs()
     return x, targets, focal_hyp(hyp, 0.5, hyp["obj_pw"])
+
+
+def cases():
+    """(golden tag, heads, targets, hyp) of cases (a)-(c)"""
+    heads, tg, hyp0 = base_inputs()
+    out = []
+    for gm in GAMMAS:
+        for pw in OBJ_PWS:
+            out.append(("a_g%g_pw%g" % (gm, pw), heads, tg, focal_hyp(hyp0, gm, pw)))
+        out.append(("b_g%g" % gm, heads, torch.zeros(0, 7), focal_hyp(hyp0, gm, hyp0["obj_pw"])))
+        out.append(("c_g%g" % gm, extreme_heads(heads), tg, focal_hyp(hyp0, gm, hyp0["obj_pw"])))
+    return out
+
+
+def golden():
+    return np.load(os.path.join(GOLDEN, "loss_focal_golden.npz"), allow_pickle=True)

@@ -221,13 +221,17 @@ def init_darknet_weights(model, seed=0):
 SMALL_ANCHORS = "ara 900, 3000, 9000 / 5.0 / -45, 45"   # 6 anchors: one area x 2 angles per scale (same angle set on every scale, as the reference loss assumes)
 
 
+def cfg_conv(f, k, s=1, bn=1, act="leaky"):
+    """one [convolutional] section of a Darknet cfg"""
+    return "[convolutional]\n%sfilters=%d\nsize=%d\nstride=%d\npad=1\nactivation=%s\n\n" % (
+        "batch_normalize=1\n" if bn else "", f, k, s, act)
+
+
 def mini_cfg(width=64, height=48):
     """A 19-block graph with every structural feature of cfg/yolov3.cfg (stride-2 convs, shortcuts, a route alias, an
     upsample, a 2-source concat whose second source also feeds a stride-2 conv, two YOLO heads) but only 13 convs, so
     that bf16 noise does not swamp a wiring check.  Reference 'ara' anchor grammar."""
-    def conv(f, k, s=1, bn=1, act="leaky"):
-        return "[convolutional]\n%sfilters=%d\nsize=%d\nstride=%d\npad=1\nactivation=%s\n\n" % (
-            "batch_normalize=1\n" if bn else "", f, k, s, act)
+    conv = cfg_conv
     def yolo(lo, hi):
         return "[yolo]\nmask = %d-%d\nanchors = %s\nclasses=1\nnum=6\n\n" % (lo, hi, SMALL_ANCHORS)
     s = "[net]\nwidth=%d\nheight=%d\nchannels=3\n\n" % (width, height)

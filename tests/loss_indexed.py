@@ -75,7 +75,6 @@ def build_targets(model, targets, hyp):
     return tcls, tbox, indices, av
 
 
-
 def compute_loss_indexed(p, targets, model, hyp):
     dev = p[0].device
     lcls = torch.zeros(1, device=dev)

@@ -2,150 +2,16 @@
 the kernels' arithmetic against cv2 and numpy live (INTER_LINEAR pre-resize tables, the fixed-point warp, the 8-bit
 HSV conversions over every colour and every HSV triplet, the gamma table), and the host half of ``train_batch``
 (draw replay, target rows) against the reference's own ``__getitem__`` / ``collate_fn`` (fixture)."""
-import os
 import random
 
 import numpy as np
 import pytest
 
-from helpers import GOLDEN
+from augment_cases import (DRAW_KEYS_NONE, GEN, Recorder, all_colours, aug_module, augment_golden, batch_case,
+                           bgr2hsv_np, f32, gamma_table_np, hsv2bgr_np, hsv_np, source, warp_np)
+from letterbox_cases import resize_np
 
-GOLD = os.path.join(GOLDEN, "augment_golden.npz")
-f32 = np.float32
 cv2 = pytest.importorskip("cv2")
-# a draw record in which nothing fires
-DRAW_KEYS_NONE = {"gray_alpha": 1.0, "affine": None, "noise": False, "gamma": None, "blur": False, "hsv": None,
-                  "hflip": False, "vflip": False, "grayscale": False}
-
-
-def _aug():
-    import rotate_yolov3_b200.augment as aug
-    return aug
-
-
-def _gold():
-    return np.load(GOLD)
-
-
-def _load_generator():
-    """the fixture generator as a module: its seeded sources, label rows and draw recorder are the tests' own, so the
-    two cannot drift apart (loading it imports neither the reference nor cv2)"""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("make_golden_augment", os.path.join(GOLDEN, "make_golden_augment.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-GEN = _load_generator()
-KINDS = ("random", "dim", "black")             # the fixture stores a source's kind as its index here
-Recorder = GEN.Recorder
-label_rows = GEN.label_rows
-
-
-def source(seed, h, w, kind=0):
-    return GEN.source(seed, h, w, KINDS[kind])
-
-
-def batch_case(g, name):
-    """a fixture batch: (seed, hyp, new_shape, mode, img_size, source images, label rows, key prefix)"""
-    k = "batch_%s_" % name
-    hyp = dict(zip([str(v) for v in g[k + "hyp_keys"]], [float(v) for v in g[k + "hyp"]]))
-    ns = g[k + "new_shape"]
-    mode = str(g[k + "mode"])
-    new_shape = int(ns[0]) if mode == "square" else (int(ns[0]), int(ns[1]))
-    seed = int(g[k + "seed"])
-    specs = [tuple(int(v) for v in r) for r in g[k + "specs"]]
-    imgs = [source(100 * seed + i, h, w, kind) for i, (h, w, kind, n) in enumerate(specs)]
-    labs = [label_rows(100 * seed + i, n) for i, (h, w, kind, n) in enumerate(specs)]
-    return seed, hyp, new_shape, mode, int(g[k + "img_size"]), imgs, labs, k
-
-
-# ---- restatements ----------------------------------------------------------------------------------------------
-
-def warp_np(img, minv, border=128):
-    """ryolo_augment_warp restated: cv2's fixed-point bilinear remap of warpAffine"""
-    h, w = img.shape[:2]
-    x = np.arange(w, dtype=np.float64)
-    y = np.arange(h, dtype=np.float64)
-    adelta = np.rint(minv[0] * x * 1024.0).astype(np.int64)
-    bdelta = np.rint(minv[3] * x * 1024.0).astype(np.int64)
-    X0 = np.rint((minv[1] * y + minv[2]) * 1024.0).astype(np.int64) + 16
-    Y0 = np.rint((minv[4] * y + minv[5]) * 1024.0).astype(np.int64) + 16
-    X = (X0[:, None] + adelta[None, :]) >> 5
-    Y = (Y0[:, None] + bdelta[None, :]) >> 5
-    sx, sy, ax, ay = X >> 5, Y >> 5, X & 31, Y & 31
-    acc = np.zeros((h, w, 3), np.int64)
-    for dy in (0, 1):
-        for dx in (0, 1):
-            wt = ((32 - ay) if dy == 0 else ay) * ((32 - ax) if dx == 0 else ax) * 32
-            xx, yy = sx + dx, sy + dy
-            inside = (xx >= 0) & (xx < w) & (yy >= 0) & (yy < h)
-            v = np.where(inside[..., None], img[np.clip(yy, 0, h - 1), np.clip(xx, 0, w - 1)].astype(np.int64), border)
-            acc += v * wt[..., None]
-    return ((acc + 16384) >> 15).astype(np.uint8)
-
-
-def _hsv_tables():
-    i = np.arange(1, 256, dtype=np.float64)
-    sdiv, hdiv = np.zeros(256, np.int64), np.zeros(256, np.int64)
-    sdiv[1:] = np.rint((255 << 12) / i)
-    hdiv[1:] = np.rint((180 << 12) / (6.0 * i))
-    return sdiv, hdiv
-
-
-def bgr2hsv_np(img):
-    sdiv, hdiv = _hsv_tables()
-    b, g, r = (img[..., k].astype(np.int64) for k in range(3))
-    v = np.maximum(np.maximum(b, g), r)
-    diff = v - np.minimum(np.minimum(b, g), r)
-    s = (diff * sdiv[v] + 2048) >> 12
-    h = np.where(v == r, g - b, np.where(v == g, b - r + 2 * diff, r - g + 4 * diff))
-    h = (h * hdiv[diff] + 2048) >> 12
-    return np.stack([h + np.where(h < 0, 180, 0), s, v], -1).astype(np.uint8)
-
-
-def _fma(a, b, c):
-    return (a.astype(np.float64) * b.astype(np.float64) + c).astype(np.float32)
-
-
-SECTORS = np.array([[1, 3, 0], [1, 0, 2], [3, 0, 1], [0, 2, 1], [0, 1, 3], [2, 1, 0]])
-
-
-def hsv2bgr_np(hsv, vec_pixels=32):
-    """cv2's 8-bit HSV2BGR: vector blocks of vec_pixels per row (fused 1 - s*h, truncation), scalar tail (rounding)"""
-    h = hsv[..., 0].astype(f32)
-    s = hsv[..., 1].astype(f32) * f32(1 / 255)
-    v = hsv[..., 2].astype(f32) * f32(1 / 255)
-    hh = h * f32(6 / 180)
-    pre = np.trunc(hh)
-    fr = hh - pre
-    sec = (pre - np.trunc(pre * f32(1 / 6)) * f32(6)).astype(np.int64)
-    one = f32(1)
-    tab = np.stack([v, v * (one - s), v * _fma(-s, fr, 1.0), v * _fma(-s, one - fr, 1.0)], -1)
-    out = np.stack([np.take_along_axis(tab, SECTORS[sec][..., k:k + 1], -1)[..., 0] for k in range(3)], -1) * f32(255)
-    w = hsv.shape[1]
-    vec = np.arange(w) < w // vec_pixels * vec_pixels
-    q = np.where(vec[None, :, None], np.trunc(out), np.rint(out))
-    return np.clip(q, 0, 255).astype(np.uint8)
-
-
-def hsv_np(img, a, b):
-    hsv = bgr2hsv_np(img)
-    S = hsv[..., 1].astype(f32) * f32(a)
-    V = hsv[..., 2].astype(f32) * f32(b)
-    hsv[..., 1] = np.minimum(S, f32(255))
-    hsv[..., 2] = np.minimum(V, f32(255))
-    return hsv2bgr_np(hsv)
-
-
-def gamma_table_np(m, gm):
-    """what the finish kernel's per-image table holds: numpy's uint8(power(v / float(M), gm) * M) for v <= M"""
-    v = np.arange(256)
-    if m == 0:
-        return np.zeros(256, np.uint8)
-    t = np.uint8(np.power(v[: m + 1] / float(m), gm) * np.uint8(m))
-    return np.concatenate([t, np.zeros(255 - m, np.uint8)])
 
 
 # ---- restatements against cv2 / numpy live ----------------------------------------------------------------------
@@ -153,8 +19,7 @@ def gamma_table_np(m, gm):
 @pytest.mark.parametrize("src_hw", [(1080, 1920), (768, 1024), (1216, 912), (611, 613), (1000, 700), (1213, 1900)])
 def test_pre_resize_tables_match_cv2_linear(src_hw):
     import rotate_yolov3_b200.preprocess as pp
-    from test_letterbox_cpu import resize_np
-    aug = _aug()
+    aug = aug_module()
     dst = aug.pre_resize_shape(src_hw, 608)
     img = source(sum(src_hw), *src_hw)
     want = cv2.resize(img, (dst[1], dst[0]), interpolation=cv2.INTER_LINEAR)
@@ -174,7 +39,7 @@ def test_exact_2x_linear_takes_the_area_path():
 
 
 def test_rotation_matrix_matches_cv2():
-    aug = _aug()
+    aug = aug_module()
     rng = np.random.default_rng(3)
     for _ in range(500):
         a, s = float(rng.uniform(-180, 180)), float(rng.uniform(0.5, 1.5))
@@ -185,7 +50,7 @@ def test_rotation_matrix_matches_cv2():
 @pytest.mark.parametrize("deg,scale,hw", [(5.0, 0.1, (608, 608)), (50.0, 0.2, (608, 608)), (50.0, 0.2, (352, 608)),
                                           (30.0, 0.5, (97, 131))])
 def test_warp_restatement_matches_cv2(deg, scale, hw):
-    aug = _aug()
+    aug = aug_module()
     rng = random.Random(int(deg) + hw[0])
     img = source(hw[0] + hw[1], *hw)
     for _ in range(4):
@@ -196,14 +61,9 @@ def test_warp_restatement_matches_cv2(deg, scale, hw):
         assert np.array_equal(warp_np(img, aug.invert_affine(M)), want)
 
 
-def _all_colours():
-    c = np.arange(1 << 24, dtype=np.uint32)
-    return np.stack([(c >> 16) & 255, (c >> 8) & 255, c & 255], -1).astype(np.uint8)
-
-
 @pytest.mark.parametrize("w", [4096, 4093, 37, 1])
 def test_bgr2hsv_every_colour(w):
-    img = _all_colours()
+    img = all_colours()
     n = img.shape[0] // w * w
     img = img[:n].reshape(-1, w, 3)
     assert np.array_equal(bgr2hsv_np(img), cv2.cvtColor(img, cv2.COLOR_BGR2HSV))
@@ -248,8 +108,8 @@ def test_gamma_tables_every_value_and_maximum():
 # ---- the host half against the reference (fixture) --------------------------------------------------------------
 
 def test_draw_replay_matches_reference():
-    aug = _aug()
-    g = _gold()
+    aug = aug_module()
+    g = augment_golden()
     for name in g["batches"]:
         seed, hyp, new_shape, mode, img_size, imgs, labs, k = batch_case(g, str(name))
         rec = Recorder(seed)
@@ -259,8 +119,8 @@ def test_draw_replay_matches_reference():
 
 
 def test_targets_match_collate_fn_rows():
-    aug = _aug()
-    g = _gold()
+    aug = aug_module()
+    g = augment_golden()
     for name in g["batches"]:
         seed, hyp, new_shape, mode, img_size, imgs, labs, k = batch_case(g, str(name))
         rng = random.Random(seed)
@@ -272,8 +132,8 @@ def test_targets_match_collate_fn_rows():
 
 def test_direct_transforms_match_reference():
     """random_affine, Gamma, HSV and the flips called directly, each forced on: the restated pixels"""
-    aug = _aug()
-    g = _gold()
+    aug = aug_module()
+    g = augment_golden()
     for name in g["directs"]:
         k = "direct_%s_" % name
         img, want, d = g[k + "img"], g[k + "out"], g[k + "draws"]
@@ -294,7 +154,7 @@ def test_direct_transforms_match_reference():
 
 
 def test_missing_hyp_key_raises_keyerror():
-    aug = _aug()
+    aug = aug_module()
     hyp = {"degrees": 5.0, "translate": 0.1, "scale": 0.1, "shear": 0.0, "noise": 0.01, "gamma": 0.2, "blur": 1.3,
            "hsv_s": 0.5, "hsv_v": 0.3, "grayscale": 0.3}
     aug.draw(hyp, random.Random(0))
@@ -308,7 +168,7 @@ def test_missing_hyp_key_raises_keyerror():
 
 def test_rect_img_size_sets_the_pre_resize():
     """a dataset img_size that is no multiple of 32: the pre-resize follows it, not the batch shape"""
-    aug = _aug()
+    aug = aug_module()
     rec = dict(DRAW_KEYS_NONE)
     plan, _ = aug.batch_plan([(1080, 1920)], [np.zeros((0, 6), np.float32)], [rec], (352, 608), "rect", 600)
     assert plan[0][1] == (337, 600)

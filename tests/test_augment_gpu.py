@@ -2,7 +2,6 @@
 own ``__getitem__`` / ``collate_fn`` bit for bit in fp32 and fp16 with identical target rows, the transforms forced
 on one at a time, the device HSV over every colour and the device gamma tables against the host restatements, mixed
 and CUDA-resident batches, the launch count, and malformed input."""
-import hashlib
 import os
 import random
 
@@ -10,23 +9,15 @@ import numpy as np
 import pytest
 import torch
 
+from augment_cases import DRAW_KEYS_NONE, all_colours, batch_case, gamma_table_np, hsv_np
+from builders import tensor_sha
 from helpers import GOLDEN
-from test_augment_cpu import DRAW_KEYS_NONE, batch_case, gamma_table_np, hsv_np
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(GOLDEN, "augment_golden.npz")
 DEV = torch.device("cuda", 0)
 HYP = {"degrees": 50.0, "translate": 0.1, "scale": 0.2, "shear": 0.0, "noise": 0.01, "gamma": 0.2, "blur": 1.3,
        "hsv_s": 0.5, "hsv_v": 0.3, "grayscale": 0.3}
-
-
-def _pkg():
-    import rotate_yolov3_b200 as pkg
-    return pkg
-
-
-def _sha(t):
-    return hashlib.sha256(t.cpu().contiguous().numpy().tobytes()).hexdigest()
 
 
 def _net(u8, dtype):
@@ -43,13 +34,13 @@ def _record(**kw):
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
 def test_every_fixture_batch_bitwise(dtype):
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     g = np.load(GOLD)
     for name in g["batches"]:
         seed, hyp, new_shape, mode, img_size, imgs, labs, k = batch_case(g, str(name))
         x, tg, draws = pkg.train_batch(imgs, labs, hyp, new_shape=new_shape, mode=mode, rng=random.Random(seed),
                                        dtype=dtype, img_size=img_size)
-        assert _sha(x) == str(g[k + ("sha32" if dtype == torch.float32 else "sha16")]), name
+        assert tensor_sha(x) == str(g[k + ("sha32" if dtype == torch.float32 else "sha16")]), name
         assert tg.is_cuda and tg.dtype == torch.float32
         assert np.array_equal(tg.cpu().numpy().view(np.int32), g[k + "targets"].view(np.int32)), name
         # the returned draws replay the batch
@@ -59,7 +50,7 @@ def test_every_fixture_batch_bitwise(dtype):
 
 
 def test_direct_transforms_bitwise():
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     g = np.load(GOLD)
     for name in g["directs"]:
         name = str(name)
@@ -80,21 +71,16 @@ def test_direct_transforms_bitwise():
             assert tg.shape == (0, 7)
 
 
-def _all_colours():
-    c = np.arange(1 << 24, dtype=np.uint32)
-    return np.stack([(c >> 16) & 255, (c >> 8) & 255, c & 255], -1).astype(np.uint8)
-
-
 @pytest.mark.parametrize("factors", [(1.0, 1.0), (1.37, 0.71), (0.55, 1.29)])
 def test_device_hsv_every_colour(factors):
-    pkg = _pkg()
-    img = _all_colours().reshape(4096, 4096, 3)
+    import rotate_yolov3_b200 as pkg
+    img = all_colours().reshape(4096, 4096, 3)
     x, _, _ = pkg.train_batch([img], [np.zeros((0, 6), np.float32)], HYP, new_shape=4096,
                               draws=[_record(hsv=factors)])
     got = torch.round(x[0] * 255).to(torch.uint8).cpu().numpy()[::-1].transpose(1, 2, 0)
     assert np.array_equal(got, hsv_np(img, *factors))
     # rows whose width leaves a scalar tail (100 = 3 x 32 + 4)
-    small = _all_colours()[::1669][:10000].reshape(100, 100, 3)
+    small = all_colours()[::1669][:10000].reshape(100, 100, 3)
     x, _, _ = pkg.train_batch([small], [np.zeros((0, 6), np.float32)], HYP, new_shape=100,
                               draws=[_record(hsv=factors)])
     got = torch.round(x[0] * 255).to(torch.uint8).cpu().numpy()[::-1].transpose(1, 2, 0)
@@ -104,8 +90,8 @@ def test_device_hsv_every_colour(factors):
 @pytest.mark.parametrize("flips", [dict(hflip=True), dict(vflip=True), dict(hflip=True, vflip=True)])
 def test_device_hsv_with_flips_at_a_width_with_a_scalar_tail(flips):
     """HSV2BGR's vector/scalar path follows a pixel's column before the flips (100 = 3 x 32 + 4)"""
-    pkg = _pkg()
-    small = _all_colours()[::1669][:10000].reshape(100, 100, 3)
+    import rotate_yolov3_b200 as pkg
+    small = all_colours()[::1669][:10000].reshape(100, 100, 3)
     want = hsv_np(small, 1.37, 0.71)
     want = want[:, ::-1] if flips.get("hflip") else want
     want = want[::-1] if flips.get("vflip") else want
@@ -115,7 +101,7 @@ def test_device_hsv_with_flips_at_a_width_with_a_scalar_tail(flips):
 
 
 def test_device_gamma_tables_every_value_and_maximum():
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     v = np.arange(256)
     imgs = [np.repeat(np.minimum(v, m).astype(np.uint8).reshape(16, 16, 1), 3, 2) for m in range(256)]
     rng = random.Random(11)
@@ -129,7 +115,7 @@ def test_device_gamma_tables_every_value_and_maximum():
 
 
 def test_mixed_batch_equals_single_calls_and_cuda_sources():
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     rng = np.random.default_rng(4)
     shapes = [(768, 1024), (1080, 1920), (300, 200), (608, 608), (900, 1300)]
     imgs = [rng.integers(0, 256, s + (3,), dtype=np.uint8) for s in shapes]
@@ -151,7 +137,7 @@ def test_mixed_batch_equals_single_calls_and_cuda_sources():
 def test_strided_cuda_sources_equal_host_arrays():
     """CUDA images whose pixels or channels are not packed (a CHW decode permuted to HWC, a column-subsampled view, a
     crop) give what the same pixels give as host arrays"""
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     rng = np.random.default_rng(8)
     base = rng.integers(0, 256, (700, 1300, 3), dtype=np.uint8)
     chw = torch.from_numpy(np.ascontiguousarray(base.transpose(2, 0, 1))).to(DEV)
@@ -166,7 +152,7 @@ def test_strided_cuda_sources_equal_host_arrays():
 
 
 def test_launches_per_batch():
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     lib = pkg._lib.lib
     big = np.zeros((1080, 1920, 3), np.uint8)
     small = np.zeros((300, 400, 3), np.uint8)
@@ -182,7 +168,7 @@ def test_launches_per_batch():
 
 
 def test_malformed_input_raises_before_any_launch():
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     lib = pkg._lib.lib
     ok = np.zeros((20, 30, 3), np.uint8)
     lab = [np.zeros((0, 6), np.float32)]

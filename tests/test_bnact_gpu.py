@@ -5,12 +5,9 @@ import ctypes
 import pytest
 import torch
 import torch.nn.functional as F
+from f64_refs import bf
 
 pytestmark = pytest.mark.gpu
-
-
-def _bf(t):
-    return t.to(torch.bfloat16).float()
 
 
 # up: False plain dy, True dy at 2x resolution (nearest-upsample adjoint), 2 dy in the space-to-depth layout of a following
@@ -27,15 +24,15 @@ def test_bn_stats_finalize_prelu_fwd_bwd_vs_autograd(c, h, w, b, res, up):
     lib = pkg._lib.lib
     dev = torch.device("cuda")
     g = torch.Generator().manual_seed(c + h)
-    z = _bf(torch.randn(b, c, h, w, generator=g) * 1.5 + 0.3).to(dev)
+    z = bf(torch.randn(b, c, h, w, generator=g) * 1.5 + 0.3).to(dev)
     gamma = (0.5 + torch.rand(c, generator=g)).to(dev)
     beta = (0.3 * torch.randn(c, generator=g)).to(dev)
     slope = 0.17
-    r = _bf(torch.randn(b, c, h, w, generator=g)).to(dev) if res else None
+    r = bf(torch.randn(b, c, h, w, generator=g)).to(dev) if res else None
     s2d = up == 2
     up = up is True
     oh, ow = (2 * h, 2 * w) if up else (h, w)
-    dy = _bf(torch.randn(b, c, oh, ow, generator=g)).to(dev)
+    dy = bf(torch.randn(b, c, oh, ow, generator=g)).to(dev)
     # ---- torch reference ----
     zt = z.clone().requires_grad_(True)
     gt, bt = gamma.clone().requires_grad_(True), beta.clone().requires_grad_(True)
@@ -108,10 +105,10 @@ def test_dgrad_via_forward_kernel_vs_autograd(cin, cout, k, stride, h, w):
     dev = torch.device("cuda")
     g = torch.Generator().manual_seed(cin + k)
     b = 2
-    x = _bf(torch.randn(b, cin, h, w, generator=g)).to(dev).requires_grad_(True)
-    wt = _bf(torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5).to(dev)
+    x = bf(torch.randn(b, cin, h, w, generator=g)).to(dev).requires_grad_(True)
+    wt = bf(torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5).to(dev)
     oh, ow = (h + stride - 1) // stride, (w + stride - 1) // stride
-    dz = _bf(torch.randn(b, cout, oh, ow, generator=g)).to(dev)
+    dz = bf(torch.randn(b, cout, oh, ow, generator=g)).to(dev)
     F.conv2d(x, wt, None, stride=stride, padding=(k - 1) // 2).backward(dz)
     bn = 256 if cout > 128 else (128 if cout > 64 else 64)
     cout_pad = L.round_up(cout, bn)
@@ -123,7 +120,7 @@ def test_dgrad_via_forward_kernel_vs_autograd(cin, cout, k, stride, h, w):
         assert lib.ryolo_zero_insert2x(pt(dzb), cout_pad, b, oh, ow, cout_pad, pt(up), cout_pad, h, w, stream) == 0
         dzb = up
     gcs = L.round_up(cin, 64) if cin != 384 else 384
-    prior = _bf(torch.randn(b, cin, h, w, generator=g)).to(dev)
+    prior = bf(torch.randn(b, cin, h, w, generator=g)).to(dev)
     gx = L.to_padded_nhwc(prior, gcs)                       # accumulate on top of an existing gradient
     desc = L.make_desc(b, h, w, cout, cout_pad, cin, gcs, k, 1, False, 0.0, True, gcs, False, False)
     wd = wt.flip(2, 3).permute(1, 0, 2, 3).contiguous()

@@ -7,7 +7,7 @@ and above cout, the neighbours in a wider buffer) is checked by the TMA-store ep
 import pytest
 import torch
 
-import test_conv_tma_epilogue_gpu as tma_epilogue
+from builders import TMA_GARBAGE, TMA_SENTINEL, tma_epilogue_run
 
 pytestmark = pytest.mark.gpu
 
@@ -43,8 +43,8 @@ def _exact(batch, h, w, cin, cout, k, width, off=0, acc=False, res_sep=False, se
 
     def buffer():
         buf = L.alloc_padded(batch, h, w, width, dev)
-        buf.fill_(tma_epilogue.SENTINEL)
-        buf[..., off:off + store_cols] = tma_epilogue.GARBAGE
+        buf.fill_(TMA_SENTINEL)
+        buf[..., off:off + store_cols] = TMA_GARBAGE
         buf[:, 1:-1, 1:-1, off:off + store_cols] = 0.0
         return buf
 
@@ -57,12 +57,12 @@ def _exact(batch, h, w, cin, cout, k, width, off=0, acc=False, res_sep=False, se
     out = buffer()
     if acc:                             # in place: the residual IS the output view
         out[:, 1:-1, 1:-1, off:off + cout] = res.permute(0, 2, 3, 1)
-        out[:, 1:-1, 1:-1, off + cout:off + store_cols] = tma_epilogue.GARBAGE
+        out[:, 1:-1, 1:-1, off + cout:off + store_cols] = TMA_GARBAGE
         res_ptr, res_stride = out.data_ptr() + 2 * off, width
     else:                               # a separate buffer with a wider channel stride than the output
         rb = L.to_padded_nhwc(res, L.round_up(cout, 64) + 64)
-        rb[:, 0] = tma_epilogue.GARBAGE
-        rb[..., cout:] = tma_epilogue.GARBAGE
+        rb[:, 0] = TMA_GARBAGE
+        rb[..., cout:] = TMA_GARBAGE
         res_ptr, res_stride = rb.data_ptr(), rb.shape[-1]
     launch(out.data_ptr() + 2 * off, res_ptr, res_stride)
     torch.cuda.synchronize()
@@ -106,4 +106,5 @@ def test_residual_epilogue_exact(cfg):
 
 @pytest.mark.parametrize("cfg", CASES, ids=_case_id)
 def test_residual_epilogue_layout(cfg):
-    tma_epilogue._run(**cfg)
+    r = tma_epilogue_run(**cfg)
+    assert r["within"] and r["halo_zero"] and r["pad_zero"] and r["sentinels"], r

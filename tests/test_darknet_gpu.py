@@ -11,6 +11,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from f64_refs import bf
 from helpers import GOLDEN, SMALL_ANCHORS, init_darknet_weights
 
 pytestmark = pytest.mark.gpu
@@ -27,16 +28,14 @@ def _model(width=96, height=64):
 
 def _emulate_bf16(model, x):
     """torch fp32 reference of the same op chain with bf16 operand rounding at the kernel's quantisation points"""
-    def q(t):
-        return t.to(torch.bfloat16).float()
     outs = []
     heads = []
     for i, (d, mod) in enumerate(zip(model.module_defs, model.module_list)):
         t = d["type"]
         if t == "convolutional":
             w, scale, bias, slope = model._folded(i, x.device)
-            wq = q(w * scale.view(-1, 1, 1, 1)) if scale is not None else q(w)
-            xin = x if i == 0 else q(x)
+            wq = bf(w * scale.view(-1, 1, 1, 1)) if scale is not None else bf(w)
+            xin = x if i == 0 else bf(x)
             # first layer (first.cu): tensor pipe with the image as bf16 hi + lo halves (16 mantissa bits: fp32 up to
             # 2^-17) and bf16 weights like every other layer -- so only the weights are quantised here
             k = w.shape[-1]
@@ -47,7 +46,7 @@ def _emulate_bf16(model, x):
             if model.module_defs[i + 1]["type"] == "yolo":
                 heads.append(y)
         elif t == "shortcut":
-            x = x + q(outs[i + int(d["from"])])
+            x = x + bf(outs[i + int(d["from"])])
         elif t == "upsample":
             x = F.interpolate(x, scale_factor=2, mode="nearest")
         elif t == "route":

@@ -3,22 +3,14 @@
 the mean of the two ranks' local gradients computed WITHOUT the wrapper (per-replica BatchNorm like the reference,
 model/models.py:62).  Needs >= 2 GPUs (skipped otherwise)."""
 import os
-import socket
 
 import pytest
 import torch
 
 import helpers
+from builders import free_port
 
 pytestmark = pytest.mark.gpu
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _local_grads(rank, use_graph, steps=1):
@@ -71,7 +63,7 @@ def test_two_rank_nccl_gradients_equal_mean_of_local_gradients(use_graph):
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, use_graph, q)) for r in range(2)]
     for p in procs:
         p.start()

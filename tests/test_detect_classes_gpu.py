@@ -15,40 +15,9 @@ import pytest
 import torch
 
 import helpers
+from builders import check_equals_per_class_pipeline, postprocess_classes
 
 pytestmark = pytest.mark.gpu
-
-MIN_WH = 2.0
-
-
-def _postprocess(io, conf_thres, nms_thres, cap):
-    from rotate_yolov3_b200.nms import detect_postprocess_classes
-    return detect_postprocess_classes(io, conf_thres, nms_thres, cap)
-
-
-def check_equals_per_class_pipeline(io, conf_thres, nms_thres, cap):
-    """detect_postprocess_classes == nms_filter -> stable top-cap -> input order -> r_nms per class, image by image"""
-    import rotate_yolov3_b200 as pkg
-    from rotate_yolov3_b200.nms import nms_filter
-    res = _postprocess(io, conf_thres, nms_thres, cap)
-    assert res["dets"].shape == (io.shape[0], cap, 8) and res["keep"].shape == (io.shape[0], cap)
-    kept_total = 0
-    for b in range(io.shape[0]):
-        cand = nms_filter(io[b].clone(), conf_thres, MIN_WH)               # [n, 8] in input order
-        top = torch.sort(torch.argsort(cand[:, 5], descending=True, stable=True)[:cap]).values
-        sel = cand[top].contiguous()
-        n = int(res["counts"][b])
-        assert n == len(sel), (b, n, len(sel))
-        assert torch.equal(res["dets"][b, :n], sel), b
-        keep = []
-        for c in sel[:, 7].unique():
-            idx = torch.nonzero(sel[:, 7] == c).flatten()
-            keep.append(idx[pkg.r_nms(sel[idx, :6].contiguous(), nms_thres).to(idx.device)])
-        want = torch.sort(torch.cat(keep)).values if keep else torch.zeros(0, dtype=torch.long, device=io.device)
-        k = int(res["num_keep"][b])
-        assert torch.equal(res["keep"][b, :k], want), (b, k, len(want))
-        kept_total += k
-    return res, kept_total
 
 
 def _image(nc, cls, conf, seed, canvas=200.0):
@@ -165,7 +134,7 @@ def test_reference_driver_golden():
     g = np.load(os.path.join(helpers.GOLDEN, "nms_driver_golden.npz"))
     pred = torch.from_numpy(g["pred"]).cuda()
     before = pred.clone()
-    out = detections_per_image(_postprocess(pred, float(g["conf_thres"]), float(g["nms_thres"]), 600))
+    out = detections_per_image(postprocess_classes(pred, float(g["conf_thres"]), float(g["nms_thres"]), 600))
     assert len(out) == 3
     for i in range(3):
         if bool(g["none_%d" % i]):
@@ -174,7 +143,7 @@ def test_reference_driver_golden():
             assert np.array_equal(out[i].cpu().numpy(), g["out_%d" % i]), i
     assert torch.equal(pred.view(torch.int32), before.view(torch.int32))     # io is not modified
     pred1 = torch.from_numpy(g["pred1"]).cuda()
-    out1 = detections_per_image(_postprocess(pred1, 0.5, 0.5, 600))
+    out1 = detections_per_image(postprocess_classes(pred1, 0.5, 0.5, 600))
     for i in range(2):
         assert np.array_equal(out1[i].cpu().numpy(), g["out1_%d" % i]), i
 
@@ -183,7 +152,7 @@ def test_detections_per_image_order():
     """confidence descending, ties by class ascending, then by input row; None for an image with nothing kept"""
     from rotate_yolov3_b200.nms import detections_per_image
     io = _batch(case_all_tied(3), case_nothing_passes(3), case_mixed(3))
-    res = _postprocess(io, 0.5, 0.4, 2000)
+    res = postprocess_classes(io, 0.5, 0.4, 2000)
     out = detections_per_image(res)
     assert out[1] is None
     for b in (0, 2):
@@ -219,7 +188,7 @@ def test_bench_shape_three_classes():
 def test_bench_shape_single_class_equals_detect_postprocess():
     from rotate_yolov3_b200.nms import detect_postprocess
     io = _bench_io(1)
-    res = _postprocess(io, 0.5, 0.5, 20000)
+    res = postprocess_classes(io, 0.5, 0.5, 20000)
     ref = detect_postprocess(io, 0.5, 0.5, 20000)
     assert torch.equal(res["counts"], ref["counts"])
     for b in range(io.shape[0]):
@@ -235,15 +204,15 @@ def test_bench_shape_single_class_equals_detect_postprocess():
 def test_repeatable_and_independent_of_batch():
     io = _batch(case_runs(15), case_mixed(15, 3000, 40, 608.0), case_nothing_passes(15), case_all_tied(15))
     for cap in (2000, 100):
-        a = _postprocess(io, 0.5, 0.4, cap)
-        b = _postprocess(io, 0.5, 0.4, cap)
+        a = postprocess_classes(io, 0.5, 0.4, cap)
+        b = postprocess_classes(io, 0.5, 0.4, cap)
         for key in ("counts", "num_keep"):
             assert torch.equal(a[key], b[key]), key
         for i in range(io.shape[0]):
             n, k = int(a["counts"][i]), int(a["num_keep"][i])
             assert torch.equal(a["dets"][i, :n].view(torch.int32), b["dets"][i, :n].view(torch.int32))
             assert torch.equal(a["keep"][i, :k], b["keep"][i, :k])
-            one = _postprocess(io[i:i + 1].contiguous(), 0.5, 0.4, cap)
+            one = postprocess_classes(io[i:i + 1].contiguous(), 0.5, 0.4, cap)
             assert int(one["counts"][0]) == n and int(one["num_keep"][0]) == k
             assert torch.equal(one["dets"][0, :n].view(torch.int32), a["dets"][i, :n].view(torch.int32))
             assert torch.equal(one["keep"][0, :k], a["keep"][i, :k])

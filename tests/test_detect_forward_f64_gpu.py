@@ -27,7 +27,7 @@ residual is the layer the [shortcut] names, the producers of a concat buffer sit
                  producer that wrote into its neighbour's channels fails the neighbour's check (the checks read the
                  final state, and a clobbered earlier producer is also caught by the s2d copy made from it)
   s2d            ryolo_space_to_depth bit for bit against a plain reshape
-  decode         io within 2^-20 M of test_detect_gpu._decode_ref on the actual head buffers
+  decode         io within 2^-20 M of f64_refs.decode_ref on the actual head buffers
   whole forward  (bench shape) the replay's io and heads == an eager forward on x_b, bit for bit; each of the 32 images
                  == a batch-1 forward of that image, bit for bit (the tile width depends on cout only and there is no
                  split-K, so no accumulation order depends on the batch: the cheap exact check of the large offsets)
@@ -58,343 +58,27 @@ import time
 import pytest
 import torch
 
-import test_train_step_f64_gpu as tsf
+from checked_step import (Acc, Run, check_buffers, check_conv, check_first, check_s2d_step, conv_want, first_check,
+                          fold_ratio, map_plan, slope)
+from f64_refs import BF16, bf16_check, bitwise, decode_ref, f32_check, interior, passed, rtz_bf16, yolov3_heads
 from helpers import init_darknet_weights
-from test_detect_gpu import _decode_ref, _yolov3_heads
-from test_train_step_f64_gpu import bf16_check, bitwise, conv_taps, f32_check, halo_zero, interior, passed, s2d, tapsum
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24
-F64 = torch.float64
-BF16 = torch.bfloat16
-TINY = 1e-30
-CHUNK_BYTES = 4e9          # float64 working set of one chunk of images
 SHAPES = {"bench": (32, 608, 608), "letterbox": (3, 352, 608)}
 X_SEEDS = (0, 5)           # x_a (bench.py's rank-0 image) and x_b
-
-
-def rup(x, m):
-    return (x + m - 1) // m * m
-
-
-class Acc:
-    """bf16_check over image chunks: the worst ratio (NaN propagates) and the rounding-bias ratio of the whole tensor"""
-
-    def __init__(self):
-        self.maxes, self.es, self.w2, self.n = [], 0.0, 0.0, 0
-
-    def add(self, got, want, e, t=0.0):
-        self.maxes.append(bf16_check(got, want, e, t)["max"])
-        self.es += float(((got.double() - want) * want.sign()).sum())
-        self.w2 += float(want.pow(2).sum())
-        self.n += want.numel()
-
-    def result(self):
-        rms = (self.w2 / self.n) ** 0.5
-        return {"max": float(torch.tensor(self.maxes, dtype=F64).max()),
-                "bias": abs(self.es / self.n) / (tsf.BIAS_TOL * rms + TINY)}
-
-
-def chunks(batch, bytes_per_image):
-    per = max(1, min(batch, int(CHUNK_BYTES // bytes_per_image)))
-    return [(b, min(batch, b + per)) for b in range(0, batch, per)]
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# float64 references
-def conv_want(s, bias, slope, res=None):
-    """act(S + bias) + res in float64 and T, the fp32 epilogue roundings (bias add, PReLU multiply, residual add)"""
-    u = s + bias
-    act = torch.where(u > 0, u, u * slope) if slope is not None else u
-    t = 2 * U * (s.abs() + bias.abs())
-    if res is None:
-        return act, t
-    r = res.double()
-    return act + r, t + U * (act.abs() + r.abs())
-
-
-def first_check(got_xs, x_nchw, wf, bias, slope, acc=None):
-    """the first layer on the fp32 image with bf16(wf), + bias, PReLU, in the space-to-depth layout of got_xs"""
-    x = x_nchw.permute(0, 2, 3, 1)
-    s, a = tapsum(x, conv_taps(wf.to(BF16).double()), x.shape[1], x.shape[2])
-    want, t = conv_want(s, bias.double(), slope)
-    e = 4 * 2.0 ** -23 * a + 2.0 ** -16 * a
-    acc = acc or Acc()
-    acc.add(got_xs, s2d(want), s2d(e), s2d(t))
-    return acc
-
-
-def fold_ratio(model, i, drop_eps=False):
-    """_folded's fp32 (scale, bias) against float64 utils/torch_utils.py:45-69, in units of their rounding bounds"""
-    _, scale, bias, _ = model._folded(i, torch.device("cuda"))
-    seq = model.module_list[i]
-    bn = seq.BatchNorm2d
-    g, be, m, v = (t.detach().double() for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
-    s64 = g / torch.sqrt(v + (0.0 if drop_eps else bn.eps))
-    b64 = be - m * s64
-    if seq.Conv2d.bias is not None:
-        b64 = b64 + seq.Conv2d.bias.detach().double() * s64
-    rs = (scale.double() - s64).abs() / (3 * U * s64.abs() + TINY)
-    rb = (bias.double() - b64).abs() / (U * (4 * (m * s64).abs() + b64.abs()) + TINY)
-    return max(float(rs.max()), float(rb.max()))
-
-
-def packed_want(model, i, s2d_layer, taps, cout_pad, cin_pad):
-    wt, scale, _, _ = model._folded(i, torch.device("cuda"))
-    if s2d_layer:
-        wt = _layout().s2d_weight(wt)
-    wf = wt * scale.view(-1, 1, 1, 1) if scale is not None else wt
-    want = torch.zeros((taps, cout_pad, cin_pad), dtype=BF16, device=wt.device)
-    for t, (_, _, m) in enumerate(conv_taps(wf)):
-        want[t, :wf.shape[0], :wf.shape[1]] = m.t().to(BF16)
-    return want
-
-
-def _layout():
-    from rotate_yolov3_b200 import layout
-    return layout
-
-
-def _lib():
-    from rotate_yolov3_b200 import _lib as lib
-    return lib
-
-
-# ---------------------------------------------------------------------------------------------------------------
-class View:
-    def __init__(self, buf, off, c):
-        self.buf, self.off, self.c = buf, off, c
-
-    @property
-    def ptr(self):
-        return self.buf.data_ptr() + 2 * self.off
-
-    def interior(self):
-        return interior(self.buf, self.off, self.c)
-
-
-class Run:
-    pass
-
-
-def _slope(model, i):
-    seq = model.module_list[i]
-    return float(seq.activation.weight.detach().float().item()) if hasattr(seq, "activation") else None
-
-
-def map_plan(st):
-    """walk module_defs beside the plan's steps: each layer's output as a View, the steps of each conv layer, the s2d
-    copies; asserts the plan's pointers are the graph's wiring"""
-    model, plan = st.model, st.plan
-    defs = model.module_defs
-    steps = plan["steps"]
-    outs, conv_of, s2d_of = {}, {}, {}
-    k = 0
-    for i, d in enumerate(defs):
-        t = d["type"]
-        if t == "convolutional":
-            if k < len(steps) and steps[k][0] == "s2d":
-                s2d_of[i] = k
-                k += 1
-            kind, a = steps[k]
-            conv_of[i] = k
-            k += 1
-            if kind == "first":
-                assert a["xs"] is not None and a["out"].buf is None      # layer 0 lives in layer 1's s2d buffer only
-                outs[0] = None
-                continue
-            assert kind == "conv", (i, kind)
-            out = a["keep"][2]
-            desc = a["desc"]
-            nxt = defs[i + 1]["type"] if i + 1 < len(defs) else None
-            if desc.out_dtype == _lib().DT_F32:
-                outs[i] = out
-                continue
-            v = View(out.buf, out.ch_off, out.c)
-            assert v.ptr == a["y"]
-            if (nxt == "shortcut" and desc.has_residual) or (nxt == "upsample" and desc.upsample2x):
-                outs[i], outs[i + 1] = None, v
-            else:
-                assert not desc.has_residual and not desc.upsample2x
-                outs[i] = v
-        elif t == "route":
-            ls = [int(x) for x in d["layers"].split(",")]
-            ls = [l if l > 0 else i + l for l in ls]
-            if len(ls) == 1:
-                outs[i] = outs[ls[0]]
-            else:
-                buf, off = outs[ls[0]].buf, 0
-                for l in ls:                                       # producers at their route offsets, one buffer
-                    assert outs[l].buf is buf and outs[l].off == off, (i, l)
-                    off += outs[l].c
-                outs[i] = View(buf, 0, off)
-        elif t in ("shortcut", "upsample"):
-            assert i in outs, (t, i)                                # materialised by the fused conv
-        elif t == "yolo":
-            outs[i] = None
-        else:
-            raise AssertionError("layer type %s in the detect graph" % t)
-    assert k == len(steps)
-    st.outs, st.conv_of, st.s2d_of = outs, conv_of, s2d_of
-
-
-def check_s2d_step(st, i):
-    a = st.plan["steps"][st.s2d_of[i]][1]
-    src = st.outs[i - 1]
-    assert a["x"] == src.ptr and a["xcs"] == src.buf.shape[-1] and a["c"] == src.c
-    xs = a["xs"]
-    c4 = 4 * src.c
-    return dict(bits=bitwise(interior(xs, 0, c4), s2d(src.interior())),
-                pad_zero=bool((xs[..., c4:] == 0).all()))
-
-
-def check_first(st):
-    model = st.model
-    kind, a = st.plan["steps"][st.conv_of[0]]
-    wt, scale, bias, slope = model._folded(0, torch.device("cuda"))
-    r = {}
-    r["w_bits"] = torch.equal(a["w"], wt * scale.view(-1, 1, 1, 1)) and torch.equal(a["b"], bias)
-    r["slope"] = a["slope"] == _slope(model, 0)
-    r["fold"] = fold_ratio(model, 0)
-    xs = a["xs"]
-    cout = a["cout"]
-    assert xs.shape[-1] == rup(4 * cout, 64)
-    b, _, h, w = st.x.shape
-    acc = Acc()
-    for b0, b1 in chunks(b, h * w * cout * 8 * 10):
-        first_check(interior(xs, 0, 4 * cout)[b0:b1], st.x[b0:b1], a["w"], bias, _slope(model, 0), acc)
-    r.update(acc.result())
-    r["xs_pad_zero"] = bool((xs[..., 4 * cout:] == 0).all())
-    if st.stash is not None:
-        st.stash["first"] = dict(x=st.x[:2].clone(), got=interior(xs, 0, 4 * cout)[:2].clone(), w=a["w"], b=bias,
-                                 slope=_slope(model, 0))
-    return r
-
-
-def conv_offsets(k, taps):
-    if k == 3:
-        return [(t // 3 - 1, t % 3 - 1) for t in range(taps)]
-    if k == 2:
-        return [(t // 2 - 1, t % 2 - 1) for t in range(taps)]
-    return [(0, 0)]
-
-
-def check_conv(st, i):
-    model, plan = st.model, st.plan
-    a = plan["steps"][st.conv_of[i]][1]
-    desc = a["desc"]
-    L = _lib()
-    r = {}
-    # inputs: the graph's wiring
-    s2d_layer = i == 1 or i in st.s2d_of
-    if s2d_layer:
-        # layer 1 reads the buffer the first layer wrote; the other stride-2 layers the copy of ryolo_space_to_depth
-        xs = plan["steps"][st.s2d_of[i] if i in st.s2d_of else st.conv_of[0]][1]["xs"]
-        assert desc.ksize == 2 and a["x"] == xs.data_ptr() and desc.cin_stride == xs.shape[-1]
-        x = interior(xs, 0, desc.cin)
-    else:
-        src = st.outs[i - 1]
-        assert a["x"] == src.ptr and desc.cin == src.c and desc.cin_stride == src.buf.shape[-1]
-        x = src.interior()
-    assert desc.stride == 1                                  # every stride-2 layer runs on a space-to-depth copy
-    assert (desc.in_h, desc.in_w) == tuple(x.shape[1:3])
-    k = abs(desc.ksize)
-    taps, cin_pad = k * k, rup(desc.cin, 64)
-    cout = desc.cout
-    cout_pad = a["w"].numel() // (2 * taps * cin_pad)
-    pk = a["w"].view(BF16).view(taps, cout_pad, cin_pad)
-    # weight pack, bias buffer, slope, folding
-    r["w_bits"] = bitwise(pk, packed_want(model, i, s2d_layer, taps, cout_pad, cin_pad))
-    _, scale, bias, _ = model._folded(i, torch.device("cuda"))
-    bias_pad = torch.zeros(cout_pad, dtype=torch.float32, device=bias.device)
-    bias_pad[:cout] = bias
-    r["b_bits"] = torch.equal(a["b"], bias_pad)
-    if scale is not None:
-        r["fold"] = fold_ratio(model, i)
-    slope = _slope(model, i)
-    r["slope"] = bool(desc.has_act) == (slope is not None) and (slope is None or desc.slope == slope)
-    # residual: the layer the [shortcut] names
-    res = None
-    if desc.has_residual:
-        frm = int(model.module_defs[i + 1]["from"])
-        rv = st.outs[i + 1 + frm if frm < 0 else frm]
-        assert a["r"] == rv.ptr and desc.res_stride == rv.buf.shape[-1] and rv.c == cout
-        res = rv.interior()
-    else:
-        assert a["r"] is None
-    head = desc.out_dtype == L.DT_F32
-    up = bool(desc.upsample2x)
-    out = st.outs[i] if not up and not desc.has_residual else st.outs[i + 1]
-    n = taps * cin_pad // 16
-    mats = [(dy, dx, pk[t, :cout, :desc.cin].double().t().contiguous())
-            for t, (dy, dx) in enumerate(conv_offsets(k, taps))]
-    b64 = bias.double()
-    oh, ow = desc.in_h, desc.in_w
-    acc = Acc()
-    heads = []
-    copies = True
-    per_img = 8 * (4 * (oh + 2) * (ow + 2) * desc.cin + 12 * oh * ow * cout)
-    keep = st.stash is not None and i in st.keep
-    kept = []
-    for b0, b1 in chunks(desc.batch, per_img):
-        s, mag = tapsum(x[b0:b1], mats, oh, ow)
-        e = n * 2.0 ** -23 * mag
-        if head:
-            got = out[b0:b1].permute(0, 2, 3, 1)
-            heads.append(f32_check(got, s + b64, e)["max"])
-        else:
-            want, t = conv_want(s, b64, slope, res[b0:b1] if res is not None else None)
-            y = out.interior()[b0:b1]
-            if up:
-                base = y[:, ::2, ::2]
-                copies = copies and all(bitwise(y[:, ry::2, rx::2], base) for ry in range(2) for rx in range(2))
-                y = base
-            acc.add(y, want, e, t)
-        if keep:
-            kept.append((s, mag))
-        del s, mag, e
-    if head:
-        r["max"] = float(torch.tensor(heads, dtype=F64).max())
-    else:
-        r.update(acc.result())
-    if up:
-        r["up_copies"] = copies
-    if keep:
-        st.stash[i] = dict(s=torch.cat([p[0] for p in kept]), mag=torch.cat([p[1] for p in kept]), n=n, bias=b64,
-                           slope=slope, res=res.clone() if res is not None else None, out=out, up=up, head=head)
-    r.update(kind="head" if head else ("s2d" if s2d_layer else "k%d" % k), cout=cout, grid="%dx%d" % (oh, ow))
-    return r
-
-
-def check_buffers(st):
-    """every halo zero; in every activation buffer the channels no producer owns are zero"""
-    owned = {}
-    for i, v in st.outs.items():
-        if isinstance(v, View):
-            owned.setdefault(id(v.buf), (v.buf, []))[1].append((v.off, v.off + v.c))
-    bufs = [b for b, _ in owned.values()]
-    bufs += [a["xs"] for kind, a in st.plan["steps"] if kind in ("s2d", "first")]
-    ok = all(halo_zero(b) for b in bufs)
-    for buf, ranges in owned.values():
-        mask = torch.ones(buf.shape[-1], dtype=torch.bool, device=buf.device)
-        for lo, hi in ranges:
-            mask[lo:hi] = False
-        ok = ok and bool((buf[..., mask] == 0).all())
-    concat = sorted({buf.shape[-1] for buf, rs in owned.values() if len({r for r in rs}) > 1})
-    return ok, concat
 
 
 def check_decode(st):
     """io against float64 _decode_ref of the actual head buffers"""
     model = st.model
-    heads = _yolov3_heads(1)
+    heads = yolov3_heads(1)
     off = 0
     worst = 0.0
     for (li, p), (anchors, _, stride), yi in zip(st.plan["heads"], heads, model.yolo_layers):
         layer = model.module_list[yi]
         assert torch.equal(layer.anchors.float(), anchors) and layer.stride == stride
-        want, mag = _decode_ref(p, anchors, stride, 1.0, 1)
+        want, mag = decode_ref(p, anchors, stride, 1.0, 1)
         rows = want.shape[1]
         got = st.io[:, off:off + rows].double()
         ratio = (got - want).abs() / (mag * 2.0 ** -20)
@@ -418,8 +102,7 @@ def run_forward(name, stash):
     model = model.cuda().eval()
     model.use_cuda_graph = True
     xa, xb = (torch.rand(batch, 3, h, w, generator=torch.Generator().manual_seed(s)).to(dev) for s in X_SEEDS)
-    st = Run()
-    st.name, st.model = name, model
+    st = Run(name, model)
     with torch.no_grad():
         io_a = model(xa)[0].clone()
         st.io, _ = model(xb)
@@ -622,7 +305,7 @@ def test_bounds_reject_plausible_bugs(bench):
     assert wrong.shape == prev["res"].shape
     found["shortcut_wrong_layer"] = conv_result(pk["res"], res=wrong)
     # the neighbouring layer's PReLU slope
-    s_next = _slope(st.model, pk["res"] - 1)
+    s_next = slope(st.model, pk["res"] - 1)
     assert s_next != prev["slope"]
     found["neighbour_slope"] = conv_result(pk["res"], slope=s_next)
     # BN folding without eps, on every BN layer: the worst and the count
@@ -639,7 +322,7 @@ def test_bounds_reject_plausible_bugs(bench):
     v32 = want.float()
     e = d["n"] * 2.0 ** -23 * d["mag"]
     assert passed(bf16_check(v32.to(BF16), want, e, t))
-    found["rtz_output"] = bf16_check(tsf.rtz_bf16(v32), want, e, t)
+    found["rtz_output"] = bf16_check(rtz_bf16(v32), want, e, t)
     del want, t, v32, e
     # the bias missing on the second 256-filter tile of a head
     h = st.stash[pk["head"]]

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import helpers
+from f64_refs import decode_ref, yolov3_heads
 
 pytestmark = pytest.mark.gpu
 
@@ -224,43 +225,6 @@ def test_detect_postprocess_equals_per_image_pipeline(inputs):
 # ---------------------------------------------------------------------------------------------------------------------
 # ryolo_yolo_decode against float64
 # ---------------------------------------------------------------------------------------------------------------------
-def _yolov3_heads(nc):
-    """(anchors [na, 3] in pixels, grid, stride) of the three heads of the 608x608 yolov3 cfg, in output row order"""
-    from rotate_yolov3_b200 import cfgs
-    from rotate_yolov3_b200.parse_config import parse_model_cfg
-    heads = []
-    for mdef, ng in zip([m for m in parse_model_cfg(cfgs.yolov3_cfg(classes=nc)) if m["type"] == "yolo"], (19, 38, 76)):
-        lo, hi = [int(v) for v in mdef["mask"].split("-")]
-        heads.append((torch.tensor(mdef["anchors"][lo:hi + 1], dtype=torch.float32), ng, 608 / ng))
-    return heads
-
-
-def _decode_ref(p, anchors, stride, ctx, nc):
-    """float64 model/models.py:198-227 ('default' arc): returns (io [B, na*ny*nx, 6+nc], per-component magnitude M)"""
-    bs, _, ny, nx = p.shape
-    na = anchors.shape[0]
-    t = p.double().view(bs, na, nc + 6, ny, nx).permute(0, 1, 3, 4, 2)
-    a = anchors.double().to(p.device)
-    aw = (a[:, 0] / stride).view(1, na, 1, 1)
-    ah = (a[:, 1] / stride).view(1, na, 1, 1)
-    at = a[:, 2].view(1, na, 1, 1)
-    gx = torch.arange(nx, device=p.device, dtype=torch.float64).view(1, 1, 1, nx)
-    gy = torch.arange(ny, device=p.device, dtype=torch.float64).view(1, 1, ny, 1)
-    sx, sy = torch.sigmoid(t[..., 0]), torch.sigmoid(t[..., 1])
-    w0 = torch.exp(t[..., 2]) * aw * stride
-    h = torch.exp(t[..., 3]) * ah * stride / ctx
-    th = torch.atan(t[..., 4])
-    want = [(sx + gx) * stride, (sy + gy) * stride, w0 - h * (ctx - 1), h, th + at]
-    mag = [(sx.abs() + gx) * stride, (sy.abs() + gy) * stride, w0.abs() + (h * (ctx - 1)).abs(), h.abs(),
-           th.abs() + at.abs()]
-    for k in range(5, nc + 6):
-        s = torch.ones_like(sx) if (nc == 1 and k == 6) else torch.sigmoid(t[..., k])
-        want.append(s)
-        mag.append(s.abs())
-    flat = lambda xs: torch.stack(xs, -1).reshape(bs, na * ny * nx, nc + 6)
-    return flat(want), flat(mag)
-
-
 @pytest.mark.parametrize("nc", [1, 3])
 @pytest.mark.parametrize("ctx", [1.0, 1.25])
 def test_yolo_decode_vs_float64_at_608_heads(nc, ctx):
@@ -268,7 +232,7 @@ def test_yolo_decode_vs_float64_at_608_heads(nc, ctx):
     6+nc] buffer through row_offset; nc = 1 runs the shared-memory staged kernel, nc = 3 the direct one.
     |got - want| <= 2^-20 * M per component, M = the sum of the magnitudes of the terms; p_out bit-exact."""
     import rotate_yolov3_b200 as pkg
-    heads = _yolov3_heads(nc)
+    heads = yolov3_heads(nc)
     bs, no, pad = 32, nc + 6, 37
     rows = sum(a.shape[0] * ng * ng for a, ng, _ in heads)
     assert rows == 545832
@@ -286,7 +250,7 @@ def test_yolo_decode_vs_float64_at_608_heads(nc, ctx):
                                             pkg._lib.stream_ptr())
         assert st == 0
         assert torch.equal(pp, p.view(bs, na, no, ng, ng).permute(0, 1, 3, 4, 2)), (ng, "p_out")
-        want, mag = _decode_ref(p, anchors, stride, ctx, nc)
+        want, mag = decode_ref(p, anchors, stride, ctx, nc)
         got = io[:, off:off + na * ng * ng].double()
         ratio = (got - want).abs() / (mag * 2.0 ** -20)
         ratio = torch.where(got == want, torch.zeros_like(ratio), ratio)   # M == 0 only where want == 0 exactly

@@ -18,65 +18,19 @@ of the reference breaks the bound by a factor of thousands.
 
 The one-pass variance E[z^2] - E[z]^2 at mean / std = 8 (E[z^2] / var = 68.5) was measured 1.6e-5 relative to float64
 against a bound of 1.4e-4 (the sum bound times that amplification); at mean / std = 0.3 it is 2e-7 to 5e-7."""
-import contextlib
 import ctypes
 import math
 
 import pytest
 import torch
 
-from test_wgrad_gpu import CASES, Case
+from builders import STEP_HYP, assert_same, repeat, ryolo_lib, small_train_model, step_targets
+from f64_refs import CASES, Case, bf, gemm_sms
 
 pytestmark = pytest.mark.gpu
 
 KAPPA_SUM = 2.0
 U = 2.0 ** -24
-
-
-def _lib():
-    import rotate_yolov3_b200 as pkg
-    return pkg._lib
-
-
-def _bf(t):
-    return t.to(torch.bfloat16).float()
-
-
-@contextlib.contextmanager
-def side_load():
-    """large bf16 matmuls on a second stream, running while the body enqueues its kernels on the current stream"""
-    cur = torch.cuda.current_stream()
-    s = torch.cuda.Stream()
-    a = torch.randn(8192, 8192, device="cuda", dtype=torch.bfloat16)
-    s.wait_stream(cur)
-    outs = []
-    with torch.cuda.stream(s):
-        for _ in range(12):
-            outs.append(a @ a)
-    yield
-    torch.cuda.synchronize()
-    del outs
-
-
-def repeat(fn, n=3):
-    """fn() -> tuple of result tensors; n runs, the last one next to the side-stream load; all bitwise equal"""
-    runs = []
-    for i in range(n):
-        if i == n - 1:
-            with side_load():
-                res = fn()
-        else:
-            res = fn()
-        torch.cuda.synchronize()
-        runs.append(tuple(t.clone() for t in res))
-    for r in runs[1:]:
-        for k, (a, b) in enumerate(zip(runs[0], r)):
-            assert torch.equal(a, b), ("run differs", k)
-    return runs[0]
-
-
-def gemm_sm_count():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -104,7 +58,7 @@ def bn_geometry(b, h, w, c, cs, sms):
 
 
 def bn_stats_call(zb, cs, b, h, w, c, eps=1e-5, momentum=0.1, gamma=None, beta=None, rm=None, rv=None):
-    L = _lib()
+    L = ryolo_lib()
     dev = zb.device
     sums = torch.full((2 * c,), 3.0, device=dev)
     mean, inv, sc, sh = (torch.empty(c, device=dev) for _ in range(4))
@@ -126,10 +80,10 @@ def sum_ratio(got, want, mag, n_add):
                                              ("pipe", 2048, 2048, 2, 5, 6), ("direct", 32, 64, 4, 38, 38)])
 def test_bn_stats_finalize_is_bitwise_repeatable(path, c, cs, b, h, w):
     from rotate_yolov3_b200 import layout as Lo
-    geo = bn_geometry(b, h, w, c, cs, gemm_sm_count())
+    geo = bn_geometry(b, h, w, c, cs, gemm_sms())
     assert geo["pipe"] == (path == "pipe") and geo["grid"] > 8
     g = torch.Generator().manual_seed(c + h)
-    z = _bf(torch.randn(b, c, h, w, generator=g) * 1.3 + 0.4).cuda()
+    z = bf(torch.randn(b, c, h, w, generator=g) * 1.3 + 0.4).cuda()
     zb = Lo.to_padded_nhwc(z, cs)
     gamma, beta = (0.5 + torch.rand(c, generator=g)).cuda(), torch.randn(c, generator=g).cuda()
     rm0, rv0 = torch.randn(c, generator=g).cuda(), (0.5 + torch.rand(c, generator=g)).cuda()
@@ -144,16 +98,16 @@ def test_bn_stats_finalize_is_bitwise_repeatable(path, c, cs, b, h, w):
 
 def _bwd_inputs(c, b, h, w, up, seed):
     g = torch.Generator().manual_seed(seed)
-    z = _bf(torch.randn(b, c, h, w, generator=g) * 1.2 + 0.1).cuda()
+    z = bf(torch.randn(b, c, h, w, generator=g) * 1.2 + 0.1).cuda()
     oh, ow = (2 * h, 2 * w) if up == 1 else (h, w)
-    dy = _bf(torch.randn(b, c, oh, ow, generator=g)).cuda()
+    dy = bf(torch.randn(b, c, oh, ow, generator=g)).cuda()
     mean = (0.1 * torch.randn(c, generator=g)).cuda()
     inv = (0.5 + torch.rand(c, generator=g)).cuda()
     return z, dy, mean, inv
 
 
 def bn_bwd_call(dyb, dcs, up, zb_master, cs, b, h, w, c, scale, shift, mean, inv, slope, has_act=1, slope_dev=None):
-    L = _lib()
+    L = ryolo_lib()
     zb = zb_master.clone()                          # the call overwrites z with dz
     sums = torch.full((2 * c + 1,), 5.0, device="cuda")
     st = L.lib.ryolo_bn_act_bwd(L.ptr(dyb), dcs, up, L.ptr(zb), cs, b, h, w, c, L.ptr(scale), L.ptr(shift), L.ptr(mean),
@@ -192,7 +146,7 @@ def test_wgrad_is_bitwise_repeatable(name):
 
 
 def _head_grad_call(g, B, C, ny, nx, cs):
-    L = _lib()
+    L = ryolo_lib()
     dst = torch.zeros((B, ny + 2, nx + 2, cs), dtype=torch.bfloat16, device="cuda")
     bias = torch.zeros(C, device="cuda")
     L.check(L.lib.ryolo_head_grad_nchw_to_padded(L.ptr(g), B, C, ny, nx, L.ptr(dst), cs, L.ptr(bias), L.stream_ptr()), "hg")
@@ -225,7 +179,7 @@ def _head(B, na, ny, nx, no, seed):
 
 
 def _obj_call(x, tobj, pw):
-    L = _lib()
+    L = ryolo_lib()
     B, na, ny, nx, no = x.shape
     strides = (ctypes.c_longlong * 5)(*x.stride())
     out = torch.zeros(1, dtype=torch.float64, device="cuda")
@@ -264,7 +218,7 @@ def _rows(B, na, ny, nx, n_rows, seed):
 
 
 def _scatter_call(g0, idx, mask, vals, scale):
-    L = _lib()
+    L = ryolo_lib()
     g = g0.clone()
     B, na, ny, nx, no = g.shape
     strides = (ctypes.c_longlong * 5)(*g.stride())
@@ -314,13 +268,13 @@ def test_rows_scatter_add_repeatable_and_vs_float64():
 ])
 def test_bn_stats_vs_float64(name, c, cs, b, h, w, mu):
     from rotate_yolov3_b200 import layout as Lo
-    geo = bn_geometry(b, h, w, c, cs, gemm_sm_count())
+    geo = bn_geometry(b, h, w, c, cs, gemm_sms())
     if name == "few_ctas":
         assert geo["grid"] < 8
     if name == "short_last":
         assert geo["rpb"] == 2 and (b * h) % geo["rpb"] != 0
     g = torch.Generator().manual_seed(h + c)
-    z = _bf(torch.randn(b, c, h, w, generator=g) + mu).cuda()
+    z = bf(torch.randn(b, c, h, w, generator=g) + mu).cuda()
     zb = Lo.to_padded_nhwc(z, cs)
     eps = 1e-5
     sums, mean, inv, _, _ = bn_stats_call(zb, cs, b, h, w, c, eps=eps)
@@ -359,7 +313,7 @@ def test_bn_bwd_sums_vs_float64(cs_mode):
     from rotate_yolov3_b200 import layout as Lo
     c, b, h, w = 64, 2, 48, 120
     cs = c if cs_mode == "pipe" else 128
-    geo = bn_geometry(b, h, w, c, cs, gemm_sm_count())
+    geo = bn_geometry(b, h, w, c, cs, gemm_sms())
     z, dy, mean, inv = _bwd_inputs(c, b, h, w, 0, 31)
     zb, dyb = Lo.to_padded_nhwc(z, cs), Lo.to_padded_nhwc(dy, cs)
     one, zero = torch.ones(c, device="cuda"), torch.zeros(c, device="cuda")
@@ -380,21 +334,8 @@ def test_bn_bwd_sums_vs_float64(cs_mode):
 
 # ---------------------------------------------------------------------------------------------------------------
 # step level
-HYP = {"giou": 0.1, "cls": 27.76, "cls_pw": 1.0, "obj": 20.35, "obj_pw": 1.0, "iou_t": 0.3, "ang_t": math.pi / 6,
-       "reg": 1.0, "context_factor": 1.0}
-
-
-def _targets():
-    # normalised [image, class, x, y, w, h, angle]; sizes near the 900 / 3000 px^2 anchors at +-45 degrees of a 160 x 128
-    # image.  Rows 0 and 3 are the same target: two matched rows on the same cell and anchor.
-    t = torch.tensor([[0, 0, 0.31, 0.42, 0.42, 0.10, 0.78], [0, 0, 0.70, 0.30, 0.75, 0.19, -0.77],
-                      [1, 0, 0.52, 0.61, 0.40, 0.11, -0.80], [0, 0, 0.31, 0.42, 0.42, 0.10, 0.78],
-                      [1, 0, 0.20, 0.75, 0.78, 0.18, 0.76]])
-    return t.cuda()
-
-
 def _setup(m):
-    m.nc, m.hyp, m.arc = 1, HYP, "default"
+    m.nc, m.hyp, m.arc = 1, STEP_HYP, "default"
     return m
 
 
@@ -403,41 +344,34 @@ def _step(m, x, t):
     for p in m.parameters():
         p.grad = None
     ps = m(x)
-    loss, items = compute_loss(ps, t.clone(), m, HYP)
+    loss, items = compute_loss(ps, t.clone(), m, STEP_HYP)
     loss.backward()
     out = {"p%d" % k: p.detach().clone() for k, p in enumerate(ps)}
     out["loss"], out["items"] = loss.detach().clone(), items.detach().clone()
     for n, p in m.named_parameters():
         out["grad:" + n] = p.grad.clone()
-    for n, bf in m.named_buffers():
-        out["buf:" + n] = bf.clone()
+    for n, buf in m.named_buffers():
+        out["buf:" + n] = buf.clone()
     torch.cuda.synchronize()
     return out
 
 
-def _same(a, b, what):
-    assert a.keys() == b.keys()
-    bad = [k for k in a if not torch.equal(a[k], b[k])]
-    assert not bad, (what, bad[:8], len(bad))
-
-
 def test_training_step_is_bitwise_repeatable():
-    from test_train_gpu import _model
-    m = _setup(_model())
+    m = _setup(small_train_model())
     sd0 = {k: v.clone() for k, v in m.state_dict().items()}
     x = torch.rand(2, 3, 128, 160, generator=torch.Generator().manual_seed(17)).cuda()
-    t = _targets()
+    t = step_targets()
     ref = _step(m, x, t)
     assert float(ref["items"][2]) > 0            # matched rows exist (regression term)
     assert all(torch.isfinite(v).all() for v in ref.values() if v.is_floating_point())
     # 1. the same model again, from the same restored state
     m.load_state_dict(sd0)
-    _same(ref, _step(m, x, t), "rerun")
+    assert_same(ref, _step(m, x, t), "rerun")
     # 2. a second instance: parameters, plan buffers and scratch at other addresses
-    m2 = _setup(_model())
+    m2 = _setup(small_train_model())
     m2.load_state_dict(sd0)
     assert m2.module_list[0].Conv2d.weight.data_ptr() != m.module_list[0].Conv2d.weight.data_ptr()
-    _same(ref, _step(m2, x, t), "second instance")
+    assert_same(ref, _step(m2, x, t), "second instance")
     del m2
     # 3. on another stream: per-stream scratch buffers
     m.load_state_dict(sd0)
@@ -446,12 +380,12 @@ def test_training_step_is_bitwise_repeatable():
     with torch.cuda.stream(side):
         out = _step(m, x, t)
     cur.wait_stream(side)
-    _same(ref, out, "side stream")
+    assert_same(ref, out, "side stream")
     # 4. CUDA graphs: the capture step and a replayed step
-    m3 = _setup(_model())
+    m3 = _setup(small_train_model())
     m3.load_state_dict(sd0)
     m3.use_cuda_graph = True
-    _same(ref, _step(m3, x, t), "graph capture step")
+    assert_same(ref, _step(m3, x, t), "graph capture step")
     m3.load_state_dict(sd0)                      # in place: the captured graphs stay valid
-    _same(ref, _step(m3, x, t), "graph replay")
+    assert_same(ref, _step(m3, x, t), "graph replay")
     assert m3._tplan.replayed_kernels > 0

@@ -3,52 +3,26 @@ cfg/HRSC+/yolov3_512_matrix.cfg): Darknet builds the reference's module tree, st
 (tests/golden/darknet_m_golden.npz, make_golden_m.py), .weights files are byte-identical to the reference's
 save_weights, the plans that have no kernel for these graphs refuse them, and the phase decomposition that the eval
 plan runs the dilated convs through equals F.conv2d(dilation=...) in float64."""
-import contextlib
 import hashlib
 import json
-import os
 import re
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import GOLDEN, init_darknet_weights
+from builders import DILATIONS, golden_text, m_cfg_text, m_golden, m_model, phase_merge, phase_split
+from helpers import init_darknet_weights
 
-REF = os.path.join(GOLDEN, "reference_cfg")
 M_CFGS = ["cfg/yolov3-m.cfg", "cfg/HRSC/yolov3-m.cfg", "cfg/HRSC+/yolov3_512_matrix.cfg"]
-DILATIONS = [(1, 2), (2, 1), (1, 4), (4, 1), (1, 8), (8, 1)]
-
-
-def _golden():
-    return np.load(os.path.join(GOLDEN, "darknet_m_golden.npz"), allow_pickle=True)   # per-parameter gradient samples
-
-
-def _text(g, key):
-    return g[key].item().decode()
-
-
-def m_cfg_text(cfg):
-    """the cfg as text; the matrix cfg's anchor file (not shipped by the reference) replaced by the golden's line"""
-    with open(os.path.join(REF, cfg)) as f:
-        text = f.read()
-    if "matrix" in cfg:
-        text = re.sub(r"^anchors\s*=.*$", "anchors = " + _text(_golden(), "matrix_anchors"), text, flags=re.M)
-    return text
-
-
-def m_model(cfg="cfg/yolov3-m.cfg", arc="default", **kw):
-    import rotate_yolov3_b200 as pkg
-    return pkg.Darknet(m_cfg_text(cfg), {"context_factor": 1.0}, arc=arc, **kw)
 
 
 @pytest.mark.parametrize("cfg", M_CFGS)
 def test_darknet_builds_the_reference_module_tree(cfg):
-    g = _golden()
+    g = m_golden()
     m = m_model(cfg)
-    assert repr(m.module_list) == _text(g, "tree:" + cfg)
-    assert [[k, list(v.shape)] for k, v in m.state_dict().items()] == json.loads(_text(g, "state:" + cfg))
+    assert repr(m.module_list) == golden_text(g, "tree:" + cfg)
+    assert [[k, list(v.shape)] for k, v in m.state_dict().items()] == json.loads(golden_text(g, "state:" + cfg))
     assert sum(p.numel() for p in m.parameters()) == int(g["n_params:" + cfg])
     assert len(m.yolo_layers) == 16 and all(m.module_list[i].na == 72 for i in m.yolo_layers)
     dconv = [i for i, d in enumerate(m.module_defs) if d["type"] == "d-convolutional"]
@@ -65,14 +39,14 @@ def test_checkpoint_round_trip_with_the_reference_keys():
 
 def test_weights_file_is_byte_identical_to_the_reference(tmp_path):
     from rotate_yolov3_b200.weights_io import load_darknet_weights, save_weights
-    g = _golden()
-    m = init_darknet_weights(m_model(), seed=json.loads(_text(g, "seeds"))["eval_w"])
+    g = m_golden()
+    m = init_darknet_weights(m_model(), seed=json.loads(golden_text(g, "seeds"))["eval_w"])
     path = str(tmp_path / "m.weights")
     save_weights(m, path)
     with open(path, "rb") as f:
         data = f.read()
     assert len(data) == int(g["weights_bytes"])
-    assert hashlib.sha256(data).hexdigest() == _text(g, "weights_sha256")
+    assert hashlib.sha256(data).hexdigest() == golden_text(g, "weights_sha256")
     # the branch blocks' own (unused) conv / BN weights are in the file, like the reference's, and load back
     m2 = m_model()
     load_darknet_weights(m2, path)
@@ -112,7 +86,7 @@ def test_training_plan_gradient_slots_and_parity_refusal():
     from rotate_yolov3_b200.parity_path import ParityPlan
     from rotate_yolov3_b200.train_path import TrainPlan
     m = m_model()
-    has = [bool(h) for h in _golden()["default_has_grad"]]
+    has = [bool(h) for h in m_golden()["default_has_grad"]]
     for h, w, grid in ((128, 160, (4, 5)), (416, 416, (13, 13)), (608, 608, (19, 19))):
         tp = TrainPlan(m, 2, h, w, torch.device("cpu"))
         got = [(int(n.split(".")[1]), ".".join(n.split(".")[2:])) in tp.param_slots for n in tp.names]
@@ -130,23 +104,6 @@ def test_training_plan_gradient_slots_and_parity_refusal():
     for training in (True, False):
         with pytest.raises(NotImplementedError, match="weight_from"):
             ParityPlan(mp, 1, 64, 64, torch.device("cpu"), training)
-
-
-def phase_split(x, dh, dw):
-    """[B, C, H, W] -> [B*dh*dw, C, ceil(H/dh), ceil(W/dw)]: image (b*dh + ry)*dw + rx holds x[b, :, ry::dh, rx::dw],
-    zero-filled where the phase is short (the index map of ryolo_dilate_split)"""
-    b, c, h, w = x.shape
-    hp, wp = -(-h // dh), -(-w // dw)
-    full = x.new_zeros(b, c, hp * dh, wp * dw)
-    full[:, :, :h, :w] = x
-    return full.view(b, c, hp, dh, wp, dw).permute(0, 3, 5, 1, 2, 4).reshape(b * dh * dw, c, hp, wp)
-
-
-def phase_merge(xp, b, h, w, dh, dw):
-    """inverse of phase_split on the interior (the index map of ryolo_dilate_merge)"""
-    c, hp, wp = xp.shape[1:]
-    full = xp.view(b, dh, dw, c, hp, wp).permute(0, 3, 4, 1, 5, 2).reshape(b, c, hp * dh, wp * dw)
-    return full[:, :, :h, :w]
 
 
 @pytest.mark.parametrize("dil", DILATIONS)

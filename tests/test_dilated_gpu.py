@@ -4,7 +4,7 @@ model's output (tests/golden/darknet_m_golden.npz, make_golden_m.py).
 
 A dilated 3x3 conv runs as ryolo_dilate_split -> ordinary pad-1 3x3 conv_bn_act_fwd on the B*dh*dw phase images ->
 ryolo_dilate_merge (+ the shortcut that follows it).  Each launch is re-run on the tensors the forward left in the plan,
-and checked on its own: the split and the merge bit for bit against the index map of test_dilated_cfg.py, the conv with
+and checked on its own: the split and the merge bit for bit against the index map of phase_split, the conv with
 the bound of test_detect_forward_f64_gpu.py (E = n 2^-23 A, n = taps * cin_pad / 16; |got - want| <= 2^-8 (|want| + E)
 + E; no bias, activation or residual terms: the branch convs have none)."""
 import ctypes
@@ -15,15 +15,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from builders import DILATIONS, golden_text, m_golden, m_model, phase_merge, phase_split, ryolo_lib
 from helpers import init_darknet_weights
-from test_dilated_cfg import DILATIONS, _golden, _text, m_model, phase_merge, phase_split
 
 pytestmark = pytest.mark.gpu
-
-
-def _lib():
-    from rotate_yolov3_b200 import _lib
-    return _lib
 
 
 def _padded(t, cs):
@@ -37,14 +32,14 @@ def _nchw(buf, c):
 
 
 def _split(x, xcs, b, h, w, c, dh, dw, xp):
-    lib = _lib()
+    lib = ryolo_lib()
     st = lib.lib.ryolo_dilate_split(ctypes.c_void_p(x), xcs, b, h, w, c, dh, dw, lib.ptr(xp), xp.shape[-1],
                                     lib.stream_ptr(xp.device))
     lib.check(st, "ryolo_dilate_split")
 
 
 def _merge(yp, b, h, w, c, dh, dw, r, rcs, acc, y, ycs):
-    lib = _lib()
+    lib = ryolo_lib()
     st = lib.lib.ryolo_dilate_merge(lib.ptr(yp), yp.shape[-1], b, h, w, c, dh, dw, ctypes.c_void_p(r) if r else None, rcs,
                                     acc, ctypes.c_void_p(y), ycs, lib.stream_ptr(yp.device))
     lib.check(st, "ryolo_dilate_merge")
@@ -128,8 +123,8 @@ def test_every_dilated_launch_vs_float64_at_416():
 
 
 def test_yolov3m_eval_vs_reference_model_output():
-    g = _golden()
-    sd = json.loads(_text(g, "seeds"))
+    g = m_golden()
+    sd = json.loads(golden_text(g, "seeds"))
     m = init_darknet_weights(m_model(), seed=sd["eval_w"]).cuda().eval()
     x = torch.rand(1, 3, 416, 416, generator=torch.Generator().manual_seed(sd["eval_x"])).cuda()
     with torch.no_grad():
@@ -185,7 +180,7 @@ def test_dropin_builds_and_runs_yolov3m():
     import rotate_yolov3_b200.dropin as dropin
     dropin.install()
     Darknet = sys.modules["model.models"].Darknet
-    from test_dilated_cfg import m_cfg_text
+    from builders import m_cfg_text
     m = Darknet(m_cfg_text("cfg/yolov3-m.cfg"), {"context_factor": 1.0}, arc="default")
     init_darknet_weights(m, seed=7)
     m = m.cuda().eval()

@@ -6,7 +6,7 @@ index map with rows and columns swapped cannot pass; an odd batch, so GEMM tiles
 (loss = sum (p * G)) reaches all 16 heads.
 
 The blocks this graph shares with yolov3 (convs, BatchNorm statistics, bn_act_fwd / bn_act_bwd, wgrad, dgrad, heads,
-head bias sums) are checked by the functions and bounds of test_train_step_f64_gpu.py, unchanged (see its docstring:
+head bias sums) are checked by checked_step.py with the bounds of test_train_step_f64_gpu.py (see its docstring:
 E = n 2^-23 A per conv, half a bf16 ulp + E for bf16 outputs, E + 2^-24 |want| for fp32 ones, L 2^-24 sum |terms| for
 reductions).  What this graph adds, checked here:
 
@@ -51,36 +51,22 @@ Bias ratios (mean signed error) stay <= 0.16.  Bugs put in fail by a factor >= 2
 the last ragged phase column dropped from a (1, 8) wgrad 1.7e3, (dh, dw) swapped in the dgrad 9.6e3, one of seven uses
 missing from owner 100 1.0e3, block 109's kink at z 996, a bias on a weight_from head 6.2e3.  Whole file: 18 s."""
 import ctypes
-import time
 import traceback
 
 import pytest
 import torch
-import torch.nn.functional as F
 
-import test_train_step_f64_gpu as T
-import test_wgrad_gpu as wgrad_test
+from builders import m_model, phase_merge, phase_split, ryolo_lib
+from checked_step import Step, check_block_bwd, conv_updates, dy_of, dz_checks, run_step, slope_of
+from f64_refs import (BF16, F64, TINY, U, bad_entries, bf16_check, bitwise, bn_chain, check_z, conv_taps, dil_conv,
+                      dil_wgrad_ref, f32_check, gemm_sms, halo_zero, interior, nchw, nhwc, passed, rup, s2_refs,
+                      sum_check, tapsum, vint, wgrad_ratio, wgrad_ref)
 from helpers import init_darknet_weights, wgrad_plan
-from test_dilated_cfg import m_model, phase_merge, phase_split
 
 pytestmark = pytest.mark.gpu
 
 SHAPES = [(2, 416, 416), (3, 352, 608), (2, 128, 160)]
-U, BF16, F64, TINY = T.U, T.BF16, T.F64, T.TINY
 BUG_OWNER = 100          # owner whose per-use weight gradients the bound self-test keeps (seven uses, 256 x 128 x 9)
-
-
-def _lib():
-    from rotate_yolov3_b200 import _lib
-    return _lib
-
-
-def nchw(t):
-    return t.permute(0, 3, 1, 2).contiguous()
-
-
-def nhwc(t):
-    return t.permute(0, 2, 3, 1)
 
 
 def psplit(x, dh, dw):
@@ -93,65 +79,10 @@ def pmerge(xp, b, h, w, dh, dw):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# float64 references of the dilated and stride-2 convs: tap sums of shifted NHWC operands (value, magnitude)
-def dil_conv(x, w64, dh, dw, adjoint=False):
-    """the 3x3 conv with dilation and padding (dh, dw) of NHWC x with weight [cout, cin, 3, 3]; adjoint: its input
-    gradient from dz (taps mirrored, W not transposed)"""
-    b, h, wd, c = x.shape
-    xp = F.pad(x.double(), (0, 0, dw, dw, dh, dh))
-    xa = xp.abs()
-    n = w64.shape[1] if adjoint else w64.shape[0]
-    out = torch.zeros(b * h * wd, n, dtype=F64, device=x.device)
-    mag = torch.zeros_like(out)
-    for kh in range(3):
-        for kw in range(3):
-            oy, ox = (kh - 1) * dh, (kw - 1) * dw
-            m = w64[:, :, kh, kw] if adjoint else w64[:, :, kh, kw].t()
-            if adjoint:
-                oy, ox = -oy, -ox
-            sl = (slice(None), slice(dh + oy, dh + oy + h), slice(dw + ox, dw + ox + wd))
-            out.addmm_(xp[sl].reshape(-1, c), m)
-            mag.addmm_(xa[sl].reshape(-1, c), m.abs())
-    return out.view(b, h, wd, n), mag.view(b, h, wd, n)
-
-
-def dil_wgrad_ref(x, dz, dh, dw):
-    """dW[kh * 3 + kw, co, ci] = sum_p dz(p, co) x(p + (dh (kh - 1), dw (kw - 1)), ci): value and magnitude"""
-    b, h, wd, cin = x.shape
-    xp = F.pad(x.double(), (0, 0, dw, dw, dh, dh))
-    d = dz.double().reshape(-1, dz.shape[3])
-    da = d.abs()
-    outs, mags = [], []
-    for kh in range(3):
-        for kw in range(3):
-            a = xp[:, kh * dh:kh * dh + h, kw * dw:kw * dw + wd].reshape(-1, cin)
-            outs.append(d.t() @ a)
-            mags.append(da.t() @ a.abs())
-    return torch.stack(outs), torch.stack(mags)
-
-
-def s2_refs(x, dz, w64):
-    """3x3 / stride 2 / pad 1 conv on the odd grid of x: torch's float64 weight gradient in the kernel's [t, co, ci]
-    layout and the input gradient (conv_transpose2d, output padding up to x's size), each with its magnitude"""
-    x64, d64 = nchw(x.double()), nchw(dz.double())
-    h, w = x.shape[1], x.shape[2]
-    op = (h - (2 * dz.shape[1] - 1), w - (2 * dz.shape[2] - 1))
-    shape = tuple(w64.shape)
-
-    def gw(a, d):
-        return torch.nn.grad.conv2d_weight(a, shape, d, stride=2, padding=1).permute(2, 3, 0, 1).reshape(9, shape[0],
-                                                                                                         shape[1])
-
-    def dx(d, ww):
-        return nhwc(F.conv_transpose2d(d, ww, stride=2, padding=1, output_padding=op))
-    return gw(x64, d64), gw(x64.abs(), d64.abs()), dx(d64, w64), dx(d64.abs(), w64.abs())
-
-
-# ---------------------------------------------------------------------------------------------------------------
 # checks of the launches yolov3 does not have
 def merge_check(got, prior, v, acc):
     """the merge of a phase gradient v into the source gradient: bf16(prior + v) when it accumulates, else v"""
-    return T.bitwise(got, (prior.float() + v.float()).to(BF16) if acc else v.to(BF16))
+    return bitwise(got, (prior.float() + v.float()).to(BF16) if acc else v.to(BF16))
 
 
 def bias_act_bwd_check(z, d, dz_got, sums, bias, slope, chain, kink_at_z=False):
@@ -163,8 +94,8 @@ def bias_act_bwd_check(z, d, dz_got, sums, bias, slope, chain, kink_at_z=False):
     u64 = z64 + bias.double()
     pos = (z64 if kink_at_z else u64) > 0
     du = torch.where(pos, d64, d64 * float(slope))
-    r = T.bf16_check(dz_got.reshape(-1, c), du, 0.0, U * du.abs())
-    r["dbias"] = T.sum_check(sums[:c], du.sum(0), chain["sums"] + 1, du.abs().sum(0))
+    r = bf16_check(dz_got.reshape(-1, c), du, 0.0, U * du.abs())
+    r["dbias"] = sum_check(sums[:c], du.sum(0), chain["sums"] + 1, du.abs().sum(0))
     ds = d64 * u64.float().double()
     r["dslope"] = float((sums[2 * c].double() - ds[~pos].sum()).abs() / (chain["slope"] * U * ds[~pos].abs().sum() + TINY))
     return r
@@ -181,7 +112,7 @@ def wgrad_record(st, blk, got, snap, want, mag, plan_w):
     """the wgrad of a block whose dW is shared (an owner or a weight_from user): the increment, recorded per owner;
     otherwise the plain split-K check"""
     if "dw" not in snap:
-        return T.wgrad_ratio(got, want, mag, plan_w)
+        return wgrad_ratio(got, want, mag, plan_w)
     owner = blk.owner if blk.owner is not None else blk.i
     before = snap["dw"][:, :blk.cout, :got.shape[2]]
     inc = got.double() - before.double()
@@ -204,28 +135,28 @@ def _w64(st, blk):
 def check_linear_fwd(st, blk):
     """a weight_from block's forward (not a head), right after its launches"""
     w64 = _w64(st, blk)
-    x = T.vint(blk.src)
-    res = T.vint(blk.res) if blk.res is not None else None
-    y = T.interior(blk.y.buf, blk.y.ch_off, blk.cout)
-    n = T.conv_updates(blk)
+    x = vint(blk.src)
+    res = vint(blk.res) if blk.res is not None else None
+    y = interior(blk.y.buf, blk.y.ch_off, blk.cout)
+    n = conv_updates(blk)
     r = {}
     if blk.dil is None:
-        want, mag = T.tapsum(x, T.conv_taps(w64), blk.oh, blk.ow)
+        want, mag = tapsum(x, conv_taps(w64), blk.oh, blk.ow)
         t = 0.0
         if res is not None:
             want = want + res.double()
             t = U * (mag + res.double().abs())
-        rr = T.bf16_check(y, want, n * 2.0 ** -23 * mag, t)
+        rr = bf16_check(y, want, n * 2.0 ** -23 * mag, t)
         r["y"], r["y_bias"] = rr["max"], rr["bias"]
         return r
     dh, dw = blk.dil
-    r["split_bits"] = T.bitwise(T.interior(blk.xp, 0, blk.cin), psplit(x, dh, dw))
-    r["split_halo"] = T.halo_zero(blk.xp) and bool((blk.xp[..., blk.cin:] == 0).all())
-    got = pmerge(T.interior(blk.zp, 0, blk.cout), st.batch, blk.oh, blk.ow, dh, dw)
+    r["split_bits"] = bitwise(interior(blk.xp, 0, blk.cin), psplit(x, dh, dw))
+    r["split_halo"] = halo_zero(blk.xp) and bool((blk.xp[..., blk.cin:] == 0).all())
+    got = pmerge(interior(blk.zp, 0, blk.cout), st.batch, blk.oh, blk.ow, dh, dw)
     want, mag = dil_conv(x, w64, dh, dw)
-    rz = T.check_z(got, want, mag, n)
+    rz = check_z(got, want, mag, n)
     r["z"], r["z_bias"] = rz["max"], rz["bias"]
-    r["merge_bits"] = T.bitwise(y, (got.float() + res.float()).to(BF16) if res is not None else got)
+    r["merge_bits"] = bitwise(y, (got.float() + res.float()).to(BF16) if res is not None else got)
     return r
 
 
@@ -234,10 +165,10 @@ def fwd_heads(st):
     for blk in st.plan.blocks:
         if not (blk.is_head and blk.owner is not None):
             continue
-        want, mag = T.tapsum(T.vint(blk.src), T.conv_taps(_w64(st, blk)), blk.oh, blk.ow)
+        want, mag = tapsum(vint(blk.src), conv_taps(_w64(st, blk)), blk.oh, blk.ow)
         got = blk.out.detach().permute(0, 2, 3, 1)
-        e = T.conv_updates(blk) * 2.0 ** -23 * mag
-        st.fwd_lin[blk.i] = {"z": T.f32_check(got, want, e)["max"]}
+        e = conv_updates(blk) * 2.0 ** -23 * mag
+        st.fwd_lin[blk.i] = {"z": f32_check(got, want, e)["max"]}
         if "head" not in st.stash:
             bias = st.model.module_list[blk.i].Conv2d.bias.detach().double()
             st.stash["head"] = dict(got=got.clone(), want=want, e=e, bias=bias)
@@ -248,14 +179,14 @@ def check_bwd(st, blk, orig):
     plain = blk.owner is None and blk.i not in st.owner_of_users and (blk.is_head or blk.has_bn) and \
         not (blk.stride == 2 and not blk.s2d)
     if plain:
-        return T.check_block_bwd(st, blk, orig)
+        return check_block_bwd(st, blk, orig)
     r, snap = {}, {}
     try:
         if not blk.is_head:
-            snap["z"] = T.interior(blk.z, 0, blk.cout).clone()
-            snap["dy"], r["dy_mode"] = T.dy_of(st.plan, blk)
+            snap["z"] = interior(blk.z, 0, blk.cout).clone()
+            snap["dy"], r["dy_mode"] = dy_of(st.plan, blk)
             if blk.gres is not None:
-                snap["gres_prior"] = T.vint(blk.gres).clone()
+                snap["gres_prior"] = vint(blk.gres).clone()
         if blk.gsrc is not None:
             snap["gbuf"] = blk.gsrc.buf.clone()
         if blk.owner is not None or blk.i in st.owner_of_users:
@@ -277,21 +208,21 @@ def _outside(blk, gbuf, prior_buf):
     allowed[blk.gsrc.ch_off:blk.gsrc.ch_off + blk.gsrc.c] = True
     if blk.gres is not None and blk.gres.buf is gbuf:
         allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
-    return torch.equal(gbuf[..., ~allowed], prior_buf[..., ~allowed]) and T.halo_zero(gbuf)
+    return torch.equal(gbuf[..., ~allowed], prior_buf[..., ~allowed]) and halo_zero(gbuf)
 
 
 def _own_bwd_checks(st, blk, snap, r):
     model = st.model
     w64 = _w64(st, blk)
     if blk.is_head or blk.has_bn:
-        dz = T.dz_checks(st, blk, snap, r)
+        dz = dz_checks(st, blk, snap, r)
     else:
-        dz = T.interior(blk.z, 0, blk.cout)
+        dz = interior(blk.z, 0, blk.cout)
         if blk.owner is not None:        # linear: dz = dy, the shortcut gradient (+)= dy
-            r["dz_bits"] = T.bitwise(dz, snap["dy"].to(BF16))
+            r["dz_bits"] = bitwise(dz, snap["dy"].to(BF16))
         else:                            # block 109: bias + PReLU
-            chain = T.bn_chain(st.batch, blk.oh, blk.ow, blk.cout)
-            slope = T._slope_of(model, blk)
+            chain = bn_chain(st.batch, blk.oh, blk.ow, blk.cout)
+            slope = slope_of(model, blk)
             bias = model.module_list[blk.i].Conv2d.bias.detach()
             rb = bias_act_bwd_check(snap["z"], snap["dy"], dz, blk.bsums, bias, slope, chain)
             r["dz"], r["dz_bias"], r["dbeta"], r["dslope"] = rb["max"], rb["bias"], rb["dbias"], rb["dslope"]
@@ -299,26 +230,26 @@ def _own_bwd_checks(st, blk, snap, r):
                                     slope=slope, chain=chain)
         if blk.gres is not None:
             d = snap["dy"]
-            r["gres_bits"] = T.bitwise(T.vint(blk.gres), (snap["gres_prior"].float() + d).to(BF16) if blk.gres_acc
+            r["gres_bits"] = bitwise(vint(blk.gres), (snap["gres_prior"].float() + d).to(BF16) if blk.gres_acc
                                        else d.to(BF16))
-        r["dz_halo"] = T.halo_zero(blk.z)
-    x = T.vint(blk.src)
-    prior = T.interior(snap["gbuf"], blk.gsrc.ch_off, blk.gsrc.c)
+        r["dz_halo"] = halo_zero(blk.z)
+    x = vint(blk.src)
+    prior = interior(snap["gbuf"], blk.gsrc.ch_off, blk.gsrc.c)
     got_dw = blk.dw[:, :blk.cout, :blk.cin]
-    gemm_sms = wgrad_test.gemm_sms()
+    sms = gemm_sms()
     if blk.dil is not None:
         dh, dw = blk.dil
         b, h, w = st.batch, blk.src.h, blk.src.w
-        r["split_bits"] = T.bitwise(T.interior(blk.zp, 0, blk.cout), psplit(dz, dh, dw))
+        r["split_bits"] = bitwise(interior(blk.zp, 0, blk.cout), psplit(dz, dh, dw))
         wr, wm = dil_wgrad_ref(x, dz, dh, dw)
-        plan_w = wgrad_plan(3, blk.cin_pad, blk.cout_pad, blk.nb, blk.hp, blk.wp, gemm_sms)
+        plan_w = wgrad_plan(3, blk.cin_pad, blk.cout_pad, blk.nb, blk.hp, blk.wp, sms)
         r["wgrad"] = wgrad_record(st, blk, got_dw, snap, wr, wm, plan_w)
-        v = pmerge(T.interior(blk.dxp, 0, blk.cin), b, h, w, dh, dw)
+        v = pmerge(interior(blk.dxp, 0, blk.cin), b, h, w, dh, dw)
         want, mag = dil_conv(dz, w64, dh, dw, adjoint=True)
-        n = 9 * T.rup(blk.cout, 64) // 16
-        rd = T.check_z(v, want, mag, n)
+        n = 9 * rup(blk.cout, 64) // 16
+        rd = check_z(v, want, mag, n)
         r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
-        r["merge_bits"] = merge_check(T.vint(blk.gsrc), prior, v, blk.gsrc_acc)
+        r["merge_bits"] = merge_check(vint(blk.gsrc), prior, v, blk.gsrc_acc)
         if (h % dh or w % dw) and max(dh, dw) > st.stash.get("dil_d", 0):     # the widest ragged dilation
             st.stash["dil_d"] = max(dh, dw)
             st.stash["dil"] = dict(i=blk.i, x=x.clone(), dz=dz.clone(), dh=dh, dw=dw, got=got_dw.clone(),
@@ -326,112 +257,66 @@ def _own_bwd_checks(st, blk, snap, r):
                                    dxp=blk.dxp.clone(), w64=w64, n=n, prior_buf=snap["gbuf"], gsrc=blk.gsrc)
     elif blk.stride == 2:
         # zero-insert path: dz on the even pixels of the input grid, zeros elsewhere
-        up = T.interior(blk.dz_up, 0, blk.cout)
+        up = interior(blk.dz_up, 0, blk.cout)
         want_up = torch.zeros_like(up)
         want_up[:, ::2, ::2] = dz
-        r["zero_insert_bits"] = T.bitwise(up, want_up) and T.halo_zero(blk.dz_up)
+        r["zero_insert_bits"] = bitwise(up, want_up) and halo_zero(blk.dz_up)
         st.stash["zi"] = dict(up=up.clone(), dz=dz.clone())
         gw, gwm, want, mag = s2_refs(x, dz, w64)
-        plan_w = wgrad_plan(3, blk.cin_pad, blk.cout_pad, st.batch, blk.src.h, blk.src.w, gemm_sms)
+        plan_w = wgrad_plan(3, blk.cin_pad, blk.cout_pad, st.batch, blk.src.h, blk.src.w, sms)
         r["wgrad"] = wgrad_record(st, blk, got_dw, snap, gw, gwm, plan_w)
-        n = 9 * T.rup(blk.cout, 64) // 16
+        n = 9 * rup(blk.cout, 64) // 16
         t = 0.0
         if blk.gsrc_acc:
             want = want + prior.double()
             t = U * (mag + prior.double().abs())
-        rd = T.bf16_check(T.vint(blk.gsrc), want, n * 2.0 ** -23 * mag, t)
+        rd = bf16_check(vint(blk.gsrc), want, n * 2.0 ** -23 * mag, t)
         r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
     else:
         p = (blk.k - 1) // 2
-        wr, wm = T.wgrad_ref(x, dz, [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)])
-        plan_w = wgrad_plan(blk.k, blk.cin_pad, blk.cout_pad, st.batch, blk.src.h, blk.src.w, gemm_sms)
+        wr, wm = wgrad_ref(x, dz, [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)])
+        plan_w = wgrad_plan(blk.k, blk.cin_pad, blk.cout_pad, st.batch, blk.src.h, blk.src.w, sms)
         r["wgrad"] = wgrad_record(st, blk, got_dw, snap, wr, wm, plan_w)
-        want, mag = T.tapsum(dz, T.conv_taps(w64, mirror=True), blk.src.h, blk.src.w)
-        n = blk.k * blk.k * T.rup(blk.cout, 64) // 16
+        want, mag = tapsum(dz, conv_taps(w64, mirror=True), blk.src.h, blk.src.w)
+        n = blk.k * blk.k * rup(blk.cout, 64) // 16
         t = 0.0
         if blk.gsrc_acc:
             want = want + prior.double()
             t = U * (mag + prior.double().abs())
-        rd = T.bf16_check(T.vint(blk.gsrc), want, n * 2.0 ** -23 * mag, t)
+        rd = bf16_check(vint(blk.gsrc), want, n * 2.0 ** -23 * mag, t)
         r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
     r["outside_untouched"] = _outside(blk, blk.gsrc.buf, snap["gbuf"])
 
 
 # ---------------------------------------------------------------------------------------------------------------
-def run_step(batch, h, w, seed):
-    dev = torch.device("cuda")
-    t0 = time.time()
-    model = init_darknet_weights(m_model(), seed=seed).to(dev).train()
-    st = T.Step()
-    st.batch, st.h, st.w = batch, h, w
-    st.model = model
-    st.x = torch.rand(batch, 3, h, w, generator=torch.Generator().manual_seed(seed + 1)).to(dev)
-    model(st.x)                          # builds the plan; the checked step is the next one
-    plan = model._tplan
-    st.plan = plan
-    st.keep_fwd, st.keep_bwd, st.stash = set(), set(), {}
-    st.owners, st.fwd_lin = {}, {}
-    st.owner_of_users = {b.owner for b in plan.blocks if b.owner is not None}
-    st.rm0, st.rv0, nbt0 = {}, {}, {}
-    for i, m in enumerate(model.module_list):
-        if hasattr(m, "BatchNorm2d"):
-            st.rm0[i] = m.BatchNorm2d.running_mean.clone()
-            st.rv0[i] = m.BatchNorm2d.running_var.clone()
-            nbt0[i] = int(m.BatchNorm2d.num_batches_tracked)
-    orig_f = plan._linear_fwd
-
-    def lin_fwd(blk, s):
-        orig_f(blk, s)
-        try:
-            st.fwd_lin[blk.i] = check_linear_fwd(st, blk)
-        except Exception:
-            st.fwd_lin[blk.i] = {"error": traceback.format_exc()}
-    plan._linear_fwd = lin_fwd
+def _lin_fwd(st, blk):
     try:
-        ps = model(st.x)
-    finally:
-        del plan._linear_fwd
-    torch.cuda.synchronize()
-    assert model._tplan is plan
-    # BN running statistics move only for the blocks whose BatchNorm runs (never a weight_from block's)
-    st.nbt_ok = all(int(model.module_list[i].BatchNorm2d.num_batches_tracked) == nbt0[i] + (b.owner is None and b.has_bn)
-                    for b in plan.blocks for i in [b.i] if i in nbt0)
-    T.forward_checks(st)
+        st.fwd_lin[blk.i] = check_linear_fwd(st, blk)
+    except Exception:
+        st.fwd_lin[blk.i] = {"error": traceback.format_exc()}
+
+
+def _prepare(st):
+    """the weight_from heads' forward checks, and the owners whose dW the weight_from blocks add into"""
     fwd_heads(st)
-    st.fwd.update(st.fwd_lin)
-    gen = torch.Generator().manual_seed(seed + 2)
-    gs = [torch.randn(p.shape, generator=gen).to(dev) for p in ps]
-    st.g_nhwc = {}
-    for blk, g in zip(plan.heads, gs):
-        b_, na, ny, nx, no = g.shape
-        st.g_nhwc[blk.i] = g.permute(0, 2, 3, 1, 4).reshape(b_, ny, nx, na * no)
-    loss = sum((p * g).sum() for p, g in zip(ps, gs))
-    st.bwd = {}
-    orig = plan._backward_block
+    st.owner_of_users = {b.owner for b in st.plan.blocks if b.owner is not None}
 
-    def wrapped(blk):
-        st.bwd[blk.i] = check_bwd(st, blk, orig)
-    plan._backward_block = wrapped
-    try:
-        loss.backward()
-    finally:
-        del plan._backward_block
-    torch.cuda.synchronize()
+
+def m_step(batch, h, w, seed):
+    """the checked step (after the warm-up step that builds the plan whose _linear_fwd is wrapped)"""
+    dev = torch.device("cuda")
+    model = init_darknet_weights(m_model(), seed=seed).to(dev).train()
+    st = Step(model, torch.rand(batch, 3, h, w, generator=torch.Generator().manual_seed(seed + 1)).to(dev))
+    st.owners, st.fwd_lin = {}, {}
+    run_step(st, seed + 2, prepare=_prepare, linear_fwd=_lin_fwd, block_check=check_bwd, gw_bits=False)
+    st.fwd.update(st.fwd_lin)
     after_backward(st)
-    st.t_total = time.time() - t0
     return st
 
 
 def after_backward(st):
-    """head bias sums, the gathers into .grad, the owners' totals"""
+    """the gathers into .grad, the owners' totals"""
     plan, model = st.plan, st.model
-    for blk in plan.blocks:
-        r = st.bwd.setdefault(blk.i, {})
-        if blk.is_head and blk.owner is None:
-            g = st.g_nhwc[blk.i].double()
-            gb = plan.garena[blk.gb_off:blk.gb_off + blk.cout]
-            r["dbias"] = T.sum_check(gb, g.sum((0, 1, 2)), T.head_bias_chain(st.batch, blk.oh, blk.ow),
-                                     g.abs().sum((0, 1, 2)))
     # every parameter's .grad is its arena slot bit for bit (dW reshaped for the conv weights); weight_from blocks' own
     # modules get none
     st.grad_bits, st.grad_none = [], []
@@ -500,22 +385,9 @@ def _print_table(st, tag):
 @pytest.fixture(scope="module", params=SHAPES, ids=["b2_416", "b3_352x608", "b2_128x160"])
 def step(request):
     batch, h, w = request.param
-    st = run_step(batch, h, w, 31)
+    st = m_step(batch, h, w, 31)
     _print_table(st, "m%dx%dx%d" % (batch, h, w))
     return st
-
-
-def _bad(d, skip=("dy_mode", "near_zero_u", "n_elems", "wgrad_rw", "mean_over_std")):
-    out = []
-    for i, r in d.items():
-        for k, v in r.items():
-            if k == "error":
-                out.append((i, k, v[-600:]))
-            elif k in skip:
-                continue
-            elif (isinstance(v, bool) and not v) or (isinstance(v, float) and not v <= 1.0):
-                out.append((i, k, v))
-    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -558,13 +430,13 @@ def test_forward_kernels_vs_float64(step):
     assert step.im2col == dict(bits=True, pad_zero=True, halo=True), step.im2col
     bad = [p[:2] for p in step.packs if not p[2]]
     assert not bad, bad
-    bad = _bad(step.fwd)
+    bad = bad_entries(step.fwd)
     assert not bad, bad
     assert step.fwd[109]["fixed_stats"]
 
 
 def test_backward_kernels_vs_float64(step):
-    bad = _bad(step.bwd)
+    bad = bad_entries(step.bwd)
     assert not bad, bad
     for i, r in step.bwd.items():
         if "near_zero_u" in r:
@@ -612,23 +484,23 @@ def test_bounds_reject_plausible_bugs(step):
     out["ragged phase edge dropped from wgrad"] = float(((inc - lost).abs() / bound).max())
     # (dh, dw) swapped in the dgrad's index map
     want, mag = dil_conv(d["dz"], d["w64"], dh, dw, adjoint=True)
-    assert T.passed(T.check_z(d["v"], want, mag, d["n"]))
+    assert passed(check_z(d["v"], want, mag, d["n"]))
     want_sw, mag_sw = dil_conv(d["dz"], d["w64"], dw, dh, adjoint=True)
-    out["dgrad with (dh, dw) swapped"] = T.check_z(d["v"], want_sw, mag_sw, d["n"])["max"]
+    out["dgrad with (dh, dw) swapped"] = check_z(d["v"], want_sw, mag_sw, d["n"])["max"]
     # the merge with accumulate = 1, run on the step's own phase gradient into a copy of the source gradient buffer
     # (which holds the step's final gradient there): correct against bf16(prior + merge), fails against an overwrite
-    lib = _lib()
+    L = ryolo_lib()
     g = d["gsrc"]
     buf = d["prior_buf"].clone()
     buf[:, 1:-1, 1:-1, g.ch_off:g.ch_off + g.c] = torch.randn(buf.shape[0], buf.shape[1] - 2, buf.shape[2] - 2, g.c,
                                                               device=buf.device, generator=torch.Generator(
                                                                   device=buf.device).manual_seed(9)).to(BF16)
-    prior = T.interior(buf, g.ch_off, g.c).clone()
-    lib.check(lib.lib.ryolo_dilate_merge(lib.ptr(d["dxp"]), d["dxp"].shape[-1], d["x"].shape[0], h, w, g.c, dh, dw, None, 0,
-                                         1, ctypes.c_void_p(buf.data_ptr() + 2 * g.ch_off), buf.shape[-1],
-                                         lib.stream_ptr(buf.device)), "dilate_merge")
+    prior = interior(buf, g.ch_off, g.c).clone()
+    L.check(L.lib.ryolo_dilate_merge(L.ptr(d["dxp"]), d["dxp"].shape[-1], d["x"].shape[0], h, w, g.c, dh, dw, None, 0,
+                                     1, ctypes.c_void_p(buf.data_ptr() + 2 * g.ch_off), buf.shape[-1],
+                                     L.stream_ptr(buf.device)), "dilate_merge")
     torch.cuda.synchronize()
-    got = T.interior(buf, g.ch_off, g.c)
+    got = interior(buf, g.ch_off, g.c)
     assert merge_check(got, prior, d["v"], True)
     out["merge overwrites instead of accumulating"] = 2.0 if not merge_check(got, prior, d["v"], False) else 0.0
     # one branch use missing from an owner's gradient
@@ -642,16 +514,16 @@ def test_bounds_reject_plausible_bugs(step):
     up_odd = torch.zeros_like(zi["up"])
     n_odd = up_odd[:, 1::2, 1::2].shape
     up_odd[:, 1::2, 1::2] = zi["dz"][:, :n_odd[1], :n_odd[2]]
-    out["zero-insert at the odd pixels"] = 0.0 if T.bitwise(zi["up"], up_odd) else 2.0
+    out["zero-insert at the odd pixels"] = 0.0 if bitwise(zi["up"], up_odd) else 2.0
     # block 109: the PReLU kink taken at z instead of z + bias
     k = s["b109"]
     args = (k["z"], k["dy"], k["dz"], k["sums"], k["bias"], k["slope"], k["chain"])
-    assert T.passed(bias_act_bwd_check(*args))
+    assert passed(bias_act_bwd_check(*args))
     out["block 109 kink at z"] = bias_act_bwd_check(*args, kink_at_z=True)["max"]
     # a bias added to a weight_from head
     hd = s["head"]
-    assert T.f32_check(hd["got"], hd["want"], hd["e"])["max"] <= 1.0
-    out["bias on a weight_from head"] = T.f32_check(hd["got"], hd["want"] + hd["bias"], hd["e"])["max"]
+    assert f32_check(hd["got"], hd["want"], hd["e"])["max"] <= 1.0
+    out["bias on a weight_from head"] = f32_check(hd["got"], hd["want"] + hd["bias"], hd["e"])["max"]
     print("\n[bite] " + ", ".join("%s %.3g" % kv for kv in out.items()))
     bad = {kk: v for kk, v in out.items() if not v > 1.0}
     assert not bad, bad

@@ -14,8 +14,8 @@ import numpy as np
 import pytest
 import torch
 
+from builders import cosine, golden_text, m_golden, m_model
 from helpers import init_darknet_weights
-from test_dilated_cfg import _golden, _text, m_model
 
 pytestmark = pytest.mark.gpu
 
@@ -30,10 +30,6 @@ TARGETS = [[0, 0, 0.30, 0.40, 57.5 / 160, 13.8 / 128, 0.5],
 def _sample_idx(numel, n, seed):
     g = torch.Generator().manual_seed(seed)
     return torch.randint(0, numel, (n,), generator=g)
-
-
-def _cos(a, b):
-    return float((a * b).sum() / (np.linalg.norm(a) * np.linalg.norm(b) + 1e-30))
 
 
 def _step(arc, seed_w, seed_x):
@@ -51,8 +47,8 @@ def _step(arc, seed_w, seed_x):
 
 @pytest.mark.parametrize("arc", ["default", "Fdefault"])
 def test_training_step_vs_reference_autograd(arc):
-    g = _golden()
-    sd = json.loads(_text(g, "seeds"))
+    g = m_golden()
+    sd = json.loads(golden_text(g, "seeds"))
     m, ps, loss, items = _step(arc, sd["train_w"], sd["train_x"])
     assert len(ps) == 16
     for k in (0, 4, 12):
@@ -77,7 +73,7 @@ def test_training_step_vs_reference_autograd(arc):
         want = g[arc + "_samples"][j].astype(np.float64)
         gflat = prm.grad.reshape(-1)
         got = gflat[_sample_idx(gflat.numel(), len(want), 1000 + j).cuda()].double().cpu().numpy()
-        cos[name] = _cos(got, want)
+        cos[name] = cosine(got, want)
         ratio[name] = float(gflat.double().norm()) / (float(g[arc + "_norms"][j]) + 1e-30)
     big = [n for n in cos if n.endswith("Conv2d.weight")]
     cb, rb = np.array([cos[n] for n in big]), np.array([ratio[n] for n in big])

@@ -6,15 +6,14 @@ sets upstream of every tensor, not from the schedule's own walk.  The arena rang
 exactly its trainable parameters."""
 import os
 import random
-import socket
 
 import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from test_dilated_cfg import m_model
-from test_graph_walk import _model
+from builders import free_port, graph_model, m_model
+
 
 CPU = torch.device("cpu")
 CFGS = ["cfg/yolov3.cfg", "cfg/HRSC+/yolov3_512_se.cfg", "cfg/yolov3-m.cfg"]
@@ -22,7 +21,7 @@ CFGS = ["cfg/yolov3.cfg", "cfg/HRSC+/yolov3_512_se.cfg", "cfg/yolov3-m.cfg"]
 
 def _plan(name):
     from rotate_yolov3_b200.train_path import TrainPlan
-    m, h, w = (m_model(), 64, 64) if name.endswith("yolov3-m.cfg") else _model(name)
+    m, h, w = (m_model(), 64, 64) if name.endswith("yolov3-m.cfg") else graph_model(name)
     return m, TrainPlan(m, 1, h, w, CPU)
 
 
@@ -163,20 +162,12 @@ def test_random_masks(name):
         _check(plan, plan._schedule(mask))
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    return port
-
-
 def _bucket_worker(rank, world, port):
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from rotate_yolov3_b200.train_path import TrainPlan
-    m, h, w = _model("cfg/yolov3.cfg")
+    m, h, w = graph_model("cfg/yolov3.cfg")
     m._ddp = {"bucket_bytes": 1 << 20, "group": None, "reserved_sms": 0}
     plan = TrainPlan(m, 1, h, w, CPU)
     full = plan.sched
@@ -206,4 +197,4 @@ def _bucket_worker(rank, world, port):
 
 
 def test_buckets_of_a_mask_two_rank_gloo():
-    mp.spawn(_bucket_worker, args=(2, _free_port()), nprocs=2, join=True)
+    mp.spawn(_bucket_worker, args=(2, free_port()), nprocs=2, join=True)

@@ -5,12 +5,12 @@ frozen backbone (blocks >= 75 train) of train.py:120-135 / :215-220, one SE's fc
 BatchNorm momentum is 0, so that every forward is the same and the running statistics do not move."""
 import math
 import os
-import socket
 
 import pytest
 import torch
 
 import helpers
+from builders import free_port, transfer_mask
 from helpers import GOLDEN, SMALL_ANCHORS
 
 pytestmark = pytest.mark.gpu
@@ -45,18 +45,13 @@ def se_model():
 
 
 def m_graph():
-    from test_dilated_cfg import m_model
+    from builders import m_model
     return _prep(m_model(), 7)
 
 
 def prebias(m):
     nf = int(m.module_defs[m.yolo_layers[0] - 1]["filters"])
     return [p.numel() == nf for p in m.parameters()]          # train.py:129-130
-
-
-def transfer(m):
-    nf = int(m.module_defs[m.yolo_layers[0] - 1]["filters"])
-    return [p.shape[0] == nf for p in m.parameters()]         # train.py:131-132
 
 
 def cutoff75(m):
@@ -115,7 +110,7 @@ def _check_mask(m, x, mask_fn):
 def test_masked_step_equals_the_full_step(mask):
     m = yolov3()
     x = torch.rand(2, 3, 128, 160, generator=torch.Generator().manual_seed(1)).cuda()
-    sch = _check_mask(m, x, {"prebias": prebias, "transfer": transfer, "cutoff75": cutoff75}[mask])
+    sch = _check_mask(m, x, {"prebias": prebias, "transfer": transfer_mask, "cutoff75": cutoff75}[mask])
     kinds = {k for k, _, _ in sch.ops(m._tplan)}
     assert kinds == {"prebias": {"head_bias"}, "transfer": {"head", "wgrad"},
                      "cutoff75": {"head", "bnact", "wgrad", "dgrad"}}[mask]
@@ -237,14 +232,6 @@ def test_reference_prebias_and_transfer_loops(tmp_path):
             assert torch.equal(p.detach(), before[n]) != p.requires_grad, n
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _ddp_worker(rank, world, port, q):
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
@@ -257,7 +244,7 @@ def _ddp_worker(rank, world, port, q):
     def make():
         m = pkg.Darknet(helpers.mini_cfg(64, 48), {"context_factor": 1.0})
         m = _prep(m, 5)
-        _set(m, transfer(m))
+        _set(m, transfer_mask(m))
         return m
     x = torch.rand(4, 3, 48, 64, generator=torch.Generator().manual_seed(100 + rank)).cuda()
     m = make()
@@ -283,7 +270,7 @@ def test_two_rank_nccl_transfer_mask():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_ddp_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()

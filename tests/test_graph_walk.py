@@ -1,61 +1,19 @@
 """The graph walk the eval, training and parity-precision plans share (rotate-yolov3_b200/graph.py), checked on the CPU
 against what the module tree states on its own: conv input channels, the blocks a conv's epilogue absorbs, concat
 placement and the heads; and the refusals of each plan."""
-import contextlib
-import os
-
 import pytest
 import torch
 
-from helpers import GOLDEN, SMALL_ANCHORS, mini_cfg
+from builders import REF_CFGS, graph_model
+from helpers import SMALL_ANCHORS, cfg_conv
 
-REF = os.path.join(GOLDEN, "reference_cfg")
-REF_CFGS = ["cfg/yolov3.cfg", "cfg/HRSC+/yolov3_512.cfg", "cfg/HRSC+/yolov3_512_ma.cfg", "cfg/HRSC+/yolov3_512_se.cfg",
-            "cfg/ICDAR/yolov3_608.cfg", "cfg/ICDAR/yolov3_608_se.cfg"]
 CPU = torch.device("cpu")
-
-
-def _conv(f, k, s=1, bn=1, act="leaky"):
-    return "[convolutional]\n%sfilters=%d\nsize=%d\nstride=%d\npad=1\nactivation=%s\n\n" % (
-        "batch_normalize=1\n" if bn else "", f, k, s, act)
-
-
-def odd_grid_cfg():
-    """at 36 x 36 the last 3x3 / stride-2 conv reads a 9 x 9 grid: no space-to-depth copy exists for it"""
-    s = "[net]\nwidth=36\nheight=36\nchannels=3\n\n"
-    s += _conv(32, 3) + _conv(64, 3, 2) + _conv(32, 1) + _conv(64, 3) + "[shortcut]\nfrom=-3\nactivation=linear\n\n"
-    s += _conv(64, 3, 2) + _conv(128, 3, 2) + _conv(64, 1) + _conv(128, 3) + "[shortcut]\nfrom=-3\nactivation=linear\n\n"
-    s += _conv(21, 1, bn=0, act="linear") + "[yolo]\nmask = 0-2\nanchors = %s\nclasses=1\nnum=6\n\n" % SMALL_ANCHORS
-    return s
-
-
-@contextlib.contextmanager
-def _cwd(path):
-    old = os.getcwd()
-    os.chdir(path)
-    try:
-        yield
-    finally:
-        os.chdir(old)
-
-
-def _model(name):
-    """(Darknet, height, width)"""
-    import rotate_yolov3_b200 as pkg
-    from rotate_yolov3_b200 import cfgs
-    if name in REF_CFGS:
-        with _cwd(REF):                    # the SE cfgs name their anchor files relative to the reference root
-            return pkg.Darknet(name, {"context_factor": 1.0}, arc="default"), 64, 64
-    cfg, h, w = {"yolov3": (cfgs.yolov3_cfg(), 64, 64), "mini": (mini_cfg(64, 48), 48, 64),
-                 "micro": (os.path.join(GOLDEN, "micro.cfg"), 32, 32), "odd": (odd_grid_cfg(), 36, 36),
-                 "tiny_trunk": (cfgs.yolov3_tiny_trunk_cfg(416, 416), 416, 416)}[name]
-    return pkg.Darknet(cfg, {"context_factor": 1.0}, arc="default"), h, w
 
 
 @pytest.mark.parametrize("name", ["yolov3", "mini", "micro", "odd", "tiny_trunk"] + REF_CFGS)
 def test_walk_matches_the_module_tree(name):
     from rotate_yolov3_b200 import graph as G
-    m, h, w = _model(name)
+    m, h, w = graph_model(name)
     defs = m.module_defs
     g = G.Graph(m, h, w, ("se", "maxpool"), "block type %r")
     convs = [i for i, d in enumerate(defs) if d["type"] == "convolutional"]
@@ -95,7 +53,7 @@ def test_walk_matches_the_module_tree(name):
 def test_odd_grid_stride2_runs_without_space_to_depth():
     from rotate_yolov3_b200.parity_path import ParityPlan
     from rotate_yolov3_b200.train_path import TrainPlan
-    m, h, w = _model("odd")
+    m, h, w = graph_model("odd")
     plan = TrainPlan(m, 1, h, w, CPU)
     odd = [b for b in plan.blocks if b.stride == 2 and b.src.h % 2]
     assert [b.i for b in odd] == [6] and not odd[0].s2d and odd[0].dz_up is not None
@@ -109,16 +67,16 @@ def test_plans_refuse_what_they_cannot_run():
     from rotate_yolov3_b200 import graph as G
     from rotate_yolov3_b200.parity_path import ParityPlan
     from rotate_yolov3_b200.train_path import TrainPlan
-    se, h, w = _model("cfg/HRSC+/yolov3_512_se.cfg")
+    se, h, w = graph_model("cfg/HRSC+/yolov3_512_se.cfg")
     for training in (True, False):
         with pytest.raises(NotImplementedError, match="bf16"):
             ParityPlan(se, 1, h, w, CPU, training)
-    tiny, h, w = _model("tiny_trunk")
+    tiny, h, w = graph_model("tiny_trunk")
     with pytest.raises(NotImplementedError, match="maxpool"):
         TrainPlan(tiny, 1, h, w, CPU)
     import rotate_yolov3_b200 as pkg
-    cfg = "[net]\nwidth=32\nheight=32\nchannels=3\n\n" + _conv(32, 3) + _conv(32, 1) + "[route]\nlayers = -2\n\n"
-    cfg += "[shortcut]\nfrom=-2\nactivation=linear\n\n" + _conv(21, 1, bn=0, act="linear")
+    cfg = "[net]\nwidth=32\nheight=32\nchannels=3\n\n" + cfg_conv(32, 3) + cfg_conv(32, 1) + "[route]\nlayers = -2\n\n"
+    cfg += "[shortcut]\nfrom=-2\nactivation=linear\n\n" + cfg_conv(21, 1, bn=0, act="linear")
     cfg += "[yolo]\nmask = 0-2\nanchors = %s\nclasses=1\nnum=6\n\n" % SMALL_ANCHORS
     m = pkg.Darknet(cfg, {"context_factor": 1.0}, arc="default")
     with pytest.raises(NotImplementedError, match="shortcut at block 3 does not follow a convolution"):

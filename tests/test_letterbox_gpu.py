@@ -2,14 +2,15 @@
 LoadImages normalisation (tests/golden/letterbox_golden.npz): the fp32 and fp16 network input is bit for bit the
 reference's for every case; border pixels, mixed-size batches, CUDA sources, CUDA-graph replay, scale_coords,
 letterbox_labels, malformed input, and a Darknet forward on the device input against one on the reference input."""
-import hashlib
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from builders import tensor_sha
 from helpers import GOLDEN
+from letterbox_cases import letterbox_case, net_input, source
 
 pytestmark = pytest.mark.gpu
 
@@ -17,30 +18,8 @@ GOLD = os.path.join(GOLDEN, "letterbox_golden.npz")
 DEV = torch.device("cuda", 0)
 
 
-def source(seed, h, w):
-    return np.random.default_rng(seed).integers(0, 256, (h, w, 3), dtype=np.uint8)
-
-
 def _gold():
     return np.load(GOLD)
-
-
-def _case(g, name):
-    k = "case_%s_" % name
-    ns = g[k + "new_shape"]
-    new_shape = int(ns[0]) if str(g[k + "mode"]) == "square" else (int(ns[0]), int(ns[1]))
-    h, w = (int(v) for v in g[k + "src"])
-    return source(int(g[k + "seed"]), h, w), new_shape, str(g[k + "mode"]), k
-
-
-def _sha(t):
-    return hashlib.sha256(t.cpu().contiguous().numpy().tobytes()).hexdigest()
-
-
-def _ref_input(lb, dtype):
-    x = np.ascontiguousarray(lb[:, :, ::-1].transpose(2, 0, 1), dtype=dtype)
-    x /= 255.0
-    return x
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
@@ -49,16 +28,16 @@ def test_every_case_bitwise_equals_reference(dtype):
     g = _gold()
     key = "sha32" if dtype == torch.float32 else "sha16"
     for name in g["cases"]:
-        img, new_shape, mode, k = _case(g, str(name))
+        img, new_shape, mode, k = letterbox_case(g, str(name))
         x, meta = letterbox([img], new_shape, mode=mode, dtype=dtype, device=DEV)
         torch.cuda.synchronize()
         assert x.dtype == dtype and tuple(x.shape[2:]) == tuple(int(v) for v in g[k + "out_hw"])
         assert meta.dtype == torch.float64 and meta[0].tolist() == g[k + "meta"].tolist(), name
         if k + "lb" in g:                          # where the reference image is stored: count differing pixels
-            want = torch.from_numpy(_ref_input(g[k + "lb"], np.float32 if dtype == torch.float32 else np.float16))
+            want = torch.from_numpy(net_input(g[k + "lb"], np.float32 if dtype == torch.float32 else np.float16))
             ndiff = int((x[0].cpu() != want).sum())
             assert ndiff == 0, "%s: %d of %d values differ from the reference input" % (name, ndiff, want.numel())
-        assert _sha(x[0]) == str(g[k + key]), name
+        assert tensor_sha(x[0]) == str(g[k + key]), name
 
 
 def test_border_is_exactly_128_over_255():
@@ -76,7 +55,7 @@ def test_mixed_batch_equals_single_calls_and_cuda_sources():
     from rotate_yolov3_b200 import letterbox
     g = _gold()
     names = ["land_1024x768", "hd_1920x1080", "int2x2", "upscale", "no_resize", "one_px_wide", "half_pad", "portrait"]
-    imgs = [_case(g, n)[0] for n in names]
+    imgs = [letterbox_case(g, n)[0] for n in names]
     batch, meta = letterbox(imgs, 608)
     for b, img in enumerate(imgs):
         one, m1 = letterbox([img], 608)
@@ -181,9 +160,9 @@ def test_darknet_io_on_device_input_equals_reference_input():
     import helpers
     import rotate_yolov3_b200 as pkg
     g = _gold()
-    img, new_shape, mode, k = _case(g, "e2e")            # 97 x 133 -> 128 x 128
+    img, new_shape, mode, k = letterbox_case(g, "e2e")            # 97 x 133 -> 128 x 128
     x, _ = pkg.letterbox([img], new_shape)
-    ref = torch.from_numpy(_ref_input(g[k + "lb"], np.float32)).unsqueeze(0).to(DEV)
+    ref = torch.from_numpy(net_input(g[k + "lb"], np.float32)).unsqueeze(0).to(DEV)
     m = pkg.Darknet(helpers.mini_cfg(128, 128), {"context_factor": 1.0}, arc="default")
     helpers.init_darknet_weights(m, seed=77)
     m = m.to(DEV).eval()

@@ -2,30 +2,13 @@
 this container (tests/golden/make_golden.py section 9): loss value, its four components and the gradient wrt every
 head tensor.  Pure PyTorch consumer -> runs on CPU."""
 import os
-import types
 
 import numpy as np
 import pytest
 import torch
 
-from helpers import GOLDEN, SMALL_ANCHORS, mini_cfg
-
-
-def _fake_model(ps, hyp):
-    """just what compute_loss reads from the model: yolo_layers, module_list[i].{ng, anchor_vec}, nc, hyp, arc"""
-    import math
-    from rotate_yolov3_b200.parse_config import cfg2anchors
-    anchors = cfg2anchors(SMALL_ANCHORS)
-    m = types.SimpleNamespace(yolo_layers=[0, 1, 2], nc=1, hyp=hyp, arc="default")
-    layers = []
-    for p, (lo, hi) in zip(ps, ((4, 5), (2, 3), (0, 1))):
-        ny, nx = p.shape[2], p.shape[3]
-        stride = max(128, 160) / max(nx, ny)
-        av = torch.tensor(anchors[lo:hi + 1], dtype=torch.float32)
-        av[:, :2] /= stride
-        layers.append(types.SimpleNamespace(ng=torch.tensor([float(nx), float(ny)]), anchor_vec=av))
-    m.module_list = layers
-    return m
+from builders import fake_loss_model
+from helpers import GOLDEN
 
 
 def test_compute_loss_vs_reference():
@@ -33,7 +16,7 @@ def test_compute_loss_vs_reference():
     g = np.load(os.path.join(GOLDEN, "loss_golden.npz"))
     hyp = {str(k): float(v) for k, v in zip(g["hyp_keys"], g["hyp_vals"])}
     ps = [torch.from_numpy(g["p%d" % k]).clone().requires_grad_(True) for k in range(3)]
-    m = _fake_model(ps, hyp)
+    m = fake_loss_model(ps, hyp)
     loss, items = compute_loss(ps, torch.from_numpy(g["targets"]).clone(), m, hyp)
     assert np.allclose(loss.detach().numpy(), g["loss"], rtol=1e-5, atol=1e-6)
     assert np.allclose(items.numpy(), g["items"], rtol=1e-5, atol=1e-6)
@@ -48,7 +31,7 @@ def test_orphan_ground_truth_gets_an_anchor():
     g = np.load(os.path.join(GOLDEN, "loss_golden.npz"))
     hyp = {str(k): float(v) for k, v in zip(g["hyp_keys"], g["hyp_vals"])}
     ps = [torch.from_numpy(g["p%d" % k]) for k in range(3)]
-    m = _fake_model(ps, hyp)
+    m = fake_loss_model(ps, hyp)
     t = torch.tensor([[0, 0, 0.5, 0.5, 0.02, 0.02, 0.3], [1, 0, 0.2, 0.7, 0.42, 0.105, 0.0]])   # first: far too small
     tcls, tbox, indices, av = build_targets(m, t.clone(), hyp)
     n_per_gt = [sum(int((idx[0] == img).sum()) for idx in indices) for img in (0, 1)]
@@ -81,7 +64,7 @@ def test_masked_loss_equals_indexed_loss():
         res = []
         for masked in (True, False):
             ps = [b.clone().requires_grad_(True) for b in base]
-            m = _fake_model(ps, hyp)
+            m = fake_loss_model(ps, hyp)
             m.nc = nc
             if nc > 1:
                 # the reference's multi-class branch feeds BCE a [nb, nc+1] input and a [nb, nc] target
@@ -115,7 +98,7 @@ def test_masked_assignment_selects_the_rows_build_targets_keeps():
     g = np.load(os.path.join(GOLDEN, "loss_golden.npz"))
     hyp = {str(k): float(v) for k, v in zip(g["hyp_keys"], g["hyp_vals"])}
     ps = [torch.from_numpy(g["p%d" % k]) for k in range(3)]
-    m = _fake_model(ps, hyp)
+    m = fake_loss_model(ps, hyp)
     gen = torch.Generator().manual_seed(11)
     for nt in (1, 5, 64):
         t = torch.rand(nt, 7, generator=gen)
@@ -145,7 +128,7 @@ def test_loss_without_targets_and_with_poisoned_unselected_rows():
     g = np.load(os.path.join(GOLDEN, "loss_golden.npz"))
     hyp = {str(k): float(v) for k, v in zip(g["hyp_keys"], g["hyp_vals"])}
     ps = [torch.from_numpy(g["p%d" % k]).clone().requires_grad_(True) for k in range(3)]
-    m = _fake_model(ps, hyp)
+    m = fake_loss_model(ps, hyp)
     loss, items = compute_loss(ps, torch.zeros(0, 7), m, hyp)
     assert float(items[1]) == 0 and float(items[2]) == 0 and torch.isfinite(loss).all()
     loss.backward()
@@ -189,7 +172,7 @@ def test_stacked_target_assignment_equals_the_per_layer_form():
             t[:, 4:6] = t[:, 4:6] * 0.6 + 0.005
             t[:, 6] = (t[:, 6] - 0.5) * 3.0
             t[nt // 2] = t[0]
-            m = _fake_model(base, hyp)
+            m = fake_loss_model(base, hyp)
             m.nc = nc
             rows = L._targets_masked(m, t.clone(), hyp)
             st = L._targets_masked_stacked(m, t.clone(), hyp)

@@ -8,23 +8,18 @@ objectness kernels (csrc/loss.cu, ryolo_obj_focal_fwd / _bwd) and the focal matc
   * the Darknet-53 graph at 160 x 128 in parity precision trained with the Fdefault loss against the reference (case d);
   * a bf16 training step with Fdefault under CUDA graphs is bitwise repeatable."""
 import ctypes
-import os
 
 import numpy as np
 import pytest
 import torch
 
 import focal_cases as FC
-from helpers import GOLDEN, SMALL_ANCHORS, init_darknet_weights
-from test_loss import _fake_model
-from test_loss_focal import _cases
+from builders import (STEP_HYP, assert_same, fake_loss_model, repeat, report_and_check_gradients, small_train_model,
+                      step_targets)
+from helpers import SMALL_ANCHORS, init_darknet_weights
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
-
-
-def _golden():
-    return np.load(os.path.join(GOLDEN, "loss_focal_golden.npz"), allow_pickle=True)
 
 
 def _nchw_leaf(t):
@@ -35,7 +30,7 @@ def _nchw_leaf(t):
 
 
 def _fmodel(heads, hyp, nc=1):
-    m = _fake_model(heads, hyp)
+    m = fake_loss_model(heads, hyp)
     m.arc, m.nc = "Fdefault", nc
     return m
 
@@ -44,8 +39,8 @@ def _fmodel(heads, hyp, nc=1):
 @pytest.mark.parametrize("case", range(6))
 def test_fused_focal_loss_vs_reference_golden(case, layout):
     from rotate_yolov3_b200.loss import compute_loss
-    g = _golden()
-    tag, heads, tg, hyp = _cases()[case]
+    g = FC.golden()
+    tag, heads, tg, hyp = FC.cases()[case]
     leaves, ps = [], []
     for h in heads:
         if layout == "contiguous":
@@ -206,7 +201,6 @@ def test_focal_kernels_vs_float64_at_608(ny, gamma):
 
 @pytest.mark.parametrize("ny", [19, 38, 76])
 def test_focal_kernels_repeatable_and_gamma0_is_bce(ny):
-    from test_determinism_gpu import repeat
     x, tobj = _head608(ny, 200 + ny)
     scale = 20.35 / (B64 * NA * ny * ny)
     s, g = repeat(lambda: _kernel_call(x, tobj, 1.0, 0.5, scale))
@@ -233,8 +227,7 @@ def test_darknet53_parity_trained_with_fdefault_vs_reference():
     import rotate_yolov3_b200 as pkg
     from rotate_yolov3_b200 import cfgs
     from rotate_yolov3_b200.loss import compute_loss
-    from test_parity_gpu import _report_and_check_gradients
-    g = _golden()
+    g = FC.golden()
     x, tg, hyp = FC.darknet_case()
     m = pkg.Darknet(cfgs.yolov3_cfg(width=160, height=128, classes=1, anchors=SMALL_ANCHORS, n_anchors=6),
                     {"context_factor": 1.0}, arc="Fdefault", precision="parity")
@@ -260,14 +253,12 @@ def test_darknet53_parity_trained_with_fdefault_vs_reference():
             continue
         rows.append((int(name.split(".")[1]), name, float(np.abs(got - smp).max()) / scale,
                      abs(float(gr.norm()) - float(norm)) / float(norm)))
-    _report_and_check_gradients("darknet-53 160x128 trained with Fdefault", rows)
+    report_and_check_gradients("darknet-53 160x128 trained with Fdefault", rows)
 
 
 def test_bf16_fdefault_training_step_with_cuda_graphs_is_bitwise_repeatable():
-    from test_determinism_gpu import HYP, _same, _targets
-    from test_train_gpu import _model
     from rotate_yolov3_b200.loss import compute_loss
-    hyp = dict(HYP, fl_gamma=0.5)
+    hyp = dict(STEP_HYP, fl_gamma=0.5)
 
     def setup(m):
         m.nc, m.hyp, m.arc = 1, hyp, "Fdefault"
@@ -284,18 +275,18 @@ def test_bf16_fdefault_training_step_with_cuda_graphs_is_bitwise_repeatable():
             out["grad:" + n] = p.grad.clone()
         torch.cuda.synchronize()
         return out
-    m = setup(_model())
+    m = setup(small_train_model())
     sd0 = {k: v.clone() for k, v in m.state_dict().items()}
     x = torch.rand(2, 3, 128, 160, generator=torch.Generator().manual_seed(17)).cuda()
-    t = _targets()
+    t = step_targets()
     ref = step(m, x, t)
     assert float(ref["items"][2]) > 0 and all(torch.isfinite(v).all() for v in ref.values())
     m.load_state_dict(sd0)
-    _same(ref, step(m, x, t), "rerun")
-    m3 = setup(_model())
+    assert_same(ref, step(m, x, t), "rerun")
+    m3 = setup(small_train_model())
     m3.load_state_dict(sd0)
     m3.use_cuda_graph = True
-    _same(ref, step(m3, x, t), "graph capture step")
+    assert_same(ref, step(m3, x, t), "graph capture step")
     m3.load_state_dict(sd0)                      # in place: the captured graphs stay valid
-    _same(ref, step(m3, x, t), "graph replay")
+    assert_same(ref, step(m3, x, t), "graph replay")
     assert m3._tplan.replayed_kernels > 0

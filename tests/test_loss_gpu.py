@@ -9,8 +9,8 @@ import numpy as np
 import pytest
 import torch
 
+from builders import fake_loss_model
 from helpers import GOLDEN
-from test_loss import _fake_model
 
 pytestmark = pytest.mark.gpu
 
@@ -44,7 +44,7 @@ def test_fused_loss_vs_reference_golden(layout):
             base.requires_grad_(True)
             leaves.append(base)
             ps.append(base.view(t.shape[0], t.shape[1], t.shape[4], t.shape[2], t.shape[3]).permute(0, 1, 3, 4, 2))
-    m = _fake_model([torch.from_numpy(g["p%d" % k]) for k in range(3)], hyp)
+    m = fake_loss_model([torch.from_numpy(g["p%d" % k]) for k in range(3)], hyp)
     loss, items = compute_loss(ps, torch.from_numpy(g["targets"]).to(dev), m, hyp)
     assert np.allclose(loss.detach().cpu().numpy(), g["loss"], rtol=1e-5, atol=1e-6)
     assert np.allclose(items.cpu().numpy(), g["items"], rtol=1e-5, atol=1e-6)
@@ -74,7 +74,7 @@ def test_fused_loss_equals_masked_cpu(nc, nt):
         t[:, 4:6] = t[:, 4:6] * 0.6 + 0.005
         t[:, 6] = (t[:, 6] - 0.5) * 3.0
         t[nt // 2] = t[0]
-    m = _fake_model(base, hyp)
+    m = fake_loss_model(base, hyp)
     m.nc = nc
     cpu = [b.clone().requires_grad_(True) for b in base]
     if nt:
@@ -116,7 +116,7 @@ def test_fused_loss_under_no_grad_and_with_detached_heads():
     g, hyp = _golden()
     dev = torch.device("cuda", 0)
     ps = [torch.from_numpy(g["p%d" % k]).to(dev) for k in range(3)]
-    m = _fake_model([torch.from_numpy(g["p%d" % k]) for k in range(3)], hyp)
+    m = fake_loss_model([torch.from_numpy(g["p%d" % k]) for k in range(3)], hyp)
     with torch.no_grad():
         loss, items = compute_loss(ps, torch.from_numpy(g["targets"]).to(dev), m, hyp)
     assert not loss.requires_grad

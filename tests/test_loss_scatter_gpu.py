@@ -18,7 +18,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_determinism_gpu import repeat
+from builders import repeat
 
 pytestmark = pytest.mark.gpu
 

@@ -8,10 +8,10 @@ the head dgrad at K = 1536 / 2048, head_grad_nchw_kernel needs its opt-in shared
 Training step, with the real loss (compute_loss, the fused path) on targets that reach every branch of it: classes
 0, nc - 1 and between, five per image, two rows on one cell (the scatter chains), one target on the right border (its
 rows fall outside every map: the fused path gathers 0 for them and writes nothing; the reference would raise).
-  every launch       test_train_step_f64_gpu's forward_checks and check_block_bwd, unchanged, on the cotangent the loss
-                     produced: conv z, BN statistics, bn_act_fwd / bn_act_bwd, wgrad, dgrad; at the heads fp32 z, the
-                     head cotangent bit for bit as RN-bf16 with its padding channels and halo zero, the bias sums under
-                     head_bias_chain, wgrad_ratio at cout_pad 1536 / 2048, the dgrad at K = 1536 / 2048
+  every launch       checked_step's forward_checks and check_block_bwd (the bounds of test_train_step_f64_gpu), on the
+                     cotangent the loss produced: conv z, BN statistics, bn_act_fwd / bn_act_bwd, wgrad, dgrad; at the
+                     heads fp32 z, the head cotangent bit for bit as RN-bf16 with its padding channels and halo zero,
+                     the bias sums under head_bias_chain, wgrad_ratio at cout_pad 1536 / 2048, the dgrad at K = 1536 / 2048
   loss and cotangent a float64 restatement of _compute_loss_masked (its target assignment, _sparse_terms, _obj_term) on
                      the same fp32 heads, differentiated by float64 autograd; the fp32 assignment equals the float64
                      one.  Bounds, U = 2^-24:
@@ -29,9 +29,9 @@ rows fall outside every map: the fused path gathers 0 for them and writes nothin
                                            U sum M over their n row terms (a worst-case sequential fp32 sum)
   coverage           test_covers_every_launch ties every entry of sched.ops and every forward block to a check.
 Detect forward (eval, CUDA-graph replay) of the same two models and of nc = 23 at batch 1 x 320 x 416 (2088-filter
-heads, which training refuses at plan build): every conv launch with test_detect_forward_f64_gpu's functions, the decode
-(direct path, no = 21 / 28 / 29) within 2^-20 M of test_detect_gpu._decode_ref, and detect_postprocess_classes on the io
-equal bit for bit to the per-image per-class pipeline of test_detect_classes_gpu.  The bound self-test puts five bugs in.
+heads, which training refuses at plan build): every conv launch with checked_step's eval-forward checks, the decode
+(direct path, no = 21 / 28 / 29) within 2^-20 M of f64_refs.decode_ref, and detect_postprocess_classes on the io
+equal bit for bit to the per-image per-class pipeline (check_equals_per_class_pipeline).  The bound self-test puts five bugs in.
 
 Measured on an H100 80GB HBM3 (132 SMs, power limit 700 W, 1980 MHz max SM clock), seeds as below; worst ratio per
 kernel (block), nc = 15 / nc = 22:
@@ -53,15 +53,14 @@ import time
 import pytest
 import torch
 
-import test_detect_forward_f64_gpu as D
-import test_train_step_f64_gpu as T
+from builders import check_equals_per_class_pipeline, pkg
+from checked_step import (Run, Step, check_block_bwd, check_buffers, check_conv, check_first, check_s2d_step, map_plan,
+                          run_step)
+from f64_refs import F64, TINY, U, bad_entries, decode_ref, halo_zero, head_bias_chain, sum_check
 from helpers import init_darknet_weights
-from test_detect_classes_gpu import check_equals_per_class_pipeline
-from test_detect_gpu import _decode_ref
 
 pytestmark = pytest.mark.gpu
 
-U, BF16, F64, TINY = T.U, T.BF16, T.F64, T.TINY
 U64 = 2.0 ** -53
 MODELS = {"nc15": (15, 2, 608, 608), "nc22": (22, 3, 320, 416)}
 NC_EVAL_ONLY = (23, 1, 320, 416)          # 2088-channel heads: eval runs them, training refuses them at plan build
@@ -72,11 +71,6 @@ K_ROW = 16         # fp32 roundings of one matched-row term or its derivative (t
 CONF, NMS_T, CAP = 0.5, 0.5, 2000
 
 
-def _pkg():
-    import rotate_yolov3_b200 as pkg
-    return pkg
-
-
 def _loss():
     from rotate_yolov3_b200 import loss
     return loss
@@ -84,7 +78,7 @@ def _loss():
 
 def make_model(nc, h, w, seed):
     from rotate_yolov3_b200 import cfgs
-    m = _pkg().Darknet(cfgs.yolov3_cfg(width=w, height=h, classes=nc), {"context_factor": 1.0}, arc="default")
+    m = pkg().Darknet(cfgs.yolov3_cfg(width=w, height=h, classes=nc), {"context_factor": 1.0}, arc="default")
     m.hyp, m.nc = HYP, nc                  # train.py sets both before compute_loss
     return init_darknet_weights(m, seed=seed)
 
@@ -239,93 +233,55 @@ def cot_check(got, want, mag, ncell):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-def run_step(name, seed=41):
+def mc_step(name, seed=41):
     nc, batch, h, w = MODELS[name]
     dev = torch.device("cuda")
     t0 = time.time()
     model = make_model(nc, h, w, seed).to(dev).train()
-    st = T.Step()
-    st.batch, st.h, st.w = batch, h, w
-    st.model, st.nc = model, nc
-    st.x = torch.rand(batch, 3, h, w, generator=torch.Generator().manual_seed(seed + 1)).to(dev)
+    st = Step(model, torch.rand(batch, 3, h, w, generator=torch.Generator().manual_seed(seed + 1)).to(dev))
+    st.nc = nc
     st.targets = make_targets(model, nc, batch, h, w, seed + 2)
-    st.rm0, st.rv0 = {}, {}
-    for i, m in enumerate(model.module_list):
-        if hasattr(m, "BatchNorm2d"):
-            st.rm0[i] = m.BatchNorm2d.running_mean.clone()
-            st.rv0[i] = m.BatchNorm2d.running_var.clone()
-    ps = model(st.x)
-    torch.cuda.synchronize()
-    plan = model._tplan
-    st.plan = plan
-    st.keep_fwd, st.keep_bwd, st.stash = set(), set(), {}
-    T.forward_checks(st)
-    # the fused loss on the heads of this forward; the float64 restatement on the same fp32 heads
-    st.p32 = [p.detach().cpu() for p in ps]
-    loss, items = _loss().compute_loss(ps, st.targets.clone().to(dev), model, HYP)
-    st.items = items.cpu().double()
-    p64 = [p.double().requires_grad_(True) for p in st.p32]
-    comps, rows = loss64(p64, st.targets.double(), model, HYP)
-    sum(comps).sum().backward()
-    st.want_items = torch.cat([c.detach() for c in comps])
-    st.g64 = [p.grad for p in p64]
-    st.rows = rows
-    st.mags, st.mag_loss = magnitudes(p64, rows, model)
-    # the fp32 assignment of the fused path equals the float64 one
-    fr = _loss()._targets_masked_stacked(model, st.targets.clone().to(dev), HYP)
-    st.masks_equal = all(torch.equal(fr["mask"][l].cpu(), r["mask"]) for l, r in enumerate(rows))
     st.cot = {}
-    st.bwd = {}
-    orig_hg, orig = plan._head_grads, plan._backward_block
 
-    def head_grads(grads):
+    def loss(st, ps):
+        """the fused loss on the heads of this forward; the float64 restatement on the same fp32 heads"""
+        st.p32 = [p.detach().cpu() for p in ps]
+        loss, items = _loss().compute_loss(ps, st.targets.clone().to(dev), model, HYP)
+        st.items = items.cpu().double()
+        p64 = [p.double().requires_grad_(True) for p in st.p32]
+        comps, rows = loss64(p64, st.targets.double(), model, HYP)
+        sum(comps).sum().backward()
+        st.want_items = torch.cat([c.detach() for c in comps])
+        st.g64 = [p.grad for p in p64]
+        st.rows = rows
+        st.mags, st.mag_loss = magnitudes(p64, rows, model)
+        # the fp32 assignment of the fused path equals the float64 one
+        fr = _loss()._targets_masked_stacked(model, st.targets.clone().to(dev), HYP)
+        st.masks_equal = all(torch.equal(fr["mask"][l].cpu(), r["mask"]) for l, r in enumerate(rows))
+        return loss
+
+    def head_grads(st, grads):
         st.g_nhwc = {}
-        for blk, g in zip(plan.heads, grads):
+        for blk, g in zip(st.plan.heads, grads):
             g = g.contiguous()
             st.g_nhwc[blk.i] = g.permute(0, 2, 3, 1)
             st.cot[blk.i] = g.view(batch, -1, nc + 6, blk.oh, blk.ow).permute(0, 1, 3, 4, 2).cpu()
-        orig_hg(grads)
 
-    def wrapped(blk):
-        st.bwd[blk.i] = T.check_block_bwd(st, blk, orig)
+    def block_check(st, blk, orig):
+        r = check_block_bwd(st, blk, orig)
         if blk.is_head and "pad" not in st.stash:
             st.stash["pad"] = dict(dz=blk.dz.clone(), cout=blk.cout)
-    plan._head_grads, plan._backward_block = head_grads, wrapped
-    try:
-        loss.backward()
-    finally:
-        del plan._head_grads, plan._backward_block
-    torch.cuda.synchronize()
-    after_backward(st)
+        return r
+    run_step(st, loss=loss, head_grads=head_grads, block_check=block_check)
+    # the first head's bias sum, kept for the bound self-test
+    hd = next(b for b in st.plan.blocks if b.is_head)
+    g = st.g_nhwc[hd.i].double()
+    st.stash["bias"] = dict(got=st.plan.garena[hd.gb_off:hd.gb_off + hd.cout].clone(), want=g.sum((0, 1, 2)),
+                            mag=g.abs().sum((0, 1, 2)), chain=head_bias_chain(st.batch, hd.oh, hd.ow))
     loss_checks(st)
     st.t_total = time.time() - t0
     _print_table(st)
     return st
-
-
-def after_backward(st):
-    """head bias sums and the weight-gradient gathers into the arena, as in test_train_step_f64_gpu"""
-    plan = st.plan
-    L = T._layout()
-    for blk in plan.blocks:
-        r = st.bwd.setdefault(blk.i, {})
-        if blk.is_head:
-            g = st.g_nhwc[blk.i].double()
-            gb = plan.garena[blk.gb_off:blk.gb_off + blk.cout]
-            want, mag = g.sum((0, 1, 2)), g.abs().sum((0, 1, 2))
-            chain = T.head_bias_chain(st.batch, blk.oh, blk.ow)
-            r["dbias"] = T.sum_check(gb, want, chain, mag)
-            if "bias" not in st.stash:
-                st.stash["bias"] = dict(got=gb.clone(), want=want, mag=mag, chain=chain)
-        if blk.i == 0:
-            want = blk.dw[0, :blk.cout, :27].reshape(blk.cout, 3, 3, 3)
-        elif blk.s2d:
-            c = blk.src.c
-            d2 = blk.dw[:, :blk.cout, :4 * c].permute(1, 2, 0).reshape(blk.cout, 4 * c, 2, 2)
-            want = L.s2d_weight_grad(d2, c)
-        else:
-            want = blk.dw[:, :blk.cout, :blk.cin].reshape(blk.k, blk.k, blk.cout, blk.cin).permute(2, 3, 0, 1)
-        r["gw_bits"] = torch.equal(blk.gw, want)
 
 
 def loss_checks(st):
@@ -393,8 +349,8 @@ def run_detect(nc, batch, h, w, seed=43):
     model = make_model(nc, h, w, seed).to(dev).eval()
     model.use_cuda_graph = True
     xa, xb = (torch.rand(batch, 3, h, w, generator=torch.Generator().manual_seed(seed + s)).to(dev) for s in (1, 2))
-    st = D.Run()
-    st.name, st.model, st.nc = "nc%d" % nc, model, nc
+    st = Run("nc%d" % nc, model)
+    st.nc = nc
     with torch.no_grad():
         io_a = model(xa)[0].clone()
         st.io, _ = model(xb)
@@ -402,18 +358,18 @@ def run_detect(nc, batch, h, w, seed=43):
     st.replayed = model._graph is not None and model.replayed_kernels == 2 * model._graph_kernels
     st.io_changed = not torch.equal(io_a, st.io)
     st.plan, st.x, st.stash = model._plan, model._x_static, None
-    D.map_plan(st)
+    map_plan(st)
     convs = sorted(st.conv_of)
-    st.res = {0: D.check_first(st)}
+    st.res = {0: check_first(st)}
     for i in convs[1:]:
-        st.res[i] = D.check_conv(st, i)
-    st.s2d = {i: D.check_s2d_step(st, i) for i in st.s2d_of}
-    st.buffers_ok, _ = D.check_buffers(st)
+        st.res[i] = check_conv(st, i)
+    st.s2d = {i: check_s2d_step(st, i) for i in st.s2d_of}
+    st.buffers_ok, _ = check_buffers(st)
     # decode: io within 2^-20 M of the float64 decode of the actual head buffers (direct path: nc + 6 > 8)
     st.decode, off = [], 0
     for (li, p), yi in zip(st.plan["heads"], model.yolo_layers):
         layer = model.module_list[yi]
-        want, mag = _decode_ref(p, layer.anchors.float(), float(layer.stride), 1.0, nc)
+        want, mag = decode_ref(p, layer.anchors.float(), float(layer.stride), 1.0, nc)
         got = st.io[:, off:off + want.shape[1]]
         st.decode.append(decode_ratio(got, want, mag))
         if off == 0:
@@ -446,23 +402,10 @@ def _get(kind, name):
     key = (kind, name)
     if key not in _CACHE:
         if kind == "step":
-            _CACHE[key] = run_step(name)
+            _CACHE[key] = mc_step(name)
         else:
             _CACHE[key] = run_detect(*(MODELS[name] if name in MODELS else NC_EVAL_ONLY))
     return _CACHE[key]
-
-
-def _bad(d, skip=("dy_mode", "near_zero_u", "n_elems", "wgrad_rw", "mean_over_std")):
-    out = []
-    for i, r in d.items():
-        for k, v in r.items():
-            if k == "error":
-                out.append((i, k, v[-600:]))
-            elif k in skip:
-                continue
-            elif (isinstance(v, bool) and not v) or (isinstance(v, float) and not v <= 1.0):
-                out.append((i, k, v))
-    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -502,7 +445,7 @@ def test_training_step_kernels_vs_float64(name):
     assert st.fwd_halo
     assert st.im2col == dict(bits=True, pad_zero=True, halo=True), st.im2col
     assert all(p[2] for p in st.packs), [p[:2] for p in st.packs if not p[2]]
-    bad = _bad(st.fwd) + _bad(st.bwd)
+    bad = bad_entries(st.fwd) + bad_entries(st.bwd)
     assert not bad, bad
     for i, r in st.bwd.items():
         if "near_zero_u" in r:
@@ -543,7 +486,7 @@ def test_training_refuses_2088_channel_heads_before_any_launch():
     nc, batch, h, w = NC_EVAL_ONLY
     model = make_model(nc, h, w, 5).cuda().train()
     x = torch.rand(batch, 3, h, w, device="cuda")
-    lib = _pkg()._lib.lib
+    lib = pkg()._lib.lib
     torch.cuda.synchronize()
     c0 = lib.ryolo_launch_count()
     with pytest.raises(NotImplementedError, match="limited to 2048 channels"):
@@ -570,14 +513,14 @@ def test_bounds_reject_plausible_bugs():
     out["scatter drops columns >= 16"] = cot_check(got, c["want"], c["m"], c["ncell"])["cls"]
     # the head bias gradient missing its last 8-channel group
     b = st.stash["bias"]
-    assert T.sum_check(b["got"], b["want"], b["chain"], b["mag"]) <= 1.0
+    assert sum_check(b["got"], b["want"], b["chain"], b["mag"]) <= 1.0
     gb = b["got"].clone()
     gb[-8:] = 0.0
-    out["head bias without its last 8 channels"] = T.sum_check(gb, b["want"], b["chain"], b["mag"])
+    out["head bias without its last 8 channels"] = sum_check(gb, b["want"], b["chain"], b["mag"])
     # a nonzero padding channel of the head dz (2016 = 63 * 32 has none: the 1512-channel heads, zcs 1536)
     d = _get("step", "nc15").stash["pad"]
     dz = d["dz"].clone()
-    assert bool((dz[..., d["cout"]:] == 0).all()) and T.halo_zero(dz)
+    assert bool((dz[..., d["cout"]:] == 0).all()) and halo_zero(dz)
     dz[1, 3, 4, d["cout"] + 5] = 1.0
     out["nonzero padding channel of the head dz"] = 0.0 if bool((dz[..., d["cout"]:] == 0).all()) else 2.0
     # decode reading the class scores with the nc = 1 row stride (anchor a's column k at channel 7 a + k)
@@ -586,12 +529,12 @@ def test_bounds_reject_plausible_bugs():
     bs, ch, ny, nx = p.shape
     no = dt.nc + 6
     na = ch // no
-    assert decode_ratio(e["got"], *_decode_ref(p, e["anchors"], e["stride"], 1.0, dt.nc)) <= 1.0
+    assert decode_ratio(e["got"], *decode_ref(p, e["anchors"], e["stride"], 1.0, dt.nc)) <= 1.0
     pb = p.view(bs, na, no, ny, nx).clone()
     for k in range(6, no):
         src = torch.arange(na, device=p.device) * 7 + k
         pb[:, :, k] = p[:, src.clamp(max=ch - 1)]
-    out["decode with the nc = 1 row stride"] = decode_ratio(e["got"], *_decode_ref(pb.view(bs, ch, ny, nx), e["anchors"],
+    out["decode with the nc = 1 row stride"] = decode_ratio(e["got"], *decode_ref(pb.view(bs, ch, ny, nx), e["anchors"],
                                                                                      e["stride"], 1.0, dt.nc))
     print("\n[bite] " + ", ".join("%s %.3g" % kv for kv in out.items()))
     bad = {k: v for k, v in out.items() if not v >= 2.0}

@@ -6,7 +6,7 @@ the outputs of a fresh plan with the new weights."""
 import pytest
 import torch
 
-from test_multiscale_train_gpu import _collect, _grid_bytes, _images, _pair, _yolov3  # noqa: F401 (_collect: fixture)
+from multiscale_cases import (collect, grid_bytes, images, pair, poison_pool, yolov3_small)  # noqa: F401 (collect: fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -15,13 +15,6 @@ def _fresh(m):
     """drop every eval plan and the pools: the next call builds its plan in zeroed storage"""
     m._plan = None
     m._pools = {}
-
-
-def _poison(m):
-    for pool in m._pools.values():
-        if pool.storage is not None:
-            pool.storage.fill_(0xFF)
-            pool.owner = None
 
 
 def _call(m, x):
@@ -38,7 +31,7 @@ def _bits(t):
 @pytest.mark.parametrize("poison", [False, True])
 def test_alternating_sizes_equal_fresh_plans(graph, poison, monkeypatch):
     from rotate_yolov3_b200 import layout as L
-    cand, ref = _pair(_yolov3, 16)
+    cand, ref = pair(yolov3_small, 16)
     cand.eval(), ref.eval()
     cand.use_cuda_graph = ref.use_cuda_graph = graph
     packs = []
@@ -55,18 +48,18 @@ def test_alternating_sizes_equal_fresh_plans(graph, poison, monkeypatch):
             seen = {}
             continue
         b, h, w = shape
-        x = _images(b, h, w, k % 2)
+        x = images(b, h, w, k % 2)
         if poison:
-            _poison(cand)
+            poison_pool(cand)
         torch.cuda.synchronize()
-        m0, g0, n0 = torch.cuda.memory_allocated(), _grid_bytes(cand), len(packs)
+        m0, g0, n0 = torch.cuda.memory_allocated(), grid_bytes(cand), len(packs)
         io, ps = _call(cand, x)
         torch.cuda.synchronize()
         key = (b, h, w)
         if key in seen:
             assert cand._plan is seen[key], "a revisit built a new plan"
             assert len(packs) == n0, "a revisit with unchanged weights packed weights"
-            assert torch.cuda.memory_allocated() - m0 == _grid_bytes(cand) - g0, "a revisit allocated device memory"
+            assert torch.cuda.memory_allocated() - m0 == grid_bytes(cand) - g0, "a revisit allocated device memory"
         seen[key] = cand._plan
         _fresh(ref)
         io_r, ps_r = _call(ref, x)

@@ -7,20 +7,19 @@ channels left by a larger shape would show; the poisoned runs fill the whole poo
 The reference model drops its plans and its pool before every step: a fresh plan in zeroed storage, the parent's
 behaviour."""
 import gc
-import math
 import os
 
 import pytest
 import torch
 
 import helpers
-from helpers import GOLDEN, SMALL_ANCHORS
+from builders import STEP_HYP, transfer_mask
+from helpers import GOLDEN
+from multiscale_cases import (collect, grid_bytes, images, pair, poison_pool, yolov3_small)  # noqa: F401 (collect: fixture)
 
 pytestmark = pytest.mark.gpu
 REF = os.path.join(GOLDEN, "reference_cfg")
 
-HYP = {"giou": 0.1, "cls": 27.76, "cls_pw": 1.0, "obj": 20.35, "obj_pw": 1.0, "iou_t": 0.3, "ang_t": math.pi / 6,
-       "reg": 1.0, "context_factor": 1.0}
 # normalised [image, class, x, y, w, h, angle]; images 0..2 so that the short batch of 3 keeps every target
 TARGETS = [[0, 0, 0.30, 0.40, 0.25, 0.08, 0.5], [1, 0, 0.70, 0.60, 0.30, 0.10, -0.9],
            [2, 0, 0.50, 0.50, 0.20, 0.07, 1.2], [0, 0, 0.20, 0.80, 0.22, 0.09, -0.3]]
@@ -30,25 +29,9 @@ SEQ = [(4, 320, 320), (4, 192, 256), (3, 320, 320), (4, 416, 416), (4, 192, 256)
 LR = 1e-3
 
 
-@pytest.fixture(autouse=True)
-def _collect():
-    """a model and its plans reference each other: collect the previous test's before this one allocates"""
-    gc.collect()
-    torch.cuda.empty_cache()
-    yield
-    gc.collect()
-
-
 def _mini():
     import rotate_yolov3_b200 as pkg
     return pkg.Darknet(helpers.mini_cfg(64, 48), {"context_factor": 1.0}, arc="default")
-
-
-def _yolov3():
-    import rotate_yolov3_b200 as pkg
-    from rotate_yolov3_b200 import cfgs
-    return pkg.Darknet(cfgs.yolov3_cfg(classes=1, anchors=SMALL_ANCHORS, n_anchors=6), {"context_factor": 1.0},
-                       arc="default")
 
 
 def _se():
@@ -62,23 +45,8 @@ def _se():
 
 
 def _m():
-    from test_dilated_cfg import m_model
+    from builders import m_model
     return m_model()
-
-
-def _pair(make, seed):
-    """two models with the same weights and buffers"""
-    out = []
-    for _ in range(2):
-        m = make()
-        helpers.init_darknet_weights(m, seed=seed)
-        m.nc, m.hyp = 1, HYP
-        out.append(m.cuda().train())
-    return out
-
-
-def _images(b, h, w, k):
-    return torch.rand(b, 3, h, w, generator=torch.Generator().manual_seed(100 + k)).cuda()
 
 
 def _targets(b):
@@ -89,24 +57,6 @@ def _fresh(m):
     """drop every training plan and the pool: the next step builds its plan in zeroed storage"""
     m._tplan = None
     m._pools = {}
-
-
-def _poison(m):
-    for pool in m._pools.values():
-        if pool.storage is not None:
-            pool.storage.fill_(0xFF)          # NaN in bf16 and fp32
-            pool.owner = None                 # the storage no longer holds any plan's invariants
-
-
-def _grid_bytes(m):
-    """device bytes of the YOLO layers' grids, which create_grids re-makes at every change of shape (as before pools)"""
-    seen = {}
-    for yi in m.yolo_layers:
-        for v in vars(m.module_list[yi]).values():
-            if isinstance(v, torch.Tensor) and v.is_cuda:
-                st = v.untyped_storage()
-                seen[st.data_ptr()] = -(-st.nbytes() // 512) * 512
-    return sum(seen.values())
 
 
 def _pool_bytes(m):
@@ -120,7 +70,7 @@ def _train_step(m, x, t, mask=None):
         p.requires_grad_(bool(tr))
         p.grad = None
     ps = m(x)
-    loss, items = compute_loss(ps, t.clone(), m, HYP)
+    loss, items = compute_loss(ps, t.clone(), m, STEP_HYP)
     loss.backward()
     out = {"p%d" % k: p.detach().cpu() for k, p in enumerate(ps)}
     out["loss"], out["items"] = loss.detach().cpu(), items.detach().cpu()
@@ -152,23 +102,23 @@ def _equal(got, want, what):
 
 
 def _run_sequence(make, seed, seq, graph, poison=False, mask_fn=None):
-    cand, ref = _pair(make, seed)
+    cand, ref = pair(make, seed)
     cand.use_cuda_graph = ref.use_cuda_graph = graph
     mask = mask_fn(cand) if mask_fn else None
     seen = {}
     for k, (b, h, w) in enumerate(seq):
-        x, t = _images(b, h, w, k), _targets(b)
+        x, t = images(b, h, w, k), _targets(b)
         key = (b, h, w, x.device)
         revisit = key in seen
         if poison:
-            _poison(cand)
+            poison_pool(cand)
         torch.cuda.synchronize()
-        m0, g0, pool0 = torch.cuda.memory_allocated(), _grid_bytes(cand), _pool_bytes(cand)
+        m0, g0, pool0 = torch.cuda.memory_allocated(), grid_bytes(cand), _pool_bytes(cand)
         got = _train_step(cand, x, t, mask)
         torch.cuda.synchronize()
         if revisit:
             assert cand._tplan is seen[key], "a revisited shape built a new plan"
-            assert torch.cuda.memory_allocated() - m0 == _grid_bytes(cand) - g0, \
+            assert torch.cuda.memory_allocated() - m0 == grid_bytes(cand) - g0, \
                 "a revisited shape allocated device memory"
         if _pool_bytes(cand) != pool0:          # growth dropped every cached plan
             assert pool0 < _pool_bytes(cand) and list(cand._tplans.values()) == [cand._tplan]
@@ -183,23 +133,18 @@ def _run_sequence(make, seed, seq, graph, poison=False, mask_fn=None):
 
 @pytest.mark.parametrize("graph", [False, True])
 @pytest.mark.parametrize("poison", [False, True])
-@pytest.mark.parametrize("make", [_mini, _yolov3], ids=["mini", "yolov3"])
+@pytest.mark.parametrize("make", [_mini, yolov3_small], ids=["mini", "yolov3"])
 def test_sequence_equals_fresh_plans(make, graph, poison):
     cand = _run_sequence(make, 11, SEQ, graph, poison)
     # the pool holds exactly the largest shape's requirement: what a fresh model needs for that shape alone
-    one, _ = _pair(make, 11)
-    _train_step(one, _images(4, 416, 416, 0), _targets(4))
+    one, _ = pair(make, 11)
+    _train_step(one, images(4, 416, 416, 0), _targets(4))
     assert _pool_bytes(cand) == _pool_bytes(one)
-
-
-def _transfer(m):
-    nf = int(m.module_defs[m.yolo_layers[0] - 1]["filters"])
-    return [p.shape[0] == nf for p in m.parameters()]         # train.py:131-132 (--transfer)
 
 
 @pytest.mark.parametrize("graph", [False, True])
 def test_sequence_with_frozen_layers(graph):
-    _run_sequence(_yolov3, 12, SEQ, graph, mask_fn=_transfer)
+    _run_sequence(yolov3_small, 12, SEQ, graph, mask_fn=transfer_mask)
 
 
 @pytest.mark.parametrize("make", [_se, _m], ids=["se", "yolov3-m"])
@@ -209,31 +154,31 @@ def test_se_and_dilated_graphs_at_two_sizes(make):
 
 
 def test_backward_after_a_forward_of_another_shape_raises():
-    m, _ = _pair(_mini, 14)
-    pa = m(_images(2, 96, 128, 0))
-    pb = m(_images(2, 64, 64, 1))
+    m, _ = pair(_mini, 14)
+    pa = m(images(2, 96, 128, 0))
+    pb = m(images(2, 64, 64, 1))
     with pytest.raises(RuntimeError):
         sum(p.sum() for p in pa).backward()
     sum(p.sum() for p in pb).backward()          # the latest forward's backward still runs
 
 
 def test_peak_memory_of_a_size_sequence_is_that_of_its_largest_shape():
-    fresh, _ = _pair(_yolov3, 15)
+    fresh, _ = pair(yolov3_small, 15)
     torch.cuda.synchronize()
     base = torch.cuda.memory_allocated()
     torch.cuda.reset_peak_memory_stats()
-    _train_step(fresh, _images(4, 416, 416, 0), _targets(4))
+    _train_step(fresh, images(4, 416, 416, 0), _targets(4))
     peak_one = torch.cuda.max_memory_allocated() - base
     need = _pool_bytes(fresh)
     del fresh, _
-    m, other = _pair(_yolov3, 15)
+    m, other = pair(yolov3_small, 15)
     del other
     gc.collect()
     torch.cuda.synchronize()
     base = torch.cuda.memory_allocated()
     torch.cuda.reset_peak_memory_stats()
     for k, s in enumerate((416, 256, 416, 320)):
-        _train_step(m, _images(4, s, s, k), _targets(4))
+        _train_step(m, images(4, s, s, k), _targets(4))
     peak_seq = torch.cuda.max_memory_allocated() - base
     assert peak_seq <= 1.05 * peak_one, (peak_seq, peak_one)
     assert _pool_bytes(m) == need

@@ -1,19 +1,12 @@
 """world_size-2 gloo tests (CPU) of the N>1 host logic: shard layout covers every unit exactly once, the optional
 row gather reassembles the matrix, and the timing reduction is a max over ranks."""
 import os
-import socket
 
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+from builders import free_port
 
 
 def _worker(rank, world, port, n_total):
@@ -70,4 +63,4 @@ def test_shard_range_properties():
 
 
 def test_two_rank_gloo():
-    mp.spawn(_worker, args=(2, _free_port(), 37), nprocs=2, join=True)
+    mp.spawn(_worker, args=(2, free_port(), 37), nprocs=2, join=True)

@@ -25,26 +25,18 @@ Operands are arbitrary fp32 values, split into three bf16 planes by ryolo_px_spl
   4. px_bn_stats + px_bn_finalize: two-pass float64 statistics, running-statistics update, eval mode.
   5. elementwise and layout kernels with one rounding each: bit for bit against a torch fp32 emulation.
   6. each bound fails on a reference with one plausible kernel bug put in."""
-import ctypes
-import math
-
 import pytest
 import torch
 import torch.nn.functional as F
 
+from builders import ryolo_lib
+from f64_refs import (NP, PX_BIAS_TOL, PX_MAX_TOL, PX_RMS_TOL, U, BnCase, bn_errors, f32_buf, gemm_sms, measure, merge3,
+                      planes_of, px_call, rup, split3, stream, ulps_f32, vp)
 from helpers import wgrad_plan
 
 pytestmark = pytest.mark.gpu
 
-NP = 3
 H100_SXM_SMS = 132
-MAX_TOL, RMS_TOL, BIAS_TOL = 5e-6, 2e-6, 1e-6
-U = 2.0 ** -24
-
-
-def _L():
-    import rotate_yolov3_b200 as pkg
-    return pkg._lib
 
 
 def _PP():
@@ -52,64 +44,15 @@ def _PP():
     return PP
 
 
-def _call(name, *args):
-    L = _L()
-    st = getattr(L.lib, name)(*args)
-    assert st == 0, (name, L.last_error())
-
-
-def _vp(t, byte_off=0):
-    return None if t is None else ctypes.c_void_p(t.data_ptr() + byte_off)
-
-
-def _st():
-    return _L().stream_ptr()
-
-
-def rup(x, m):
-    return (x + m - 1) // m * m
-
-
-def gemm_sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 # ---------------------------------------------------------------------------------------------------------------
 # split operands
-def split3(v):
-    """the kernels' split of fp32 v into three bf16 planes (plane k = bf16 of what planes < k left over)"""
-    p0 = v.to(torch.bfloat16)
-    r = v - p0.float()
-    p1 = r.to(torch.bfloat16)
-    r = r - p1.float()
-    return p0, p1, r.to(torch.bfloat16)
-
-
-def merge3(p0, p1, p2):
-    """the kernels' rebuild: fp32 sum starting from 0, smallest plane first"""
-    return ((torch.zeros_like(p0, dtype=torch.float32) + p2.float()) + p1.float()) + p0.float()
-
-
 def split_buf(x, plane, ch_off=0, cs=None):
     """fp32 NCHW -> split padded NHWC [B, H+2, W+2, NP*plane] (or cs channels): x at channels ch_off.. of every plane"""
     b, c, h, w = x.shape
     cs = NP * plane if cs is None else cs
     buf = torch.zeros((b, h + 2, w + 2, cs), dtype=torch.bfloat16, device=x.device)
-    _call("ryolo_px_split_from_nchw", _vp(x.contiguous()), b, c, h, w, _vp(buf, 2 * ch_off), cs, plane, NP, _st())
+    px_call("ryolo_px_split_from_nchw", vp(x.contiguous()), b, c, h, w, vp(buf, 2 * ch_off), cs, plane, NP, stream())
     return buf
-
-
-def planes_of(buf, plane, c, ch_off=0):
-    """the NP planes of channels [ch_off, ch_off + c) of a split buffer, interior pixels, NCHW"""
-    return [buf[:, 1:-1, 1:-1, k * plane + ch_off:k * plane + ch_off + c].permute(0, 3, 1, 2) for k in range(NP)]
-
-
-def from_buf(buf, plane, c, ch_off=0):
-    return merge3(*planes_of(buf, plane, c, ch_off))
-
-
-def f32_buf(b, h, w, cs, dev="cuda"):
-    return torch.zeros((b, h + 2, w + 2, cs), dtype=torch.float32, device=dev)
 
 
 def nchw(buf, c, ch_off=0):
@@ -118,15 +61,8 @@ def nchw(buf, c, ch_off=0):
 
 # ---------------------------------------------------------------------------------------------------------------
 # the three bounds
-def measure(got, want):
-    err = got.double() - want
-    rms = float(want.pow(2).mean().sqrt())
-    return dict(max=float(err.abs().max()) / float(want.abs().max()), rms=float(err.pow(2).mean().sqrt()) / rms,
-                bias=float((err * want.sign()).mean()) / rms)
-
-
 def within(m):
-    return m["max"] <= MAX_TOL and m["rms"] <= RMS_TOL and abs(m["bias"]) <= BIAS_TOL
+    return m["max"] <= PX_MAX_TOL and m["rms"] <= PX_RMS_TOL and abs(m["bias"]) <= PX_BIAS_TOL
 
 
 def fmt(m):
@@ -148,7 +84,7 @@ class WgradCase:
             img = torch.randn(batch, 3, h, w, generator=g).to(dev)
             self.x = img
             self.xw = torch.zeros((batch, h + 2, w + 2, NP * 64), dtype=torch.bfloat16, device=dev)
-            _call("ryolo_px_im2col_first", _vp(img), batch, h, w, _vp(self.xw), NP * 64, 64, NP, _st())
+            px_call("ryolo_px_im2col_first", vp(img), batch, h, w, vp(self.xw), NP * 64, 64, NP, stream())
             self.gh, self.gw, self.k = h, w, 1
             self.dz = torch.randn(batch, cout, h, w, generator=g).to(dev)
         elif kind == "s2d":              # 3x3 / stride 2 on [B, cin, h, w]: 2x2 taps on the space-to-depth buffer
@@ -158,8 +94,8 @@ class WgradCase:
             self.p4 = rup(4 * cin, 64)
             self.xw = torch.zeros((batch, h // 2 + 2, w // 2 + 2, NP * self.p4), dtype=torch.bfloat16, device=dev)
             for k in range(NP):
-                _call("ryolo_space_to_depth", _vp(src, 2 * k * plane), NP * plane, batch, h, w, cin,
-                      _vp(self.xw, 2 * k * self.p4), NP * self.p4, _st())
+                px_call("ryolo_space_to_depth", vp(src, 2 * k * plane), NP * plane, batch, h, w, cin,
+                      vp(self.xw, 2 * k * self.p4), NP * self.p4, stream())
             self.gh, self.gw, self.k = h // 2, w // 2, 2
             self.dz = torch.randn(batch, cout, h // 2, w // 2, generator=g).to(dev)
         else:                            # k x k stride 1, x at channel ch_off of a ctot-channel buffer
@@ -179,22 +115,22 @@ class WgradCase:
     def run(self, entry="ryolo_px_wgrad"):
         dev = self.dz.device
         dw = torch.zeros((self.k * self.k, NP * self.po, self.xcs), dtype=torch.float32, device=dev)
-        _call(entry, _vp(self.dzb), NP * self.po, NP * self.po, _vp(self.xw), self.xcs, self.xcs, self.b, self.gh, self.gw,
-              self.k, _vp(dw), _st())
+        px_call(entry, vp(self.dzb), NP * self.po, NP * self.po, vp(self.xw), self.xcs, self.xcs, self.b, self.gh, self.gw,
+              self.k, vp(dw), stream())
         return dw
 
     def unpack(self, dw):
         pi = self.xcs // NP
         if self.kind == "first":
             gw = torch.full((self.cout, 27, 1, 1), float("nan"), device=dw.device)
-            _call("ryolo_px_unpack_wgrad", _vp(dw), self.po, pi, NP, 0, self.cout, 27, 1, 0, _vp(gw), _st())
+            px_call("ryolo_px_unpack_wgrad", vp(dw), self.po, pi, NP, 0, self.cout, 27, 1, 0, vp(gw), stream())
             return gw.view(self.cout, 3, 3, 3)
         if self.kind == "s2d":
             gw = torch.full((self.cout, self.cin, 3, 3), float("nan"), device=dw.device)
-            _call("ryolo_px_unpack_wgrad", _vp(dw), self.po, pi, NP, 2, self.cout, self.cin, 3, 0, _vp(gw), _st())
+            px_call("ryolo_px_unpack_wgrad", vp(dw), self.po, pi, NP, 2, self.cout, self.cin, 3, 0, vp(gw), stream())
             return gw
         gw = torch.full((self.cout, self.cin, self.k, self.k), float("nan"), device=dw.device)
-        _call("ryolo_px_unpack_wgrad", _vp(dw), self.po, pi, NP, 0, self.cout, self.cin, self.k, self.ch_off, _vp(gw), _st())
+        px_call("ryolo_px_unpack_wgrad", vp(dw), self.po, pi, NP, 0, self.cout, self.cin, self.k, self.ch_off, vp(gw), stream())
         return gw
 
     def ref_fn(self):
@@ -256,7 +192,7 @@ def test_px_wgrad_vs_float64(name):
     if po["updates"] >= 700:
         # the 608 x 608 layers: one unrestarted accumulator over >= 700 updates is biased towards zero (measured on an
         # H100 SXM: bias/rms -9.0e-6 .. -2.1e-5 at batch 2, -7.5e-5 .. -1.7e-4 at batch 16)
-        assert mo["bias"] < -BIAS_TOL, (name, mo)
+        assert mo["bias"] < -PX_BIAS_TOL, (name, mo)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -271,19 +207,19 @@ def run_dgrad(dz, wt, h, w, stride, gbuf, ch_off, accumulate):
     dzb = split_buf(dz, po)
     dev = dz.device
     if stride == 1:
-        pwd = torch.empty(_L().lib.ryolo_px_packed_weight_bytes(cin, cout, k, PP.NTERMS), dtype=torch.uint8, device=dev)
-        _call("ryolo_px_pack_weights", _vp(wt), cin, cout, k, PP.NTERMS, PP.W_CODE, 1, _vp(pwd), _st())
-        _call("ryolo_px_conv", _vp(dzb), NP * po, 0, po, cout, _vp(pwd), PP.NTERMS, PP.A_CODE, b, h, w, k, cin,
-              _vp(gbuf, 4 * ch_off), gbuf.shape[-1], rup(cin, 4), accumulate, _st())
+        pwd = torch.empty(ryolo_lib().lib.ryolo_px_packed_weight_bytes(cin, cout, k, PP.NTERMS), dtype=torch.uint8, device=dev)
+        px_call("ryolo_px_pack_weights", vp(wt), cin, cout, k, PP.NTERMS, PP.W_CODE, 1, vp(pwd), stream())
+        px_call("ryolo_px_conv", vp(dzb), NP * po, 0, po, cout, vp(pwd), PP.NTERMS, PP.A_CODE, b, h, w, k, cin,
+              vp(gbuf, 4 * ch_off), gbuf.shape[-1], rup(cin, 4), accumulate, stream())
     else:
         p4 = rup(4 * cin, 64)
-        pwd = torch.empty(_L().lib.ryolo_px_packed_weight_bytes(4 * cin, cout, 2, PP.NTERMS), dtype=torch.uint8, device=dev)
-        _call("ryolo_px_pack_weights", _vp(wt), 4 * cin, cout, -2, PP.NTERMS, PP.W_CODE, 3, _vp(pwd), _st())
+        pwd = torch.empty(ryolo_lib().lib.ryolo_px_packed_weight_bytes(4 * cin, cout, 2, PP.NTERMS), dtype=torch.uint8, device=dev)
+        px_call("ryolo_px_pack_weights", vp(wt), 4 * cin, cout, -2, PP.NTERMS, PP.W_CODE, 3, vp(pwd), stream())
         dxs = f32_buf(b, h // 2, w // 2, p4, dev)
-        _call("ryolo_px_conv", _vp(dzb), NP * po, 0, po, cout, _vp(pwd), PP.NTERMS, PP.A_CODE, b, h // 2, w // 2, -2,
-              4 * cin, _vp(dxs), p4, p4, 0, _st())
-        _call("ryolo_px_depth_to_space", _vp(dxs), p4, b, h, w, cin, _vp(gbuf, 4 * ch_off), gbuf.shape[-1], accumulate,
-              _st())
+        px_call("ryolo_px_conv", vp(dzb), NP * po, 0, po, cout, vp(pwd), PP.NTERMS, PP.A_CODE, b, h // 2, w // 2, -2,
+              4 * cin, vp(dxs), p4, p4, 0, stream())
+        px_call("ryolo_px_depth_to_space", vp(dxs), p4, b, h, w, cin, vp(gbuf, 4 * ch_off), gbuf.shape[-1], accumulate,
+              stream())
 
 
 def ref_dgrad(dz, wt, h, w, stride):
@@ -347,114 +283,6 @@ def test_px_dgrad_vs_float64(name):
 
 # ---------------------------------------------------------------------------------------------------------------
 # 3. BN + PReLU backward
-class BnCase:
-    def __init__(self, c, batch, h, w, act=True, up=False, batch_stats=1, gres=None, seed=0, zero_u=True):
-        dev = torch.device("cuda")
-        g = torch.Generator().manual_seed(seed)
-        self.c, self.b, self.h, self.w, self.act, self.up, self.bs, self.gres_mode = c, batch, h, w, act, up, batch_stats, gres
-        self.po = rup(c, 64)
-        mu = torch.randn(c, generator=g) * 2.0
-        sd = torch.rand(c, generator=g) * 2.0 + 0.25
-        z = (torch.randn(batch, c, h, w, generator=g) * sd[None, :, None, None] + mu[None, :, None, None]).to(dev)
-        nz = min(4, c) if zero_u else 0
-        for ch in range(nz):                 # four pixels of the first channels share one value z0 ...
-            z[0, ch, 1, :3] = z[0, ch, 0, 0]
-        self.mean = z.double().mean((0, 2, 3)).float()
-        self.invstd = (1.0 / (z.double().var((0, 2, 3), unbiased=False) + 1e-5).sqrt()).float()
-        gamma = (torch.rand(c, generator=g) * 0.8 + 0.6).to(dev)
-        beta = (torch.randn(c, generator=g) * 0.2).to(dev)
-        self.scale = gamma * self.invstd
-        self.shift = beta - self.mean * self.scale
-        for ch in range(nz):                 # ... where u = (z0 * scale) + shift is exactly 0: shift = -(z0 * scale)
-            self.shift[ch] = -(z[0, ch, 0, 0] * self.scale[ch])
-        self.z = z
-        self.slope = torch.tensor([0.17], device=dev)
-        dh, dw_ = (2 * h, 2 * w) if up else (h, w)
-        self.dy = torch.randn(batch, c, dh, dw_, generator=g).to(dev)
-        self.old = torch.randn(batch, c, h, w, generator=g).to(dev) if gres == "acc" else None
-
-    def u(self):
-        return (self.z * self.scale[None, :, None, None]) + self.shift[None, :, None, None]
-
-    def d(self):
-        """dy as the kernel loads it: the 2x2 upsample's four gradients added in fp32, in the kernel's order"""
-        if not self.up:
-            return self.dy
-        s = torch.zeros_like(self.z)
-        for ry in range(2):
-            for rx in range(2):
-                s = s + self.dy[:, :, ry::2, rx::2]
-        return s
-
-    def mask(self):
-        return self.u() > 0 if self.act else torch.ones_like(self.z, dtype=torch.bool)
-
-    def run(self):
-        dev = self.z.device
-        b, c, h, w, po = self.b, self.c, self.h, self.w, self.po
-        zb = f32_buf(b, h, w, po)
-        zb[:, 1:-1, 1:-1, :c] = self.z.permute(0, 2, 3, 1)
-        dh, dw_ = self.dy.shape[2:]
-        dyb = f32_buf(b, dh, dw_, po)
-        dyb[:, 1:-1, 1:-1, :c] = self.dy.permute(0, 2, 3, 1)
-        sums = torch.full((2 * c + 1,), float("nan"), dtype=torch.float64, device=dev)
-        g = torch.Generator().manual_seed(5)
-        self.dz_init = torch.randn(b, h + 2, w + 2, NP * po, generator=g).to(torch.bfloat16).to(dev)   # sentinels
-        dzb = self.dz_init.clone()
-        gres = None
-        if self.gres_mode is not None:
-            gres = f32_buf(b, h, w, po)
-            gres[:, 1:-1, 1:-1, c:] = 5.0
-            if self.old is not None:
-                gres[:, 1:-1, 1:-1, :c] = self.old.permute(0, 2, 3, 1)
-            self.gres_init = gres.clone()
-        _call("ryolo_px_bn_act_bwd", _vp(dyb), po, int(self.up), _vp(zb), po, b, h, w, c, _vp(self.scale), _vp(self.shift),
-              _vp(self.mean), _vp(self.invstd), _vp(self.slope) if self.act else None, self.bs, _vp(sums), _vp(dzb),
-              NP * po, po, _vp(gres), po if gres is not None else 0, int(self.old is not None), NP, _st())
-        torch.cuda.synchronize()
-        return sums, dzb, gres
-
-    def ref(self, mask=None):
-        """float64 BN backward through PReLU on the kernel's inputs; mask: which u count as > 0"""
-        mask = self.mask() if mask is None else mask
-        d = self.d().double()
-        slope = float(self.slope) if self.act else 1.0
-        u = self.u().double()
-        du = torch.where(mask, d, d * slope)
-        zh = (self.z.double() - self.mean.double()[None, :, None, None]) * self.invstd.double()[None, :, None, None]
-        dbeta, dgamma = du.sum((0, 2, 3)), (du * zh).sum((0, 2, 3))
-        neg = ~mask
-        dslope = (d * u)[neg].sum() if self.act else torch.zeros((), dtype=torch.float64, device=d.device)
-        mags = (du.abs().sum((0, 2, 3)), (du * zh).abs().sum((0, 2, 3)), (d * u)[neg].abs().sum() if self.act else None)
-        n = du.shape[0] * du.shape[2] * du.shape[3]
-        sc = self.scale.double()[None, :, None, None]
-        if self.bs:
-            m1, m2 = (dbeta / n)[None, :, None, None], (dgamma / n)[None, :, None, None]
-            dz = sc * (du - m1 - zh * m2)
-            # the kernel's channel means are sums of fp32 du and du * zhat: each is off by a few ulps of the mean of the
-            # |terms|, which is far above |mean| when the terms cancel
-            a1, a2 = (mags[0] / n)[None, :, None, None], (mags[1] / n)[None, :, None, None]
-            dz_mag = sc.abs() * (du.abs() + m1.abs() + a1 + zh.abs() * (m2.abs() + a2))
-        else:
-            dz, dz_mag = sc * du, (sc * du).abs()
-        return dict(dbeta=dbeta, dgamma=dgamma, dslope=dslope, mags=mags, dz=dz, dz_mag=dz_mag)
-
-
-DZ_ULPS = 8
-
-
-def bn_errors(case, sums, dzb, r):
-    """worst error of each output over its bound (<= 1 passes)"""
-    c = case.c
-    out = dict(dbeta=float(((sums[:c] - r["dbeta"]).abs() / (1e-6 * r["mags"][0] + 1e-300)).max()),
-               dgamma=float(((sums[c:2 * c] - r["dgamma"]).abs() / (1e-6 * r["mags"][1] + 1e-300)).max()))
-    if case.act:
-        out["dslope"] = float((sums[2 * c] - r["dslope"]).abs() / (1e-6 * r["mags"][2] + 1e-300))
-    got = from_buf(dzb, case.po, c).double()
-    out["dz"] = float(((got - r["dz"]).abs() / (DZ_ULPS * U * r["dz_mag"] + 1e-38)).max())
-    return out
-
-
 BN_CASES = {
     "c8_act": dict(c=8, batch=2, h=20, w=20),
     "c40_up": dict(c=40, batch=2, h=19, w=19, up=True),
@@ -493,12 +321,6 @@ def test_px_bn_act_bwd_vs_float64(name):
 
 # ---------------------------------------------------------------------------------------------------------------
 # 4. statistics
-def ulps_f32(x):
-    """fp32 spacing at |x| (the distance to the next float away from zero)"""
-    a = x.float().abs()
-    return (torch.nextafter(a, torch.full_like(a, math.inf)) - a).double()
-
-
 def test_px_bn_stats_and_finalize_vs_float64():
     dev = torch.device("cuda")
     g = torch.Generator().manual_seed(11)
@@ -514,7 +336,7 @@ def test_px_bn_stats_and_finalize_vs_float64():
     zb[:, 1:-1, 1:-1, :c] = z.permute(0, 2, 3, 1)
     zb[..., c:] = 1e9                                                      # neighbouring channels are not read
     sums = torch.full((2 * c,), float("nan"), dtype=torch.float64, device=dev)
-    _call("ryolo_px_bn_stats", _vp(zb), po + 64, b, h, w, c, _vp(sums), _st())
+    px_call("ryolo_px_bn_stats", vp(zb), po + 64, b, h, w, c, vp(sums), stream())
     gamma = (torch.rand(c, generator=g) + 0.5).to(dev)
     beta = torch.randn(c, generator=g).to(dev)
     rm0 = torch.randn(c, generator=g).to(dev)
@@ -523,8 +345,8 @@ def test_px_bn_stats_and_finalize_vs_float64():
     outs = [torch.full((c,), float("nan"), device=dev) for _ in range(4)]
     n = b * h * w
     eps, mom = 1e-5, 0.1
-    _call("ryolo_px_bn_finalize", _vp(sums), c, float(n), eps, mom, _vp(gamma), _vp(beta), 0, *[_vp(t) for t in outs],
-          _vp(rm), _vp(rv), _st())
+    px_call("ryolo_px_bn_finalize", vp(sums), c, float(n), eps, mom, vp(gamma), vp(beta), 0, *[vp(t) for t in outs],
+          vp(rm), vp(rv), stream())
     torch.cuda.synchronize()
     mean, invstd, scale, shift = outs
     z64 = z.double()
@@ -552,8 +374,8 @@ def test_px_bn_stats_and_finalize_vs_float64():
     # eval mode: the running statistics, nothing written back (sums are not read)
     rm_e, rv_e = rm.clone(), rv.clone()
     outs_e = [torch.full((c,), float("nan"), device=dev) for _ in range(4)]
-    _call("ryolo_px_bn_finalize", None, c, 0.0, eps, mom, _vp(gamma), _vp(beta), 1, *[_vp(t) for t in outs_e], _vp(rm_e),
-          _vp(rv_e), _st())
+    px_call("ryolo_px_bn_finalize", None, c, 0.0, eps, mom, vp(gamma), vp(beta), 1, *[vp(t) for t in outs_e], vp(rm_e),
+          vp(rv_e), stream())
     torch.cuda.synchronize()
     assert torch.equal(rm_e, rm) and torch.equal(rv_e, rv)
     assert torch.equal(outs_e[0], rm)
@@ -597,8 +419,8 @@ def test_px_bn_act_fwd_bitwise(form):
     oh, ow = (2 * h, 2 * w) if up else (h, w)
     y_init = torch.randn(b, oh + 2, ow + 2, NP * po, generator=g).to(torch.bfloat16).to(dev)
     yb = y_init.clone()
-    _call("ryolo_px_bn_act_fwd", _vp(zb), po, b, h, w, c, _vp(scale), _vp(shift), _vp(slope) if act else None, _vp(resb),
-          NP * po if res is not None else 0, po if res is not None else 0, _vp(yb), NP * po, po, int(up), NP, _st())
+    px_call("ryolo_px_bn_act_fwd", vp(zb), po, b, h, w, c, vp(scale), vp(shift), vp(slope) if act else None, vp(resb),
+          NP * po if res is not None else 0, po if res is not None else 0, vp(yb), NP * po, po, int(up), NP, stream())
     torch.cuda.synchronize()
     u = (z * scale[None, :, None, None]) + shift[None, :, None, None]
     if act:
@@ -617,7 +439,7 @@ def test_px_head_grad_bitwise(na, no, dlo):
     b, ny, nx = 2, 19, 17
     gr = torch.randn(b, na, ny, nx, no, generator=torch.Generator().manual_seed(na)).to(dev)
     dst = torch.zeros((b, ny + 2, nx + 2, NP * dlo), dtype=torch.bfloat16, device=dev)
-    _call("ryolo_px_head_grad", _vp(gr), b, na, no, ny, nx, _vp(dst), NP * dlo, dlo, NP, _st())
+    px_call("ryolo_px_head_grad", vp(gr), b, na, no, ny, nx, vp(dst), NP * dlo, dlo, NP, stream())
     torch.cuda.synchronize()
     v = gr.permute(0, 1, 4, 2, 3).reshape(b, na * no, ny, nx)              # channel a * no + k
     assert_planes(dst, dlo, v)
@@ -634,7 +456,7 @@ def test_px_to_nchw_bitwise(bias):
     zb = torch.randn(b, h + 2, w + 2, zcs, generator=g).to(dev)
     bv = torch.randn(c, generator=g).to(dev) if bias else None
     out = torch.full((b, c, h, w), float("nan"), device=dev)
-    _call("ryolo_px_to_nchw", _vp(zb), zcs, b, c, h, w, _vp(bv), _vp(out), _st())
+    px_call("ryolo_px_to_nchw", vp(zb), zcs, b, c, h, w, vp(bv), vp(out), stream())
     torch.cuda.synchronize()
     want = nchw(zb, c)
     if bias:
@@ -647,7 +469,7 @@ def test_px_im2col_first_bitwise():
     b, h, w = 2, 37, 29
     img = torch.randn(b, 3, h, w, generator=torch.Generator().manual_seed(41)).to(dev)
     col = torch.zeros((b, h + 2, w + 2, NP * 64), dtype=torch.bfloat16, device=dev)
-    _call("ryolo_px_im2col_first", _vp(img), b, h, w, _vp(col), NP * 64, 64, NP, _st())
+    px_call("ryolo_px_im2col_first", vp(img), b, h, w, vp(col), NP * 64, 64, NP, stream())
     torch.cuda.synchronize()
     # column c * 9 + kh * 3 + kw, zero outside the image: F.unfold's order
     want = F.unfold(img, 3, padding=1).view(b, 27, h, w)

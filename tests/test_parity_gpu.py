@@ -16,10 +16,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from builders import PARITY_TOL as TOL, report_and_check_gradients
 from helpers import GOLDEN, SMALL_ANCHORS, init_darknet_weights, mini_cfg
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
 
 
 def _split(x_nchw, plane):
@@ -176,45 +176,10 @@ def test_darknet53_small_training_vs_reference():
             continue
         rows.append((int(name.split(".")[1]), name, float(np.abs(got - smp).max()) / scale,
                      abs(float(gr.norm()) - float(norm)) / float(norm)))
-    _report_and_check_gradients("darknet-53 160x128 training", rows)
+    report_and_check_gradients("darknet-53 160x128 training", rows)
     bn0 = m.module_list[0].BatchNorm2d
     _check("running_mean0", bn0.running_mean.cpu().numpy(), g["rm0"])
     _check("running_var0", bn0.running_var.cpu().numpy(), g["rv0"])
-
-
-def _report_and_check_gradients(tag, rows, slope_scale=None):
-    """rows: (block index, parameter name, max sample error / gradient scale, relative norm error).
-    North_star's 1e-4 is asserted where it is stated -- conv activations (above) -- and, as VERDICT r1 asks, on the
-    head-layer gradients.  Below the heads the comparison with an fp32 golden stops being meaningful at the first PReLU
-    KINK CROSSING: an activation u with |u| below the forward rounding noise gets another sign in the two
-    implementations, its gradient factor flips between 1 and the slope, and through the BatchNorm backward (the channel
-    means of du and du*zhat) the whole channel -- and through dgrad everything upstream -- shifts by ~1 / (pixels per
-    channel).  A float64 evaluation of the same graph arbitrates: blocks between the heads and the first crossing agree to 1e-5, the affected rows are
-    single output channels, and the fp32 REFERENCE ITSELF is 3e-3..9e-3 away from float64 in the same layers (ours
-    7e-3..2e-2 at 160 x 128, where a channel has only ~300 pixels).  So: tiered bounds, everything printed."""
-    heads = {n for i, n, _, _ in rows if n.endswith("Conv2d.bias")}
-    heads |= {n.replace("bias", "weight") for n in heads}
-    assert heads
-    kinds = {"conv": lambda n: n.endswith("Conv2d.weight") or n.endswith("Conv2d.bias"), "bn": lambda n: "BatchNorm2d" in n,
-             "slope": lambda n: n.endswith("activation.weight")}
-    worst = {}
-    print("%s: gradient error by depth and kind (max over the group of max(sample err / scale, norm err))" % tag)
-    for k in range(0, 8):
-        line = []
-        for kind, f in kinds.items():
-            sel = [(max(es, en), n) for i, n, es, en in rows if i // 15 == k and f(n)]
-            if sel:
-                w = max(sel)
-                worst[kind] = max(worst.get(kind, 0.0), w[0])
-                line.append("%s %.2e" % (kind, w[0]))
-        if line:
-            print("   blocks %3d-%3d: %s" % (15 * k, 15 * k + 14, "   ".join(line)))
-    worst_head = max(max(es, en) for i, n, es, en in rows if n in heads)
-    print("   head-layer gradients: %.2e   worst conv %.2e / bn %.2e / slope %.2e" % (worst_head, worst.get("conv", 0),
-                                                                                  worst.get("bn", 0), worst.get("slope", 0)))
-    assert worst_head <= TOL, worst_head
-    assert worst.get("conv", 0.0) <= 0.1, worst
-    assert worst.get("bn", 0.0) <= 0.3 and worst.get("slope", 0.0) <= 0.1, worst
 
 
 def _idx(numel, n, seed):
@@ -277,7 +242,7 @@ def test_baseline_shape_608_training_vs_reference():
             continue
         rows.append((int(name.split(".")[1]), name, float(np.abs(got - np.asarray(smp, dtype=np.float32)).max()) / float(amax),
                      abs(float(gr.norm()) - float(norm)) / float(norm)))
-    _report_and_check_gradients("608x608 training", rows)
+    report_and_check_gradients("608x608 training", rows)
     bn0 = m.module_list[0].BatchNorm2d
     _check("running_mean0", bn0.running_mean.cpu().numpy(), g["rm0"])
     _check("running_var0", bn0.running_var.cpu().numpy(), g["rv0"])

@@ -85,16 +85,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import test_parity_bwd_gpu as PB
-import test_train_step_f64_gpu as T
-import test_wgrad_gpu as W
+from builders import pkg
+from f64_refs import (BF16, NP, PX_BIAS_TOL, PX_MAX_TOL, PX_RMS_TOL, TINY, U, BnCase, _shift, bitwise, bn_errors, cdiv,
+                      conv_taps, d2s, gemm_sms, halo_zero, interior, measure, merge3, rup, s2d, s2d_dgrad_ref, split3,
+                      tapsum, ulps_f32, wgrad_ref)
 from helpers import SMALL_ANCHORS, init_darknet_weights, wgrad_plan
 
 pytestmark = pytest.mark.gpu
 
-U, F64, BF16, TINY = T.U, T.F64, T.BF16, T.TINY
 U64 = 2.0 ** -53
-NP = PB.NP
 SEG_UPDATES = 32              # wgmma k16 updates between two accumulator restarts (8 k-steps of 64)
 SEG_K = 512                   # GEMM K per accumulator segment
 TERMS = 1.0 + 2.0 ** -7       # sum of |a_i w_j| over the plane products, relative to |a| |w|
@@ -110,30 +109,13 @@ EXTRA_ENTRIES = ("ryolo_space_to_depth",)
 NOT_LAUNCHES = ("ryolo_px_packed_weight_bytes",)
 
 
-def _pkg():
-    import rotate_yolov3_b200 as pkg
-    return pkg
-
-
-def rup(x, m):
-    return (x + m - 1) // m * m
-
-
-def cdiv(a, b):
-    return -(-a // b)
-
-
-def interior(buf, off, c):
-    return buf[:, 1:-1, 1:-1, off:off + c]
-
-
 def plane_views(buf, lo, off, c):
     """interior [B, H, W, c] of the three planes of channels [off, off + c), plane k at off + k * lo"""
     return [interior(buf, off + k * lo, c) for k in range(NP)]
 
 
 def merged(buf, lo, off, c):
-    return PB.merge3(*plane_views(buf, lo, off, c))
+    return merge3(*plane_views(buf, lo, off, c))
 
 
 def lo_of(view):
@@ -146,7 +128,7 @@ def view_val(view):
 
 
 def split_equal(planes, v):
-    want = PB.split3(v.contiguous())
+    want = split3(v.contiguous())
     return all(torch.equal(p.contiguous().view(torch.int16), w.view(torch.int16)) for p, w in zip(planes, want))
 
 
@@ -184,13 +166,13 @@ def wgrad_e(mag, pw):
 def gemm_check(got, want, e):
     """element bound |got - want| <= e and the tensor-wide bounds of test_parity_bwd_gpu, as ratios (<= 1 passes)"""
     err = (got.double() - want).abs()
-    m = PB.measure(got, want)
-    return {"elem": float((err / (e + TINY)).max()), "max": m["max"] / PB.MAX_TOL, "rms": m["rms"] / PB.RMS_TOL,
-            "bias": abs(m["bias"]) / PB.BIAS_TOL, "_bias": m["bias"]}
+    m = measure(got, want)
+    return {"elem": float((err / (e + TINY)).max()), "max": m["max"] / PX_MAX_TOL, "rms": m["rms"] / PX_RMS_TOL,
+            "bias": abs(m["bias"]) / PX_BIAS_TOL, "_bias": m["bias"]}
 
 
 def ulps(x):
-    return PB.ulps_f32(x)
+    return ulps_f32(x)
 
 
 def wgrad_s2(x, dz):
@@ -203,7 +185,7 @@ def wgrad_s2(x, dz):
     outs, mags = [], []
     for kh in range(3):
         for kw in range(3):
-            a = T._shift(xp, kh - 1, kw - 1, oh, ow, 2).reshape(-1, cin)
+            a = _shift(xp, kh - 1, kw - 1, oh, ow, 2).reshape(-1, cin)
             outs.append(d.t() @ a)
             mags.append(d.abs().t() @ a.abs())
     return (torch.stack(outs).view(3, 3, cout, cin).permute(2, 3, 0, 1),
@@ -228,8 +210,8 @@ def unpack_emul(dw, po, pi, cout, cin, ks, off):
     return s.view(cout, cin, ks, ks)
 
 
-class PlanBn(PB.BnCase):
-    """test_parity_bwd_gpu's BnCase on a plan block's own tensors (z and dy fp32 NHWC, as the kernel read them)"""
+class PlanBn(BnCase):
+    """f64_refs.BnCase (test_parity_bwd_gpu) on a plan block's own tensors (z and dy fp32 NHWC, as the kernel read them)"""
 
     def __init__(self, z, d, mean, invstd, scale, shift, slope, po):
         self.z, self._d = z.permute(0, 3, 1, 2), d.permute(0, 3, 1, 2)
@@ -368,7 +350,7 @@ def _im2col(run, blk, a, snap):
     b, _, h, w = x.shape
     want = F.unfold(x, 3, padding=1).view(b, 27, h, w).permute(0, 2, 3, 1)
     run.put("im2col", 0, {"bits": split_equal(plane_views(plan.col, 64, 0, 27), want),
-                          "pad_zero": planes_pad_zero(plan.col, 64, 27), "halo": T.halo_zero(plan.col)})
+                          "pad_zero": planes_pad_zero(plan.col, 64, 27), "halo": halo_zero(plan.col)})
     return True
 
 
@@ -377,9 +359,9 @@ def _s2d(run, blk, a, snap):
     src, c4 = blk.src, 4 * blk.cin
     sp = interior(src.buf, src.ch_off + k * lo_of(src), src.c)
     got = interior(blk.xs, k * blk.p4, c4)
-    run.put("s2d", blk.i, {"bits": T.bitwise(got, T.s2d(sp)),
+    run.put("s2d", blk.i, {"bits": bitwise(got, s2d(sp)),
                            "pad_zero": bool((blk.xs[..., k * blk.p4 + c4:(k + 1) * blk.p4] == 0).all()),
-                           "halo": T.halo_zero(blk.xs)})
+                           "halo": halo_zero(blk.xs)})
     return True
 
 
@@ -393,13 +375,13 @@ def _conv_fwd(run, blk, a):
     w64 = run.weight(blk).double()
     if blk.i == 0:
         x = merged(plan.col, 64, 0, 27)
-        want, mag = T.tapsum(x, [(0, 0, w64.reshape(blk.cout, 27).t())], blk.oh, blk.ow)
+        want, mag = tapsum(x, [(0, 0, w64.reshape(blk.cout, 27).t())], blk.oh, blk.ow)
     else:
-        want, mag = T.tapsum(view_val(blk.src), T.conv_taps(w64), blk.oh, blk.ow, blk.stride)
+        want, mag = tapsum(view_val(blk.src), conv_taps(w64), blk.oh, blk.ow, blk.stride)
     k = a[6] * a[11] * a[11] * rup(a[4], 64)
     got = interior(blk.z, 0, blk.cout)
     r = gemm_check(got, want, conv_e(mag, k))
-    r["pad_zero"] = bool((blk.z[..., blk.cout:] == 0).all()) and T.halo_zero(blk.z)
+    r["pad_zero"] = bool((blk.z[..., blk.cout:] == 0).all()) and halo_zero(blk.z)
     run.put("head_z" if blk.is_head else "z", blk.i, r)
 
 
@@ -409,13 +391,13 @@ def _conv_dgrad(run, blk, a, snap):
     k = a[6] * a[11] * a[11] * rup(a[4], 64)
     src, gs = blk.src, blk.gsrc
     if blk.s2d:
-        want, mag = T.s2d_dgrad_ref(dz, w64, src.h, src.w)
+        want, mag = s2d_dgrad_ref(dz, w64, src.h, src.w)
         c4 = 4 * blk.cin
         r = gemm_check(interior(blk.dxs, 0, c4), want, conv_e(mag, k))
-        r["pad_zero"] = bool((blk.dxs[..., c4:] == 0).all()) and T.halo_zero(blk.dxs)
+        r["pad_zero"] = bool((blk.dxs[..., c4:] == 0).all()) and halo_zero(blk.dxs)
         run.put("dgrad", blk.i, r)
         return
-    want, mag = T.tapsum(dz, T.conv_taps(w64, mirror=True), src.h, src.w)
+    want, mag = tapsum(dz, conv_taps(w64, mirror=True), src.h, src.w)
     e = conv_e(mag, k)
     got = interior(gs.buf, gs.ch_off, gs.c)
     prior = interior(snap["gbuf"], gs.ch_off, gs.c)
@@ -430,7 +412,7 @@ def _conv_dgrad(run, blk, a, snap):
     r["_acc"] = float(acc)
     allowed = torch.zeros(gs.cs, dtype=torch.bool, device=got.device)
     allowed[gs.ch_off:gs.ch_off + gs.c] = True
-    r["outside"] = torch.equal(gs.buf[..., ~allowed], snap["gbuf"][..., ~allowed]) and T.halo_zero(gs.buf)
+    r["outside"] = torch.equal(gs.buf[..., ~allowed], snap["gbuf"][..., ~allowed]) and halo_zero(gs.buf)
     run.wrote(gs)
     run.put("dgrad", blk.i, r)
 
@@ -545,7 +527,7 @@ def _head_grad(run, blk, a, snap):
     b, na, ny, nx, no = g.shape
     v = g.permute(0, 2, 3, 1, 4).reshape(b, ny, nx, na * no)
     run.put("head_grad", blk.i, {"bits": split_equal(plane_views(blk.dz, blk.po, 0, na * no), v),
-                                 "pad_zero": planes_pad_zero(blk.dz, blk.po, na * no) and T.halo_zero(blk.dz)})
+                                 "pad_zero": planes_pad_zero(blk.dz, blk.po, na * no) and halo_zero(blk.dz)})
     return True
 
 
@@ -567,8 +549,8 @@ def _bn_bwd(run, blk, a, snap):
         d = g
     slope = seq.activation.weight.detach() if blk.has_act else None
     case = PlanBn(z, d, blk.mean, blk.invstd, blk.scale, blk.shift, slope, blk.po)
-    r = PB.bn_errors(case, blk.bsums, blk.dz, case.ref())
-    r["dz_pad_zero"] = planes_pad_zero(blk.dz, blk.po, c) and T.halo_zero(blk.dz)
+    r = bn_errors(case, blk.bsums, blk.dz, case.ref())
+    r["dz_pad_zero"] = planes_pad_zero(blk.dz, blk.po, c) and halo_zero(blk.dz)
     if blk.gres is not None:
         gr = blk.gres
         prior = interior(snap["gres"], gr.ch_off, c)
@@ -577,7 +559,7 @@ def _bn_bwd(run, blk, a, snap):
         r["gres_flag"] = bool(a[21]) == acc
         allowed = torch.zeros(gr.cs, dtype=torch.bool, device=z.device)
         allowed[gr.ch_off:gr.ch_off + c] = True
-        r["gres_outside"] = torch.equal(gr.buf[..., ~allowed], snap["gres"][..., ~allowed]) and T.halo_zero(gr.buf)
+        r["gres_outside"] = torch.equal(gr.buf[..., ~allowed], snap["gres"][..., ~allowed]) and halo_zero(gr.buf)
         run.wrote(gr)
     run.put("bn_act_bwd", blk.i, r)
     return True
@@ -600,24 +582,24 @@ def _unpack(run, blk, a, snap):
     run.gw[blk.i] = mine
     dz = merged(blk.dz, blk.po, 0, blk.cout)
     if blk.i == 0:
-        wr, wm = T.wgrad_ref(merged(plan.col, 64, 0, 27), dz, [(0, 0)])
+        wr, wm = wgrad_ref(merged(plan.col, 64, 0, 27), dz, [(0, 0)])
         want, mag = wr[0].reshape(w.shape), wm[0].reshape(w.shape)
     elif blk.s2d:
         want, mag = wgrad_s2(view_val(blk.src), dz)
     else:
         p = (blk.k - 1) // 2
         offs = [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)]
-        wr, wm = T.wgrad_ref(view_val(blk.src), dz, offs)
+        wr, wm = wgrad_ref(view_val(blk.src), dz, offs)
         want = wr.reshape(blk.k, blk.k, blk.cout, blk.cin).permute(2, 3, 0, 1)
         mag = wm.reshape(blk.k, blk.k, blk.cout, blk.cin).permute(2, 3, 0, 1)
-    pw = wgrad_plan(aw[9], aw[5], aw[2], aw[6], aw[7], aw[8], W.gemm_sms(), segmented=True)
+    pw = wgrad_plan(aw[9], aw[5], aw[2], aw[6], aw[7], aw[8], gemm_sms(), segmented=True)
     e = wgrad_e(mag, pw)
     r = gemm_check(mine, want, e)
     r["operands"] = aw[0] == blk.dz.data_ptr() and aw[3] == blk.xw_buf.data_ptr() and aw[10] == blk.dw.data_ptr()
     r["_ksplit"], r["_per_split"] = float(pw["ksplit"]), float(pw["per_split"])
     run.put("wgrad", blk.i, r)
     if run.want_stash:
-        old = wgrad_plan(aw[9], aw[5], aw[2], aw[6], aw[7], aw[8], W.gemm_sms())
+        old = wgrad_plan(aw[9], aw[5], aw[2], aw[6], aw[7], aw[8], gemm_sms())
         best = run.stash.get("conv_wgrad")
         if blk.i > 0 and (best is None or old["updates"] > best["updates"]):
             run.stash["conv_wgrad"] = dict(i=blk.i, updates=old["updates"], dz=blk.dz.clone(), aw=aw, ua=list(a),
@@ -636,13 +618,13 @@ def _d2s_pre(run, blk, a):
 
 def _d2s(run, blk, a, snap):
     gs = blk.gsrc
-    v = T.d2s(interior(blk.dxs, 0, 4 * blk.cin), blk.cin)
+    v = d2s(interior(blk.dxs, 0, 4 * blk.cin), blk.cin)
     acc = run.expect_acc(gs)
     prior = interior(snap["gbuf"], gs.ch_off, gs.c)
     r = {"bits": f32_equal(interior(gs.buf, gs.ch_off, gs.c), prior + v if acc else v), "acc_flag": bool(a[8]) == acc}
     allowed = torch.zeros(gs.cs, dtype=torch.bool, device=v.device)
     allowed[gs.ch_off:gs.ch_off + gs.c] = True
-    r["outside"] = torch.equal(gs.buf[..., ~allowed], snap["gbuf"][..., ~allowed]) and T.halo_zero(gs.buf)
+    r["outside"] = torch.equal(gs.buf[..., ~allowed], snap["gbuf"][..., ~allowed]) and halo_zero(gs.buf)
     run.wrote(gs)
     run.put("d2s", blk.i, r)
     return True
@@ -673,19 +655,19 @@ def buffer_checks(run):
         for v in (b.src, None if b.is_head else b.y, b.res):
             if v is not None and v.buf is not None and v.buf.dtype == BF16:
                 real[id(v.buf)] = (v.buf, max(real.get(id(v.buf), (None, 0))[1], v.ch_off + v.c))
-    ok = all(T.halo_zero(buf) and planes_pad_zero(buf, buf.shape[-1] // NP, c) for buf, c in real.values())
+    ok = all(halo_zero(buf) and planes_pad_zero(buf, buf.shape[-1] // NP, c) for buf, c in real.values())
     run.put("buffers", None, {"halo_and_pad": ok})
 
 
 # ---------------------------------------------------------------------------------------------------------------
 def make_model(kw, seed):
     from rotate_yolov3_b200 import cfgs
-    m = _pkg().Darknet(cfgs.yolov3_cfg(**kw), {"context_factor": 1.0}, arc="default", precision="parity")
+    m = pkg().Darknet(cfgs.yolov3_cfg(**kw), {"context_factor": 1.0}, arc="default", precision="parity")
     return init_darknet_weights(m, seed=seed)
 
 
 def run_shape(name):
-    pkg = _pkg()
+    import rotate_yolov3_b200 as pkg
     kw, batch, h, w = SHAPES[name]
     dev = torch.device("cuda")
     t0 = time.time()
@@ -838,10 +820,10 @@ def test_bounds_reject_plausible_bugs(runs):
     got = interior(blk.z, 0, blk.cout)
     n = rup(blk.cin, 64) // 64
     k = 6 * 9 * n * 64
-    want, mag = T.tapsum(view_val(src), T.conv_taps(w64), blk.oh, blk.ow)
+    want, mag = tapsum(view_val(src), conv_taps(w64), blk.oh, blk.ow)
     assert not failures(gemm_check(got, want, conv_e(mag, k)))
     x2 = (torch.zeros_like(pl[0], dtype=torch.float32) + pl[1].float()) + pl[0].float()
-    want2, mag2 = T.tapsum(x2, T.conv_taps(w64), blk.oh, blk.ow)
+    want2, mag2 = tapsum(x2, conv_taps(w64), blk.oh, blk.ow)
     found["two_planes"] = gemm_check(got, want2, conv_e(mag2, k))
     # the last segment: term a0 * w0 (last in the term table), the last 8 (tap, 64-channel chunk) k-steps
     w0 = w.to(BF16).double()
@@ -850,7 +832,7 @@ def test_bounds_reject_plausible_bugs(runs):
         tap, ch = divmod(r_, n)
         kh, kw = divmod(tap, 3)
         sl = slice(64 * ch, min(64 * ch + 64, blk.cin))
-        part, _ = T.tapsum(pl[0][..., sl].double(), [(kh - 1, kw - 1, w0[:, sl, kh, kw].t())], blk.oh, blk.ow)
+        part, _ = tapsum(pl[0][..., sl].double(), [(kh - 1, kw - 1, w0[:, sl, kh, kw].t())], blk.oh, blk.ow)
         lost += part
     found["lost_segment"] = gemm_check(got, want - lost, conv_e(mag, k))
     # ryolo_conv_wgrad (one unrestarted accumulator per split) on the same planes: biased towards zero
@@ -859,14 +841,14 @@ def test_bounds_reject_plausible_bugs(runs):
     b_ = plan.blocks[[b.i for b in plan.blocks].index(cw["i"])]
     dw = torch.zeros_like(b_.dw)
     vp = ctypes.c_void_p
-    s = _pkg()._lib.stream_ptr()
+    s = pkg()._lib.stream_ptr()
     assert run.real.ryolo_conv_wgrad(vp(cw["dz"].data_ptr()), aw[1], aw[2], vp(aw[3]), aw[4], aw[5], aw[6], aw[7], aw[8],
                                      aw[9], vp(dw.data_ptr()), s) == 0
     gw_old = torch.full(cw["shape"], float("nan"), device=dw.device)
     assert run.real.ryolo_px_unpack_wgrad(vp(dw.data_ptr()), *ua[1:9], vp(gw_old.data_ptr()), s) == 0
     torch.cuda.synchronize()
-    m_old = PB.measure(gw_old, cw["want"])
-    found["conv_wgrad"] = {"bias": abs(m_old["bias"]) / PB.BIAS_TOL, "_bias": m_old["bias"]}
+    m_old = measure(gw_old, cw["want"])
+    found["conv_wgrad"] = {"bias": abs(m_old["bias"]) / PX_BIAS_TOL, "_bias": m_old["bias"]}
     # a dgrad that overwrites where it must accumulate
     ow = st["overwrite"]
     found["overwrite"] = gemm_check(ow["got"], ow["want"], ow["e"])
@@ -886,9 +868,9 @@ def test_bounds_reject_plausible_bugs(runs):
     xb = ((torch.zeros_like(p0, dtype=torch.float32) + p2.float()) + p1w.float()) + p0.float()
     wb = run.weight(sb).double()
     k_s = 6 * 4 * rup(4 * sb.cin, 64)
-    want_s, mag_s = T.tapsum(view_val(s2), T.conv_taps(wb), sb.oh, sb.ow, 2)
+    want_s, mag_s = tapsum(view_val(s2), conv_taps(wb), sb.oh, sb.ow, 2)
     assert not failures(gemm_check(interior(sb.z, 0, sb.cout), want_s, conv_e(mag_s, k_s)))
-    want_b, mag_b = T.tapsum(xb, T.conv_taps(wb), sb.oh, sb.ow, 2)
+    want_b, mag_b = tapsum(xb, conv_taps(wb), sb.oh, sb.ow, 2)
     found["plane_stride"] = gemm_check(interior(sb.z, 0, sb.cout), want_b, conv_e(mag_b, k_s))
     # a nonzero padding channel in a head dz
     hb = plan.heads[0]
@@ -906,4 +888,4 @@ def test_bounds_reject_plausible_bugs(runs):
           "per chain)" % (n_rv, len(run.rv_biased), cw["i"], cw["updates"]))
     for name_, r in found.items():
         assert failures(r), (name_, r)
-    assert found["conv_wgrad"]["_bias"] < -PB.BIAS_TOL
+    assert found["conv_wgrad"]["_bias"] < -PX_BIAS_TOL

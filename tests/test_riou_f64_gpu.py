@@ -90,7 +90,7 @@ import pytest
 import torch
 
 import helpers
-from test_riou_loss_gpu import _pairs
+from builders import overlapping_pairs
 
 pytestmark = pytest.mark.gpu
 
@@ -332,7 +332,7 @@ def fam_far(g, parts):
 
 
 def fam_generic():
-    a, b = _pairs(160, 21)
+    a, b = overlapping_pairs(160, 21)
     return a.numpy(), b.numpy()
 
 
@@ -1018,7 +1018,7 @@ def test_match_detections_restates_greedy_loop(t):
 # ------------------------------------------------------------------------------------------------------------------
 def test_riou_loss_backpropagates_through_wide_and_strided_rows():
     from rotate_yolov3_b200.iou import riou_loss, rotated_iou
-    a, b = _pairs(64, 31)
+    a, b = overlapping_pairs(64, 31)
     a7 = torch.cat([a, torch.randn(64, 2)], 1).cuda()
     b7 = torch.cat([b, torch.randn(64, 2)], 1).cuda()
     w = torch.linspace(-1, 1, 64).cuda()

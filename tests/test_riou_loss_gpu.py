@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import helpers
+from builders import overlapping_pairs
 
 pytestmark = pytest.mark.gpu
 DP = ctypes.POINTER(ctypes.c_double)
@@ -20,20 +21,10 @@ def _oracle_iou(a, b):
     return orc.orc_skew_iou(a.ctypes.data_as(DP), b.ctypes.data_as(DP), 0)
 
 
-def _pairs(n, seed):
-    a = helpers.gen_boxes(n, seed, 200.0)
-    g = torch.Generator().manual_seed(seed + 1)
-    b = a.clone()
-    b[:, 0:2] += (torch.rand(n, 2, generator=g) - 0.5) * 0.6 * a[:, 3:4]
-    b[:, 2:4] *= 0.7 + 0.6 * torch.rand(n, 2, generator=g)
-    b[:, 4] += (torch.rand(n, generator=g) - 0.5) * 0.5
-    return a, b
-
-
 def test_value_and_gradient_vs_float64_oracle():
     from rotate_yolov3_b200.iou import riou_loss, rotated_iou
     n = 400
-    a, b = _pairs(n, 3)
+    a, b = overlapping_pairs(n, 3)
     # fp32-representable inputs on both sides
     ad = a.cuda().requires_grad_(True)
     bd = b.cuda().requires_grad_(True)
@@ -80,7 +71,7 @@ def test_value_and_gradient_vs_float64_oracle():
 
 def test_gradient_descent_on_riou_loss_aligns_boxes():
     from rotate_yolov3_b200.iou import riou_loss
-    a, b = _pairs(64, 9)
+    a, b = overlapping_pairs(64, 9)
     pred = a.cuda().clone().requires_grad_(True)
     target = b.cuda()
     opt = torch.optim.Adam([pred], lr=0.05)          # scale-free steps: pixels and radians have very different gradients

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+from builders import se_golden
 from helpers import GOLDEN
 
 REF = os.path.join(GOLDEN, "reference_cfg")
@@ -27,16 +28,12 @@ def in_reference_layout():
         os.chdir(cwd)
 
 
-def _golden():
-    return np.load(os.path.join(GOLDEN, "darknet_se_golden.npz"), allow_pickle=True)
-
-
 @pytest.mark.parametrize("cfg", SE_CFGS)
 def test_se_cfgs_parse_like_the_reference(cfg):
     from rotate_yolov3_b200.parse_config import parse_model_cfg
     with in_reference_layout():
         ours = parse_model_cfg(cfg)
-    want = json.loads(_golden()["parse:" + cfg].item().decode())
+    want = json.loads(se_golden()["parse:" + cfg].item().decode())
     assert len(ours) == len(want) == 128
     for i, (a, b) in enumerate(zip(ours, want)):
         assert set(a) == set(b), (i, set(a) ^ set(b))
@@ -60,7 +57,7 @@ def test_darknet_builds_the_reference_module_tree(cfg):
     from rotate_yolov3_b200.models import SELayer
     with in_reference_layout():
         m = pkg.Darknet(cfg, {"context_factor": 1.0}, arc="default")
-    g = _golden()
+    g = se_golden()
     assert list(m.state_dict().keys()) == [str(n) for n in g["state_names"]]
     assert sum(p.numel() for p in m.parameters()) == int(g["n_params"])
     se = [i for i, mod in enumerate(m.module_list) if isinstance(mod, SELayer)]

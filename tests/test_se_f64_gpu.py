@@ -18,53 +18,23 @@ each `from=-4` shortcut adds x, the concat routes' sources 36 / 61 are the unsca
 the concat consumer's dgrad, the unit's shortcut gradient, the SE), and the halos of u and gu are zero.  A last test puts
 plausible bugs into the stored tensors and requires a check to fail on each."""
 import os
+import types
 
 import pytest
 import torch
 
-from helpers import GOLDEN, init_darknet_weights
+from builders import REF_CFG
+from checked_step import Step, backward, dense_loss
+from f64_refs import TINY, U, bf16_check, halo_zero, rtz_bf16, se_chain, vint
+from helpers import init_darknet_weights
 
 pytestmark = pytest.mark.gpu
 
-REF = os.path.join(GOLDEN, "reference_cfg")
-U = 2.0 ** -24
-HALF_BF16 = 2.0 ** -8
-BIAS_TOL = 2.0 ** -12
-TINY = 1e-30
 BATCH = 2
-
-
-def interior(view):
-    return view.buf[:, 1:-1, 1:-1, view.ch_off:view.ch_off + view.c]
-
-
-def halo_zero(buf):
-    return bool((buf[:, 0] == 0).all() and (buf[:, -1] == 0).all() and (buf[:, :, 0] == 0).all()
-                and (buf[:, :, -1] == 0).all())
-
-
-def se_chain(h, w, c):
-    """longest fp32 addition chain of se_partial_kernel + the span sum (csrc/se.cu se_nsplit)"""
-    items = h * w * (c // 8)
-    nsplit = max(1, min(128, -(-items // 4096)))
-    span = -(-(h * w) // nsplit)
-    lanes = 256 // (c // 8)
-    return -(-span // lanes) + lanes + nsplit
-
-
-def rtz_bf16(v32):
-    return (v32.contiguous().view(torch.int32) & -65536).view(torch.float32).to(torch.bfloat16)
 
 
 def ratio(got, want, bound):
     return float(((got.double() - want).abs() / (bound + TINY)).max())
-
-
-def bf16_check(got, want, e):
-    err = got.double() - want
-    bound = HALF_BF16 * (want.abs() + e) + e + TINY
-    rms = float(want.pow(2).mean().sqrt())
-    return {"max": float((err.abs() / bound).max()), "bias": abs(float((err * want.sign()).mean())) / (BIAS_TOL * rms + TINY)}
 
 
 def fwd_refs(se, x, w1, w2):
@@ -112,53 +82,48 @@ def bwd_refs(se, gu, x, gx_old, w1, w2, gw1, gw2):
     return dict(ds=(ds64, ds_b), dm=(dm64, dm_b), gw1=(gw1_64, gw1_b), gw2=(gw2_64, gw2_b), gx=(gx64, gx_e))
 
 
-class Step:
-    pass
-
-
 def _run(cfg, size, seed):
     import rotate_yolov3_b200 as pkg
     cwd = os.getcwd()
-    os.chdir(REF)
+    os.chdir(REF_CFG)
     try:
         model = pkg.Darknet(cfg, {"context_factor": 1.0}, arc="default")
     finally:
         os.chdir(cwd)
     init_darknet_weights(model, seed=seed)
     model = model.cuda().train()
-    st = Step()
-    st.model = model
     x = torch.rand(BATCH, 3, size, size, generator=torch.Generator().manual_seed(seed + 1)).cuda()
+    st = Step(model, x)
     ps = model(x)
     torch.cuda.synchronize()
     plan = model._tplan
     st.plan = plan
     st.ses = [b.se for b in plan.blocks if b.se is not None]
-    st.fwd, st.bwd, st.keep = {}, {}, {}
+    st.fwd, st.keep = {}, {}
     for se in st.ses:
         fc = model.module_list[se.i].fc
         w1, w2 = fc[0].weight.detach().double(), fc[2].weight.detach().double()
-        xv = interior(se.x)
+        xv = vint(se.x)
         refs = fwd_refs(se, xv, w1, w2)
         r = {}
         B = BATCH
         r["m"] = ratio(se.m.view(B, se.c), *refs["m"])
         r["p"] = ratio(se.p.view(B, se.cr), *refs["p"])
         r["s"] = ratio(se.s.view(B, se.c), *refs["s"])
-        r.update({"u_" + k: v for k, v in bf16_check(interior(se.u), *refs["u"]).items()})
+        r.update({"u_" + k: v for k, v in bf16_check(vint(se.u), *refs["u"]).items()})
         r["halo_u"] = halo_zero(se.u.buf)
         st.fwd[se.i] = r
-    gen = torch.Generator().manual_seed(seed + 2)
-    gs = [torch.randn(p.shape, generator=gen).cuda() for p in ps]
-    loss = sum((p * g).sum() for p, g in zip(ps, gs))
-    orig = plan._backward_block
+    loss = dense_loss(st, ps, seed + 2)
 
-    def wrapped(blk):
+    def check(st, blk, orig):
+        """the SE of the block: gu, x and the prior gx snapshotted, the block and its SE run, then checked (recorded
+        under the SE's layer index)"""
         se = blk.se
         if se is None:
-            return orig(blk)
-        gu, xv = interior(se.gu).clone(), interior(se.x).clone()
-        gx_old = interior(se.gx).clone() if se.gx_acc else None
+            orig(blk)
+            return None
+        gu, xv = vint(se.gu).clone(), vint(se.x).clone()
+        gx_old = vint(se.gx).clone() if se.gx_acc else None
         orig(blk)
         fc = model.module_list[se.i].fc
         refs = bwd_refs(se, gu, xv, gx_old, fc[0].weight.detach().double(), fc[2].weight.detach().double(), se.gw1, se.gw2)
@@ -168,18 +133,13 @@ def _run(cfg, size, seed):
         r["dm"] = ratio(se.dm.view(B, se.c), *refs["dm"])
         r["gw1"] = ratio(se.gw1.view(se.cr, se.c), *refs["gw1"])
         r["gw2"] = ratio(se.gw2.view(se.c, se.cr), *refs["gw2"])
-        r.update({"gx_" + k: v for k, v in bf16_check(interior(se.gx), *refs["gx"]).items()})
+        r.update({"gx_" + k: v for k, v in bf16_check(vint(se.gx), *refs["gx"]).items()})
         r["halo_gu"] = halo_zero(se.gu.buf)
         st.bwd[se.i] = r
         if se.i == st.ses[0].i:
             st.keep = dict(se=se, gu=gu, x=xv, gx_old=gx_old, refs=refs,
                            fwd=fwd_refs(se, xv, fc[0].weight.detach().double(), fc[2].weight.detach().double()))
-    plan._backward_block = wrapped
-    try:
-        loss.backward()
-    finally:
-        del plan._backward_block
-    torch.cuda.synchronize()
+    backward(st, loss, check)
     return st
 
 
@@ -283,8 +243,7 @@ def test_se_kernels_first_writer_accumulate_and_relu_at_zero():
     assert lib.ryolo_se_bwd(P(gu), 256, P(x), 256, P(gx), 256, 0, B, h, w, c, P(w1), P(w2), cr, P(m), P(p), P(s), P(ds), P(dm),
                             P(gw1), P(gw2), P(ws), ws.numel(), st) == 0
     torch.cuda.synchronize()
-    se = Step()
-    se.h, se.w, se.c, se.cr, se.m, se.p, se.s, se.ds, se.dm = h, w, c, cr, m, p, s, ds, dm
+    se = types.SimpleNamespace(h=h, w=w, c=c, cr=cr, m=m, p=p, s=s, ds=ds, dm=dm)
     xi, gui = x[:, 1:-1, 1:-1], gu[:, 1:-1, 1:-1]
     r = bf16_check(gx[:, 1:-1, 1:-1], *bwd_refs(se, gui, xi, None, w1.double(), w2.double(), gw1, gw2)["gx"])
     assert r["max"] <= 1 and r["bias"] <= 1, r                     # first writer

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import torch
 
+from builders import cosine, golden_text, se_golden
 from helpers import GOLDEN, init_darknet_weights
 
 pytestmark = pytest.mark.gpu
@@ -33,16 +34,8 @@ def _in_reference_layout():
         os.chdir(cwd)
 
 
-def _golden():
-    return np.load(os.path.join(GOLDEN, "darknet_se_golden.npz"), allow_pickle=True)
-
-
-def _text(g, key):
-    return g[key].item().decode()
-
-
 def _seeds(g):
-    return json.loads(_text(g, "seeds"))
+    return json.loads(golden_text(g, "seeds"))
 
 
 def se_model(cfg, seed):
@@ -78,15 +71,11 @@ def _grad_stats(g, prefix, model, seed0):
     return out
 
 
-def _cos(a, b):
-    return float((a * b).sum() / (np.linalg.norm(a) * np.linalg.norm(b) + 1e-30))
-
-
 def test_small_se_graph_eval_and_train_vs_reference():
     import rotate_yolov3_b200 as pkg
-    g = _golden()
+    g = se_golden()
     sd = _seeds(g)
-    m = pkg.Darknet(_text(g, "small_cfg"), {"context_factor": 1.0}, arc="default")
+    m = pkg.Darknet(golden_text(g, "small_cfg"), {"context_factor": 1.0}, arc="default")
     init_darknet_weights(m, seed=sd["small_w"])
     m = m.cuda().eval()
     x = torch.rand(4, 3, 48, 64, generator=torch.Generator().manual_seed(sd["small_x"])).cuda()
@@ -112,7 +101,7 @@ def test_small_se_graph_eval_and_train_vs_reference():
         if name.endswith("activation.weight"):
             assert abs(float(got[0]) - float(want[0])) <= 0.3 * slope_scale, (name, float(got[0]), float(want[0]))
             continue
-        cos = _cos(got, want)
+        cos = cosine(got, want)
         if ".fc." in name:
             # an SE weight gradient starts from ds = sum over the image of gu * x, a sum with heavy cancellation of
             # bf16-rounded terms, and fc.0's is nearly rank one (the channel means of the 4 images are alike), so its
@@ -132,7 +121,7 @@ def test_small_se_graph_eval_and_train_vs_reference():
 
 
 def test_se512_train_forward_backward_vs_reference_autograd():
-    g = _golden()
+    g = se_golden()
     sd = _seeds(g)
     m = se_model(CFG_512, sd["train_w"]).train()
     x = torch.rand(2, 3, 128, 160, generator=torch.Generator().manual_seed(sd["train_x"])).cuda()
@@ -150,7 +139,7 @@ def test_se512_train_forward_backward_vs_reference_autograd():
     names = [str(n) for n in g["train_names"]]
     assert names == [n for n, _ in m.named_parameters()]
     stats = _grad_stats(g, "train", m, 1000)
-    cos_all = np.array([_cos(got, want) for _, got, want, _ in stats])
+    cos_all = np.array([cosine(got, want) for _, got, want, _ in stats])
     ratio_all = np.array([r for _, _, _, r in stats])
     idx = {n: i for i, n in enumerate(names)}
     se_names = [n for n in names if ".fc." in n]
@@ -196,7 +185,7 @@ SE_BOUNDS = dict(cos_min=0.3, cos_median=0.7, ratio_max=0.8, ratio_median=0.08)
 
 
 def test_se512_eval_vs_reference_model_output():
-    g = _golden()
+    g = se_golden()
     sd = _seeds(g)
     m = se_model(CFG_512, sd["eval_w"]).eval()
     x = torch.rand(1, 3, 512, 512, generator=torch.Generator().manual_seed(sd["eval_x"])).cuda()

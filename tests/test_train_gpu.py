@@ -11,23 +11,15 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GOLDEN, SMALL_ANCHORS, init_darknet_weights
+from builders import small_train_model
+from helpers import GOLDEN, init_darknet_weights
 
 pytestmark = pytest.mark.gpu
 
 
-def _model():
-    import rotate_yolov3_b200 as pkg
-    from rotate_yolov3_b200 import cfgs
-    text = cfgs.yolov3_cfg(width=160, height=128, classes=1, anchors=SMALL_ANCHORS, n_anchors=6)
-    m = pkg.Darknet(text, {"context_factor": 1.0}, arc="default")
-    init_darknet_weights(m, seed=321)
-    return m.cuda().train()
-
-
 def test_train_forward_backward_vs_reference_autograd():
     g = np.load(os.path.join(GOLDEN, "darknet_train_golden.npz"), allow_pickle=True)
-    m = _model()
+    m = small_train_model()
     x = torch.from_numpy(g["x"]).cuda()
     ps = m(x)
     assert isinstance(ps, list) and len(ps) == 3
@@ -124,7 +116,7 @@ def test_mini_graph_eval_and_train_vs_reference():
 
 def test_sgd_step_reduces_a_toy_loss():
     """three SGD steps on a fixed batch with a quadratic loss on the heads: the loss must go down"""
-    m = _model()
+    m = small_train_model()
     opt = torch.optim.SGD(m.parameters(), lr=2e-4, momentum=0.0)
     x = torch.rand(2, 3, 128, 160, device="cuda")
     losses = []

@@ -15,136 +15,16 @@ test_bound_rejects_a_lost_k_step).
 
 wgrad_plan() mirrors the host heuristic of ryolo_conv_wgrad (tile width BN, taps per CTA TG, split count), so that each
 case can assert the path it covers and a change to the heuristic cannot silently drop coverage."""
-import ctypes
-import math
-
 import pytest
 import torch
-import torch.nn.functional as F
 
+from builders import ryolo_lib
+from f64_refs import CASES, U, Case, bf, gemm_sms, ref_wgrad, unpacked, wgrad, worst_ratio
 from helpers import wgrad_plan
 
 pytestmark = pytest.mark.gpu
 
-KAPPA = 1.0
-U = 2.0 ** -24
-TINY = 1e-30
 H100_SXM_SMS = 132
-
-
-def gemm_sms(reserved=0):
-    n = torch.cuda.get_device_properties(0).multi_processor_count
-    return n - reserved if n - reserved > 8 else n
-
-
-def _bf(t):
-    return t.to(torch.bfloat16).float()
-
-
-def _lib():
-    import rotate_yolov3_b200 as pkg
-    return pkg._lib
-
-
-def wgrad(dzb, zcs, cout_pad, xb, xcs, cin_pad, b, h, w, k, dw, stream=None):
-    L = _lib()
-    sp = ctypes.c_void_p(stream.cuda_stream) if stream is not None else L.stream_ptr(dw.device)
-    st = L.lib.ryolo_conv_wgrad(L.ptr(dzb), zcs, cout_pad, L.ptr(xb), xcs, cin_pad, b, h, w, k, L.ptr(dw), sp)
-    assert st == 0, L.last_error()
-
-
-def ref_wgrad(x, dz, k, stride=1):
-    """float64 weight gradient of the k x k conv (k = 2: taps at offsets -1..0, the space-to-depth form) and its magnitude"""
-    x64, dz64 = x.double(), dz.double()
-    if k == 2:
-        shape = (dz.shape[1], x.shape[1], 2, 2)
-        f = lambda a, d: torch.nn.grad.conv2d_weight(F.pad(a, (1, 0, 1, 0)), shape, d, stride=1, padding=0)
-    else:
-        shape = (dz.shape[1], x.shape[1], k, k)
-        f = lambda a, d: torch.nn.grad.conv2d_weight(a, shape, d, stride=stride, padding=(k - 1) // 2)
-    return f(x64, dz64), f(x64.abs(), dz64.abs())
-
-
-def worst_ratio(got, want, mag, n_add, extra=None):
-    """max over entries of |got - want| / bound; <= 1 everywhere means the kernel is within the float64 bound"""
-    bound = KAPPA * math.sqrt(n_add) * U * mag + TINY
-    if extra is not None:
-        bound = bound + extra
-    return float(((got.double() - want).abs() / bound).max())
-
-
-def unpacked(dw, k, cout_pad, cin_pad, cout, cin):
-    return dw.view(k, k, cout_pad, cin_pad)[:, :, :cout, :cin].permute(2, 3, 0, 1)
-
-
-def s2d_nchw(x):
-    """space-to-depth of an NCHW tensor: channel (py * 2 + px) * C + c holds pixel (2Y + py, 2X + px)"""
-    return torch.cat([x[:, :, py::2, px::2] for py in range(2) for px in range(2)], 1)
-
-
-class Case:
-    """one wgrad launch: operands in padded NHWC, their float64 reference and the mirrored launch plan"""
-
-    def __init__(self, batch, h, w, cout, ksize, cin=None, s2d_c=None, narrow=False, seed=0):
-        from rotate_yolov3_b200 import layout as L
-        dev = torch.device("cuda")
-        g = torch.Generator().manual_seed(seed)
-        self.b, self.k = batch, ksize
-        if s2d_c is not None:        # 3x3/stride-2 layer on a [b, C, 2h, 2w] input, in its space-to-depth form
-            self.x_full = _bf(torch.randn(batch, s2d_c, 2 * h, 2 * w, generator=g)).to(dev)
-            self.x = s2d_nchw(self.x_full)
-            cin = 4 * s2d_c
-        else:
-            self.x = _bf(torch.randn(batch, cin, h, w, generator=g)).to(dev)
-        self.h, self.w, self.cin, self.cout = h, w, cin, cout
-        self.dz = _bf(torch.randn(batch, cout, h, w, generator=g)).to(dev)
-        self.cin_pad = L.round_up(cin, 64)
-        self.cout_pad = L.round_up(cout, 64 if cout <= 64 else (128 if cout <= 128 else 256))
-        self.xcs = L.round_up(cin, 32) if narrow else self.cin_pad
-        self.zcs = L.round_up(cout, 32) if narrow else self.cout_pad
-        if s2d_c is not None:        # built by the library's own space-to-depth kernel, as the training step does
-            xf = L.to_padded_nhwc(self.x_full, L.round_up(s2d_c, 64))
-            self.xb = L.alloc_padded(batch, h, w, self.xcs, dev)
-            st = _lib().lib.ryolo_space_to_depth(_lib().ptr(xf), xf.shape[-1], batch, 2 * h, 2 * w, s2d_c,
-                                                 _lib().ptr(self.xb), self.xcs, _lib().stream_ptr(dev))
-            assert st == 0, _lib().last_error()
-        else:
-            self.xb = L.to_padded_nhwc(self.x, self.xcs)
-        self.dzb = L.to_padded_nhwc(self.dz, self.zcs)
-        self._ref = None
-
-    def plan(self, reserved=0):
-        return wgrad_plan(self.k, self.cin_pad, self.cout_pad, self.b, self.h, self.w, gemm_sms(reserved))
-
-    def ref(self):
-        if self._ref is None:
-            self._ref = ref_wgrad(self.x, self.dz, self.k)
-        return self._ref
-
-    def new_dw(self, fill=None):
-        shape = (self.k * self.k, self.cout_pad, self.cin_pad)
-        if fill is None:
-            return torch.zeros(shape, dtype=torch.float32, device="cuda")
-        return fill.clone()
-
-    def run(self, dw, stream=None):
-        wgrad(self.dzb, self.zcs, self.cout_pad, self.xb, self.xcs, self.cin_pad, self.b, self.h, self.w, self.k, dw, stream)
-        return dw
-
-    def got(self, dw):
-        return unpacked(dw, self.k, self.cout_pad, self.cin_pad, self.cout, self.cin)
-
-
-# (case kwargs, expected plan: bn, tg always; ksplit and a short last split on a 132-SM H100 SXM)
-CASES = {
-    "k3_c64_tg3": (dict(batch=4, h=76, w=76, cin=64, cout=64, ksize=3), dict(bn=64, tg=3, ksplit=24, short_last=True, last=13)),
-    "k3_c128_tg1": (dict(batch=2, h=76, w=76, cin=128, cout=64, ksize=3), dict(bn=128, tg=1, ksplit=12, short_last=True)),
-    "s2d_c32_tg2": (dict(batch=4, h=38, w=38, s2d_c=32, cout=64, ksize=2), dict(bn=128, tg=2, ksplit=7, short_last=True)),
-    "s2d_c16_tg2": (dict(batch=4, h=38, w=38, s2d_c=16, cout=64, ksize=2), dict(bn=64, tg=2, ksplit=7)),
-    "s2d_c64_bn256": (dict(batch=2, h=38, w=38, s2d_c=64, cout=128, ksize=2), dict(bn=256, tg=1, ksplit=4, short_last=True)),
-    "k1_c768_3n2m": (dict(batch=2, h=38, w=38, cin=768, cout=256, ksize=1), dict(bn=256, tg=1, ksplit=4, tiles=6)),
-    "k3_narrow32": (dict(batch=2, h=40, w=40, cin=32, cout=32, ksize=3, narrow=True), dict(bn=64, tg=3, ksplit=4)),
-}
 
 
 def check_plan(plan, want):
@@ -229,7 +109,7 @@ def test_wgrad_accumulates_into_dw():
 def test_wgrad_split_counts_via_reserved_sms():
     """ryolo_set_reserved_sms shrinks the GEMM grid and with it the split count: every split count stays within the
     float64 bound, and repeated launches at one setting are bitwise equal.  The setting is process-global: restored."""
-    L = _lib()
+    L = ryolo_lib()
     c = Case(batch=8, h=76, w=76, cin=64, cout=64, ksize=3, seed=4)
     want, mag = c.ref()
     seen = {}
@@ -292,7 +172,7 @@ def test_wgrad_scratch_growth_and_concurrent_streams():
 def test_stride2_wgrad_space_to_depth_end_to_end(c_in, cout):
     """space_to_depth(x) -> 2x2-tap wgrad at h/2 x w/2 -> unpack mode 2 == float64 gradient of the 3x3/stride-2/pad-1
     conv; the multi-tensor unpack (one job table, as the training step builds it) writes the same bits"""
-    L = _lib()
+    L = ryolo_lib()
     from rotate_yolov3_b200 import _lib as lm
     c = Case(batch=4 if c_in < 64 else 2, h=38, w=38, s2d_c=c_in, cout=cout, ksize=2, seed=c_in)
     plan = c.plan()
@@ -325,12 +205,12 @@ def test_stride2_wgrad_space_to_depth_end_to_end(c_in, cout):
 def test_stride2_wgrad_zero_insert_end_to_end():
     """zero_insert2x(dz) -> 3x3 wgrad at input resolution == float64 gradient of the 3x3/stride-2/pad-1 conv"""
     from rotate_yolov3_b200 import layout as Lo
-    L = _lib()
+    L = ryolo_lib()
     dev = torch.device("cuda")
     g = torch.Generator().manual_seed(12)
     b, cin, cout, h, w = 4, 64, 128, 76, 76
-    x = _bf(torch.randn(b, cin, h, w, generator=g)).to(dev)
-    dz = _bf(torch.randn(b, cout, h // 2, w // 2, generator=g)).to(dev)
+    x = bf(torch.randn(b, cin, h, w, generator=g)).to(dev)
+    dz = bf(torch.randn(b, cout, h // 2, w // 2, generator=g)).to(dev)
     cin_pad, cout_pad = 64, 128
     xb = Lo.to_padded_nhwc(x, cin_pad)
     dzb = Lo.to_padded_nhwc(dz, cout_pad)

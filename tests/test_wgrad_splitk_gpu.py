@@ -15,15 +15,16 @@ import ctypes
 import pytest
 import torch
 
+from builders import ryolo_lib
+from f64_refs import Case, gemm_sms, worst_ratio
 from helpers import wgrad_plan
-from test_wgrad_gpu import Case, _lib, gemm_sms, worst_ratio
 
 pytestmark = pytest.mark.gpu
 
 
 def run(c, cout_pad, segmented=False, stream=None, dw=None):
     """c's launch with an explicit cout_pad (>= c.cout_pad; dz keeps its channel stride)"""
-    L = _lib()
+    L = ryolo_lib()
     if dw is None:
         dw = torch.zeros(c.k * c.k, cout_pad, c.cin_pad, dtype=torch.float32, device="cuda")
     fn = L.lib.ryolo_px_wgrad if segmented else L.lib.ryolo_conv_wgrad

@@ -27,7 +27,7 @@ from se_step_times import event_ms, gpu_info  # noqa: E402
 def _model(cfg):
     import rotate_yolov3_b200 as pkg
     from helpers import init_darknet_weights
-    from test_dilated_cfg import m_cfg_text
+    from builders import m_cfg_text
     text = m_cfg_text(cfg)
     m = pkg.Darknet(text, {"context_factor": 1.0}, arc="default")
     return init_darknet_weights(m, seed=1).cuda().eval()

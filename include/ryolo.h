@@ -588,6 +588,74 @@ int ryolo_augment_warp(const ryolo_warp_job* jobs_dev, int njobs, uint8_t* rowma
 int ryolo_augment_finish(const ryolo_finish_job* jobs_dev, int njobs, const uint8_t* rowmax, void* out, int h, int w,
                          int out_dtype, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * JPEG decode <- cv2.imread(path) (IMREAD_COLOR)          utils/datasets.py:105, 382, 434
+ * Decodes a batch of 8-bit sequential Huffman JPEG streams with one interleaved scan (1 or 3 components,
+ * sampling 4:4:4, 4:2:2, 4:2:0, 4:4:0, 4:1:1) into uint8 HWC BGR images, byte for byte what libjpeg-turbo's
+ * default decompression computes (ISLOW IDCT, fancy upsampling, YCbCr -> BGR), with the Exif orientation
+ * applied as cv2.imread applies it.  The host parses the markers and builds the tables
+ * (rotate-yolov3_b200/decode.py); csrc/jpeg.cuh holds the per-symbol and per-pixel arithmetic.
+ *
+ * Entropy decoding runs per restart interval (a segment: the bytes [start, end) between markers), split into
+ * chunks of chunk_bytes, one thread per chunk (Weissenberger & Schmidt, ICPP 2018): each chunk is decoded from
+ * its first byte, then each thread decodes on from where the previous chunk's decoder stopped until its state
+ * (bit position, coefficient index, block within the MCU) matches the state the chunk decoder reached at the same
+ * chunk end, and the chunks on the true decode path write the coefficients.
+ * chunk_seg[c] is chunk c's segment; a segment's chunks are consecutive (first_chunk .. first_chunk + nchunk).
+ * huff holds the Huffman tables the images refer to, quant 64 quantisation values per table in natural order.
+ * max_blocks >= blocks of any image (mcux * mcuy * bpm), max_out_h >= out rows of any image.
+ * status[i] is set to a nonzero RYOLO_JPEG_ST_* mask when image i cannot be decoded on the device (a code not
+ * in its table, a coefficient run past the block, data ending before the last block, a chunk that does not
+ * synchronise); its output is then unspecified.  Every read stays inside its segment.
+ * stages: RYOLO_JPEG_ENTROPY (status, coefficients), RYOLO_JPEG_PIXELS (IDCT, upsampling, colour, store) or both;
+ * the second reads the coefficients the first left in the workspace.  image_bytes: the size of the image area
+ * the images' coef_off / plane_off point into.  Allocates nothing; capturable in a CUDA graph; data < 4 GiB.
+ * ------------------------------------------------------------------------------------------ */
+#define RYOLO_JPEG_YCC 0         /* YCbCr -> BGR                                                        */
+#define RYOLO_JPEG_RGB 1         /* stored as RGB (Adobe transform 0 or component ids 'R', 'G', 'B')    */
+#define RYOLO_JPEG_GRAY 2        /* one component, replicated into B, G, R                             */
+#define RYOLO_JPEG_ENTROPY 1
+#define RYOLO_JPEG_PIXELS 2
+#define RYOLO_JPEG_ST_BAD_CODE 1  /* a code not in its table, or a run past coefficient 63          */
+#define RYOLO_JPEG_ST_TRUNCATED 2 /* the segment ends before its last block                         */
+#define RYOLO_JPEG_ST_NO_SYNC 4   /* a chunk on the decode path did not synchronise                 */
+typedef struct ryolo_jpeg_image {
+  int64_t out_off;      /* byte offset of the [out_h, out_w, 3] BGR image in out                              */
+  int64_t coef_off;     /* byte offset in the image area of the int16 coefficient blocks, in decode order      */
+  int64_t plane_off[3]; /* byte offsets in the image area of the component sample planes                      */
+  int32_t width, height;  /* stored size                                                                   */
+  int32_t out_w, out_h;   /* size after the orientation                                                    */
+  int32_t orient;         /* Exif orientation 1..8                                                         */
+  int32_t ncomp, color;   /* 1 or 3; RYOLO_JPEG_YCC / RGB / GRAY                                           */
+  int32_t hmax, vmax;     /* largest sampling factors                                                      */
+  int32_t mcux, mcuy, bpm; /* MCUs per row, MCU rows, blocks per MCU                                       */
+  int32_t h[3], v[3];     /* sampling factors                                                              */
+  int32_t boff[3];        /* first block of the component within the MCU (64 for absent components)        */
+  int32_t pitch[3];       /* plane row bytes, mcux * h * 8 (rows: mcuy * v * 8)                            */
+  int32_t dw[3], dh[3];   /* component size, ceil(width * h / hmax) x ceil(height * v / vmax)              */
+  int32_t qtab[3];        /* first value of the component's quantisation table in quant                    */
+  int32_t dctab[3], actab[3]; /* the component's Huffman tables in huff                                    */
+  int32_t reserved;
+} ryolo_jpeg_image;
+typedef struct ryolo_jpeg_segment {
+  int64_t start, end;      /* entropy-coded bytes [start, end) in data, stuffing included                       */
+  int32_t image, first_mcu, nmcu;
+  int32_t first_chunk, nchunk;
+  int32_t reserved;
+} ryolo_jpeg_segment;
+typedef struct ryolo_jpeg_huff {
+  uint16_t lut[512];    /* 9-bit lookahead: (length << 8) | symbol, 0 when the code is longer than 9 bits       */
+  int32_t maxcode[18];  /* largest code of each length, -1 when there is none (libjpeg's derived table)          */
+  int32_t valoff[18];   /* symbol index minus code, per length                                                  */
+  uint8_t vals[256];    /* symbols in code order                                                                */
+} ryolo_jpeg_huff;
+size_t ryolo_jpeg_workspace_bytes(int nchunks, long long image_bytes);
+int ryolo_jpeg_decode(const ryolo_jpeg_image* images, int nimages, const ryolo_jpeg_segment* segs, int nsegs,
+                      const int32_t* chunk_seg, int nchunks, int chunk_bytes, const uint8_t* data,
+                      long long data_bytes, const ryolo_jpeg_huff* huff, const uint16_t* quant, int max_blocks,
+                      int max_out_h, uint8_t* out, int32_t* status, void* workspace, size_t workspace_bytes,
+                      long long image_bytes, int stages, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,6 +10,7 @@ from .nms import nms_filter, non_max_suppression, r_nms  # noqa: F401
 from .models import Darknet, YOLOLayer  # noqa: F401
 from .preprocess import letterbox, letterbox_labels, scale_coords  # noqa: F401
 from .augment import train_batch  # noqa: F401
+from .decode import decode_images  # noqa: F401
 
 __all__ = ["r_nms", "non_max_suppression", "nms_filter", "skew_bbox_iou", "rotated_iou_matrix", "Darknet", "YOLOLayer",
-           "letterbox", "letterbox_labels", "scale_coords", "train_batch"]
+           "letterbox", "letterbox_labels", "scale_coords", "train_batch", "decode_images"]

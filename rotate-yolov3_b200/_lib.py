@@ -75,6 +75,30 @@ class FinishJob(ctypes.Structure):
                 ("reserved", ctypes.c_int32)]
 
 
+class JpegImage(ctypes.Structure):
+    """mirror of ryolo_jpeg_image"""
+    _fields_ = [("out_off", ctypes.c_int64), ("coef_off", ctypes.c_int64), ("plane_off", ctypes.c_int64 * 3),
+                ("width", ctypes.c_int32), ("height", ctypes.c_int32), ("out_w", ctypes.c_int32),
+                ("out_h", ctypes.c_int32), ("orient", ctypes.c_int32), ("ncomp", ctypes.c_int32),
+                ("color", ctypes.c_int32), ("hmax", ctypes.c_int32), ("vmax", ctypes.c_int32), ("mcux", ctypes.c_int32),
+                ("mcuy", ctypes.c_int32), ("bpm", ctypes.c_int32)]
+    _fields_ += [(n, ctypes.c_int32 * 3) for n in ("h", "v", "boff", "pitch", "dw", "dh", "qtab", "dctab", "actab")]
+    _fields_ += [("reserved", ctypes.c_int32)]
+
+
+class JpegSegment(ctypes.Structure):
+    """mirror of ryolo_jpeg_segment"""
+    _fields_ = [("start", ctypes.c_int64), ("end", ctypes.c_int64), ("image", ctypes.c_int32),
+                ("first_mcu", ctypes.c_int32), ("nmcu", ctypes.c_int32), ("first_chunk", ctypes.c_int32),
+                ("nchunk", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
+class JpegHuff(ctypes.Structure):
+    """mirror of ryolo_jpeg_huff"""
+    _fields_ = [("lut", ctypes.c_uint16 * 512), ("maxcode", ctypes.c_int32 * 18), ("valoff", ctypes.c_int32 * 18),
+                ("vals", ctypes.c_uint8 * 256)]
+
+
 # name -> (restype, argtypes); must list every symbol include/ryolo.h declares (tests/test_abi.py checks it)
 SIGNATURES = {
     "ryolo_abi_version": (_i, []),
@@ -107,6 +131,9 @@ SIGNATURES = {
     "ryolo_letterbox": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _vp]),
     "ryolo_augment_warp": (_i, [_vp, _i, _vp, _i, _i, _vp]),
     "ryolo_augment_finish": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _vp]),
+    "ryolo_jpeg_workspace_bytes": (_sz, [_i, ctypes.c_longlong]),
+    "ryolo_jpeg_decode": (_i, [_vp, _i, _vp, _i, _vp, _i, _i, _vp, ctypes.c_longlong, _vp, _vp, _i, _i, _vp, _vp, _vp,
+                               _sz, ctypes.c_longlong, _i, _vp]),
     "ryolo_conv_unpack_wgrad_multi": (_i, [_vp, _i, _vp, ctypes.c_longlong, _vp]),
     "ryolo_conv_bn_act_fwd": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_conv_first_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp]),

@@ -6,7 +6,10 @@ test_detect_forward_f64_gpu.py) bring their model, shape and extra checks and re
 Training step (run_step): after model(x) every buffer a forward kernel wrote is still there, so forward_checks checks
 each launch post hoc on the plan's own input buffers; plan._backward_block is wrapped (instance attribute) so that each
 block's inputs are snapshotted, the production code runs unchanged and its outputs are checked right after
-(check_block_bwd).  The bounds are stated in test_train_step_f64_gpu.py.
+(check_block_bwd).  The bounds are stated in test_train_step_f64_gpu.py.  run_step_chunked runs the same checks at a
+batch whose activations fill the card (test_train_scale_f64_gpu.py): over image chunks, with host copies of only what a
+block overwrites.  schedule_rows mirrors what each launch's schedule derives from the shape, from a plan built or only
+laid out (plan_layout).
 
 Eval forward (map_plan, check_first, check_conv, check_s2d_step, check_buffers): the steps of the eval plan mapped to the
 graph's layers and every conv launch checked on its own input buffers; the bounds are stated in
@@ -18,9 +21,10 @@ import torch
 import torch.nn.functional as F
 
 from builders import ryolo_lib
-from f64_refs import (BF16, BIAS_TOL, F64, STAT_TOL, TINY, U, bf16_check, bitwise, bn_act_fwd_ref, bn_chain, check_z,
-                      conv_taps, d2s, f32_check, gemm_sms, halo_zero, head_bias_chain, interior, rup, s2d,
-                      s2d_dgrad_ref, sum_check, tapsum, vint, wgrad_ratio, wgrad_ref, worst_ratio)
+from f64_refs import (BF16, BIAS_TOL, F64, STAT_TOL, TINY, U, bf16_check, bitwise, bn_act_fwd_ref, bn_chain, bn_pieces,
+                      check_z, conv_schedule, conv_taps, d2s, f32_check, gemm_sms, halo_zero, head_bias_blocks,
+                      head_bias_chain, interior, rup, s2d, s2d_dgrad_ref, sum_check, tapsum, vint, wgrad_ratio, wgrad_ref,
+                      worst_ratio)
 from helpers import wgrad_plan
 
 
@@ -70,17 +74,41 @@ def stats_check(z, c, sums, mean, invstd, scale, shift, rm0, rv0, rm, rv, gamma,
     statistics (target 2^-12), the finalisation and the running statistics against both the float64 statistics and the
     fp32 arithmetic of bn_finalize_channel applied to the kernel's own sums"""
     z64 = z.double().reshape(-1, c)
-    n = z64.shape[0]
     m64 = z64.mean(0)
-    v64 = (z64 - m64).pow(2).mean(0)
+    ref = dict(n=z64.shape[0], m64=m64, v64=(z64 - m64).pow(2).mean(0), s1=z64.sum(0), a1=z64.abs().sum(0),
+               s2=z64.pow(2).sum(0))
+    return stats_ratios(ref, z.device, c, sums, mean, invstd, scale, shift, rm0, rv0, rm, rv, gamma, beta, eps, mom, l,
+                        unbiased)
+
+
+def stats_ref_chunked(z, c, chunk_list):
+    """the float64 reductions stats_ratios needs, over image chunks of z [B, h, w, c] (two passes)"""
+    s1 = torch.zeros(c, dtype=F64, device=z.device)
+    a1, s2, q = s1.clone(), s1.clone(), s1.clone()
+    for b0, b1 in chunk_list:
+        z64 = z[b0:b1].double().reshape(-1, c)
+        s1 += z64.sum(0)
+        a1 += z64.abs().sum(0)
+        s2 += z64.pow(2).sum(0)
+        del z64
+    n = z.numel() // c
+    m64 = s1 / n
+    for b0, b1 in chunk_list:
+        q += (z[b0:b1].double().reshape(-1, c) - m64).pow(2).sum(0)
+    return dict(n=n, m64=m64, v64=q / n, s1=s1, a1=a1, s2=s2)
+
+
+def stats_ratios(ref, device, c, sums, mean, invstd, scale, shift, rm0, rv0, rm, rv, gamma, beta, eps, mom, l,
+                 unbiased=True):
+    n, m64, v64 = ref["n"], ref["m64"], ref["v64"]
     std = (v64 + eps).sqrt()
     s1, s2 = sums[:c].double(), sums[c:2 * c].double()
     r = {}
-    r["sums"] = max(sum_check(s1, z64.sum(0), l, z64.abs().sum(0)), sum_check(s2, z64.pow(2).sum(0), l, z64.pow(2).sum(0)))
+    r["sums"] = max(sum_check(s1, ref["s1"], l, ref["a1"]), sum_check(s2, ref["s2"], l, ref["s2"]))
     r["mean"] = float(((mean.double() - m64).abs() / (STAT_TOL * std)).max())
     r["invstd"] = float(((invstd.double() - 1.0 / std).abs() / (STAT_TOL / std)).max())
     # bn_finalize_channel on the kernel's sums: mean = s1 / n (IEEE), var = s2 / n - mean^2 (contracted or not)
-    cnt = torch.tensor(float(n), dtype=torch.float32, device=z.device)
+    cnt = torch.tensor(float(n), dtype=torch.float32, device=device)
     mean_e = sums[:c] / cnt
     q = (sums[c:2 * c] / cnt).double()
     me = mean_e.double()
@@ -115,43 +143,66 @@ def bn_bwd_check(z, d, dz_got, sums_got, mean, invstd, sc, sh, slope, chain, dro
     """float64 BatchNorm backward (batch statistics) through PReLU on the kernel's fp32 statistics, with d = the dy the
     kernel read (fp32).  The PReLU branch is decided by the fp32 u = fma(z, scale, shift) as in the kernel; elements within
     four fp32 ulps of u = 0 are left out of the element-wise dz bound (counted)."""
-    c = z.shape[-1]
-    z64 = z.double().reshape(-1, c)
-    d64 = d.double().reshape(-1, c)
-    n = z64.shape[0]
-    zs = z64 * sc.double()
-    u64 = zs + sh.double()
-    u32 = u64.float().double()
-    pos = u32 > 0
-    near = u64.abs() <= 4 * U * (zs.abs() + sh.double().abs())
-    du = torch.where(pos, d64, d64 * float(slope))
-    zh = (z64 - mean.double()) * invstd.double()
-    duzh = du * zh
-    dbeta, dgamma = du.sum(0), duzh.sum(0)
-    neg = ~pos
-    dslope = (d64 * u32)[neg].sum()
-    a1, a2 = du.abs().sum(0), duzh.abs().sum(0)
-    a_s = (d64 * u32)[neg].abs().sum()
+    r, near = bn_bwd_check_chunked(lambda: [(z, d, dz_got)], z.shape[-1], sums_got, mean, invstd, sc, sh, slope, chain,
+                                   drop_m2)
+    return r, near
+
+
+def bn_bwd_check_chunked(parts, c, sums_got, mean, invstd, sc, sh, slope, chain, drop_m2=False):
+    """bn_bwd_check over image chunks: parts() yields (z, d, dz_got) of each chunk; two passes, the channel sums first"""
+    def terms(z, d):
+        z64 = z.double().reshape(-1, c)
+        d64 = d.double().reshape(-1, c)
+        zs = z64 * sc.double()
+        u64 = zs + sh.double()
+        u32 = u64.float().double()
+        pos = u32 > 0
+        near = u64.abs() <= 4 * U * (zs.abs() + sh.double().abs())
+        du = torch.where(pos, d64, d64 * float(slope))
+        zh = (z64 - mean.double()) * invstd.double()
+        return d64, u32, pos, near, du, zh
+    dbeta = dgamma = a1 = a2 = dslope = a_s = 0.0
+    n = near_n = 0
+    finite = True
+    for z, d, dz_got in parts():
+        d64, u32, pos, near, du, zh = terms(z, d)
+        duzh = du * zh
+        dbeta, dgamma = dbeta + du.sum(0), dgamma + duzh.sum(0)
+        a1, a2 = a1 + du.abs().sum(0), a2 + duzh.abs().sum(0)
+        neg = ~pos
+        dslope = dslope + (d64 * u32)[neg].sum()
+        a_s = a_s + (d64 * u32)[neg].abs().sum()
+        n += du.shape[0]
+        near_n += int(near.sum())
+        finite = finite and bool(torch.isfinite(dz_got).all())
+        del d64, u32, pos, near, du, zh, duzh
     m1 = dbeta / n
     m2 = torch.zeros_like(dgamma) if drop_m2 else dgamma / n
-    want = sc.double() * (du - m1 - zh * m2)
-    t = sc.double().abs() * (8 * U * (du.abs() + m1.abs() + (zh * m2).abs()) + chain["sums"] * U * (a1 + zh.abs() * a2) / n)
-    keep = ~near
-    r = bf16_check(dz_got.reshape(-1, c)[keep], want[keep], 0.0, t[keep])
-    r["finite"] = bool(torch.isfinite(dz_got).all())
+    acc = Acc()
+    for z, d, dz_got in parts():
+        _, _, _, near, du, zh = terms(z, d)
+        want = sc.double() * (du - m1 - zh * m2)
+        t = sc.double().abs() * (8 * U * (du.abs() + m1.abs() + (zh * m2).abs())
+                                 + chain["sums"] * U * (a1 + zh.abs() * a2) / n)
+        keep = ~near
+        acc.add(dz_got.reshape(-1, c)[keep], want[keep], 0.0, t[keep])
+        del near, du, zh, want, t, keep
+    r = acc.result()
+    r["finite"] = finite
     r["dbeta"] = sum_check(sums_got[:c], dbeta, chain["sums"] + 1, a1)
     r["dgamma"] = sum_check(sums_got[c:2 * c], dgamma, chain["sums"] + 3, a2)
     r["dslope"] = float((sums_got[2 * c].double() - dslope).abs() / (chain["slope"] * U * a_s + TINY))
-    return r, int(near.sum())
+    return r, near_n
 
 
-def dy_of(plan, blk, shift=0):
+def dy_of(plan, blk, shift=0, imgs=slice(None)):
     """(dy as bn_act_bwd reads it, fp32 [B, oh, ow, c]; mode): the gy view, the 2x2 sum of the up-sampled gradient in the
-    kernel's order, or the consumer's dxs in place (mode 2).  shift: read the gradient buffer that many channels off."""
+    kernel's order, or the consumer's dxs in place (mode 2).  shift: read the gradient buffer that many channels off;
+    imgs: the images to read."""
     cons = getattr(blk, "dy_s2d", None)
     if cons is not None:
-        return d2s(interior(cons.dxs, 0, cons.xs_cs), blk.cout).float(), 2
-    g = interior(blk.gy.buf, blk.gy.ch_off + shift, blk.cout).float()
+        return d2s(interior(cons.dxs, 0, cons.xs_cs)[imgs], blk.cout).float(), 2
+    g = interior(blk.gy.buf, blk.gy.ch_off + shift, blk.cout)[imgs].float()
     if not blk.fuse_up:
         return g, 0
     s = torch.zeros_like(g[:, ::2, ::2])
@@ -429,9 +480,13 @@ def gather_checks(st, gw_bits=True):
     for blk in plan.blocks:
         r = st.bwd.setdefault(blk.i, {})
         if blk.is_head and blk.owner is None:
-            g = st.g_nhwc[blk.i].double()
+            g = st.g_nhwc[blk.i]
+            s = a = 0.0
+            for b0, b1 in chunks(st.batch, 8 * 3 * g[0].numel(), getattr(st, "budget", None)):
+                g64 = g[b0:b1].double()
+                s, a = s + g64.sum((0, 1, 2)), a + g64.abs().sum((0, 1, 2))
             gb = plan.garena[blk.gb_off:blk.gb_off + blk.cout]
-            r["dbias"] = sum_check(gb, g.sum((0, 1, 2)), head_bias_chain(st.batch, blk.oh, blk.ow), g.abs().sum((0, 1, 2)))
+            r["dbias"] = sum_check(gb, s, head_bias_chain(st.batch, blk.oh, blk.ow), a)
         if not gw_bits:
             continue
         if blk.i == 0:
@@ -446,13 +501,13 @@ def gather_checks(st, gw_bits=True):
 
 
 def run_step(st, cot_seed=None, *, prepare=None, linear_fwd=None, loss=None, head_grads=None,
-             block_check=check_block_bwd, gw_bits=True):
+             block_check=check_block_bwd, gw_bits=True, fwd_check=forward_checks):
     """one checked training step of st.model on st.x.
 
     prepare(st) runs once the checked forward has built st.plan, before any check.  linear_fwd(st, blk) runs right after
     each plan._linear_fwd launch; the plan must exist to be wrapped, so with linear_fwd the checked step follows one
     warm-up step that builds it.  loss(st, ps) gives the loss (default: dense_loss with cot_seed); head_grads and
-    block_check as in backward(); gw_bits as in gather_checks()."""
+    block_check as in backward(); gw_bits as in gather_checks(); fwd_check(st) checks the forward."""
     model = st.model
     t0 = time.time()
     plan = None
@@ -487,13 +542,377 @@ def run_step(st, cot_seed=None, *, prepare=None, linear_fwd=None, loss=None, hea
     by = {b.i: b for b in plan.blocks}
     st.nbt_ok = all(i in by and int(model.module_list[i].BatchNorm2d.num_batches_tracked)
                     == nbt0[i] + (by[i].owner is None and by[i].has_bn) for i in nbt0)
-    forward_checks(st)
+    fwd_check(st)
     torch.cuda.synchronize()
     st.t_fwd = time.time() - t0
     backward(st, loss(st, ps) if loss is not None else dense_loss(st, ps, cot_seed), block_check, head_grads)
     gather_checks(st, gw_bits)
     st.t_total = time.time() - t0
     return st
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the training step at full batch: the same checks over image chunks, nothing of activation size cloned on the device
+def f64_bytes(c_in, c_out, hw_in, hw_out):
+    """float64 working set per image of a tap-sum reference and its check: the padded operand, its |.|, one shifted
+    copy; value, magnitude and about eight temporaries of the result"""
+    return 8 * (3 * c_in * hw_in + 10 * c_out * hw_out)
+
+
+def ref_bytes(blk):
+    """float64 bytes per image of the block's conv, wgrad and dgrad references and their checks"""
+    gh, gw = (blk.src.h // 2, blk.src.w // 2) if blk.s2d else (blk.src.h, blk.src.w)
+    cin = 27 if blk.i == 0 else blk.cin_eff
+    hw = blk.src.h * blk.src.w
+    out = dict(fwd=f64_bytes(cin, blk.cout, (gh + 2) * (gw + 2), blk.oh * blk.ow),
+               wgrad=f64_bytes(cin, blk.cout, (gh + 2) * (gw + 2), gh * gw))
+    if blk.s2d:        # dz zero-inserted on the input grid, then the mirrored 3x3 taps
+        out["dgrad"] = f64_bytes(blk.cout, blk.src.c, hw, hw) + 8 * hw * blk.cout
+    elif blk.i > 0:
+        out["dgrad"] = f64_bytes(blk.cout, blk.cin, hw, hw)
+    return out
+
+
+def _img_bytes(t):
+    return t[0].numel() * t.element_size()
+
+
+class _LeanDot(torch.autograd.Function):
+    """sum(p * G) whose gradient is G itself: no cotangent-sized temporaries"""
+
+    @staticmethod
+    def forward(ctx, p, g):
+        ctx.g = g
+        return sum((p[b] * g[b]).sum() for b in range(p.shape[0]))
+
+    @staticmethod
+    def backward(ctx, go):
+        assert float(go) == 1.0
+        return ctx.g, None
+
+
+def lean_dense_loss(st, ps, seed):
+    """dense_loss with G drawn in the layout of the fp32 head buffers, so that the cotangent the plan receives is G
+    itself (one copy of G on the device, no product or transpose of it)"""
+    gen = torch.Generator().manual_seed(seed)
+    st.g_nhwc = {}
+    loss = 0.0
+    for blk, p in zip(st.plan.heads, ps):
+        b, na, ny, nx, no = p.shape
+        g = torch.randn((b, na * no, ny, nx), generator=gen).to(p.device)
+        st.g_nhwc[blk.i] = g.permute(0, 2, 3, 1)                              # channel a * no + k
+        loss = loss + _LeanDot.apply(p, g.view(b, na, no, ny, nx).permute(0, 1, 3, 4, 2))
+    return loss
+
+
+def _host(t, chunk_list):
+    """t (an image-major device view) copied to host memory chunk by chunk"""
+    return torch.cat([t[b0:b1].cpu() for b0, b1 in chunk_list])
+
+
+def _max_offset(v, buf):
+    """largest element offset into the buffer buf that its view v addresses"""
+    return v.storage_offset() - buf.storage_offset() + sum((s - 1) * d for s, d in zip(v.shape, v.stride()))
+
+
+def forward_checks_chunked(st):
+    """forward_checks over image chunks of at most st.budget float64 bytes: post hoc on the plan's buffers"""
+    plan, model = st.plan, st.model
+    L = _layout()
+    B = st.batch
+    out = {}
+    st.checked_offsets = {}
+    bits = pad = True
+    col = plan.col
+    for b0, b1 in chunks(B, 8 * 27 * st.h * st.w, st.budget):
+        want = F.unfold(st.x[b0:b1], 3, padding=1).view(b1 - b0, 27, st.h, st.w).permute(0, 2, 3, 1).to(BF16)
+        bits = bits and bitwise(interior(col, 0, 27)[b0:b1], want)
+        pad = pad and bool((interior(col, 27, 37)[b0:b1] == 0).all())
+        del want
+    st.checked_offsets["col"] = (col.numel(), _max_offset(interior(col, 27, 37), col))
+    st.im2col = dict(bits=bits, pad_zero=pad, halo=halo_zero(col))
+    packs = []
+    for blk in plan.blocks:
+        w = _weight(model, blk)
+        wf = w.reshape(blk.cout, 27, 1, 1).contiguous() if blk.i == 0 else w
+        packs.append((blk.i, "fwd", torch.equal(blk.pw, L.pack_weights(blk.fdesc, wf, mode=2 if blk.s2d else 0))))
+        if blk.i > 0:
+            packs.append((blk.i, "dgrad", torch.equal(blk.pwd, L.pack_weights(blk.ddesc, w, mode=3 if blk.s2d else 1))))
+    st.packs = packs
+    ratios = []
+    for blk in plan.blocks:
+        assert blk.owner is None
+        r = {}
+        w64 = _weight(model, blk).to(BF16).double()
+        if blk.i == 0:
+            x, taps, s = interior(plan.col, 0, 27), [(0, 0, w64.reshape(blk.cout, 27).t())], 1
+        else:
+            x, taps, s = vint(blk.src), conv_taps(w64), blk.stride
+        n = conv_updates(blk)
+        cl = chunks(B, ref_bytes(blk)["fwd"], st.budget)
+        if blk.is_head:
+            bias = model.module_list[blk.i].Conv2d.bias.detach().double()
+            got = blk.out.detach().permute(0, 2, 3, 1)
+            worst = []
+            for b0, b1 in cl:
+                want, mag = tapsum(x[b0:b1], taps, blk.oh, blk.ow, s)
+                worst.append(f32_check(got[b0:b1], want + bias, n * 2.0 ** -23 * mag)["max"])
+                del want, mag
+            r["z"] = float(torch.tensor(worst, dtype=F64).max())
+            out[blk.i] = r
+            continue
+        z = interior(blk.z, 0, blk.cout)
+        acc = Acc()
+        for b0, b1 in cl:
+            want, mag = tapsum(x[b0:b1], taps, blk.oh, blk.ow, s)
+            acc.add(z[b0:b1], want, n * 2.0 ** -23 * mag)
+            del want, mag
+        rz = acc.result()
+        r["z"], r["z_bias"] = rz["max"], rz["bias"]
+        cz = chunks(B, 8 * 6 * _img_bytes(z), st.budget)
+        if blk.has_bn:
+            bn = _bn_of(model, blk)
+            rs, ratio = stats_ratios(stats_ref_chunked(z, blk.cout, cz), z.device, blk.cout, blk.sums, blk.mean,
+                                     blk.invstd, blk.scale, blk.shift, st.rm0[blk.i], st.rv0[blk.i], bn.running_mean,
+                                     bn.running_var, bn.weight.detach(), bn.bias.detach(), bn.eps, bn.momentum,
+                                     bn_chain(B, blk.oh, blk.ow, blk.cout)["sums"])
+            r.update(rs)
+            r["mean_over_std"] = ratio
+            ratios.append(ratio)
+        else:
+            bias = model.module_list[blk.i].Conv2d.bias.detach()
+            r["fixed_stats"] = bool((blk.scale == 1).all()) and torch.equal(blk.shift, bias)
+        res = vint(blk.res) if blk.res is not None else None
+        y = interior(blk.y.buf, blk.y.ch_off, blk.cout)
+        acc, copies = Acc(), True
+        for b0, b1 in cz:
+            want_y, t = bn_act_fwd_ref(z[b0:b1], blk.scale, blk.shift, slope_of(model, blk),
+                                       res[b0:b1] if res is not None else None)
+            yc = y[b0:b1]
+            if blk.fuse_up:
+                base = yc[:, ::2, ::2]
+                copies = copies and all(bitwise(yc[:, ry::2, rx::2], base) for ry in range(2) for rx in range(2))
+                yc = base
+            acc.add(yc, want_y, 0.0, t)
+            del want_y, t
+        ry_ = acc.result()
+        r["y"], r["y_bias"] = ry_["max"], ry_["bias"]
+        if blk.fuse_up:
+            r["up_copies"] = copies
+        out[blk.i] = r
+    for blk in plan.blocks:
+        if blk.s2d:
+            src = vint(blk.src)
+            xs = interior(blk.xs, 0, 4 * blk.src.c)
+            out[blk.i]["xs"] = all(bitwise(xs[b0:b1], s2d(src[b0:b1])) for b0, b1 in chunks(B, 4 * _img_bytes(xs), st.budget))
+    bufs = {}
+    for blk in plan.blocks:
+        for v in (blk.src, blk.y if not blk.is_head else None):
+            if v is not None and v.buf is not None:
+                bufs[id(v.buf)] = v.buf
+        if not blk.is_head:
+            bufs[id(blk.z)] = blk.z
+        if blk.s2d:
+            bufs[id(blk.xs)] = blk.xs
+    st.fwd_halo = all(halo_zero(b) for b in bufs.values())
+    st.fwd = out
+    st.max_ratio = max(ratios)
+
+
+def _overlap(a, b):
+    return a is not None and b is not None and a.buf is b.buf and a.ch_off < b.ch_off + b.c and b.ch_off < a.ch_off + a.c
+
+
+def check_block_bwd_chunked(st, blk, orig):
+    """check_block_bwd over image chunks: before the block, only what it overwrites and later checks read goes to host
+    memory (z, which becomes dz in place; the prior of an accumulated gradient view; the channels of a shared gradient
+    buffer outside the block's views); dy is read after the block from buffers the block does not write"""
+    B = st.batch
+    r, snap = {}, {}
+    try:
+        if not blk.is_head:
+            z = interior(blk.z, 0, blk.cout)
+            snap["z"] = _host(z, chunks(B, _img_bytes(z), st.budget))
+            assert not _overlap(blk.gy, blk.gsrc) and not _overlap(blk.gy, blk.gres) and blk.gy.buf is not blk.z
+            if blk.gres is not None and blk.gres_acc:
+                snap["gres_prior"] = _host(vint(blk.gres), chunks(B, _img_bytes(vint(blk.gres)), st.budget))
+        if blk.gsrc is not None:
+            gbuf = blk.gsrc.buf
+            if blk.gsrc_acc:
+                snap["prior"] = _host(vint(blk.gsrc), chunks(B, _img_bytes(vint(blk.gsrc)), st.budget))
+            allowed = torch.zeros(gbuf.shape[-1], dtype=torch.bool)
+            allowed[blk.gsrc.ch_off:blk.gsrc.ch_off + blk.gsrc.c] = True
+            if blk.gres is not None and blk.gres.buf is gbuf:
+                allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
+            snap["outside"] = (~allowed).nonzero().flatten().to(gbuf.device)
+            if len(snap["outside"]):
+                snap["gbuf_outside"] = torch.cat([gbuf[b0:b1].index_select(3, snap["outside"]).cpu()
+                                                  for b0, b1 in chunks(B, _img_bytes(gbuf), st.budget)])
+    except Exception:
+        r["error"] = traceback.format_exc()
+    orig(blk)
+    if "error" in r:
+        return r
+    try:
+        _bwd_checks_chunked(st, blk, snap, r)
+    except Exception:
+        r["error"] = traceback.format_exc()
+    return r
+
+
+def _bwd_checks_chunked(st, blk, snap, r):
+    plan, model = st.plan, st.model
+    B = st.batch
+    dev = st.x.device
+    w64 = _weight(model, blk).to(BF16).double()
+    if blk.is_head:
+        dz = interior(blk.dz, 0, blk.cout)
+        g = st.g_nhwc[blk.i]
+        r["dz_bits"] = all(bitwise(dz[b0:b1], g[b0:b1].to(BF16)) for b0, b1 in chunks(B, 4 * _img_bytes(dz), st.budget))
+        r["dz_pad_zero"] = bool((blk.dz[..., blk.cout:] == 0).all()) and halo_zero(blk.dz)
+    else:
+        dz = interior(blk.z, 0, blk.cout)
+        _, r["dy_mode"] = dy_of(plan, blk, imgs=slice(0, 1))
+        rpp = 2 if r["dy_mode"] == 2 and blk.cout // 8 * 2 <= 640 else 1
+        chain = bn_chain(B, blk.oh, blk.ow, blk.cout, rpp)
+        cl = chunks(B, 8 * 12 * blk.oh * blk.ow * blk.cout, st.budget)
+
+        def parts():
+            for b0, b1 in cl:
+                yield snap["z"][b0:b1].to(dev), dy_of(plan, blk, imgs=slice(b0, b1))[0], dz[b0:b1]
+        rb, near = bn_bwd_check_chunked(parts, blk.cout, blk.bsums, blk.mean, blk.invstd, blk.scale, blk.shift,
+                                        slope_of(model, blk), chain)
+        r["dz"], r["dz_bias"] = rb["max"], rb["bias"]
+        for k in ("dbeta", "dgamma", "dslope", "finite"):
+            r[k] = rb[k]
+        r["near_zero_u"] = near
+        r["n_elems"] = dz.numel()
+        if blk.gres is not None:
+            gres = vint(blk.gres)
+            ok = True
+            for b0, b1 in cl:
+                d = dy_of(plan, blk, imgs=slice(b0, b1))[0]
+                want = (snap["gres_prior"][b0:b1].to(dev).float() + d).to(BF16) if blk.gres_acc else d.to(BF16)
+                ok = ok and bitwise(gres[b0:b1], want)
+            r["gres_bits"] = ok
+        r["dz_halo"] = halo_zero(blk.z)
+    # weight gradient: the float64 reference summed over image chunks
+    if blk.i == 0:
+        x, offs, cin = interior(plan.col, 0, 27), [(0, 0)], 27
+    elif blk.s2d:
+        x, cin = interior(blk.xs, 0, blk.cin_eff), blk.cin_eff
+        offs = [(qy - 1, qx - 1) for qy in range(2) for qx in range(2)]
+    else:
+        x, cin = vint(blk.src), blk.cin
+        p = (blk.k - 1) // 2
+        offs = [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)]
+    gh, gw_ = x.shape[1], x.shape[2]
+    wr = wm = 0.0
+    for b0, b1 in chunks(B, ref_bytes(blk)["wgrad"], st.budget):
+        a, m = wgrad_ref(x[b0:b1], dz[b0:b1], offs)
+        wr, wm = wr + a, wm + m
+        del a, m
+    plan_w = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, B, gh, gw_, gemm_sms())
+    got = blk.dw[:, :blk.cout, :cin]
+    r["wgrad"] = wgrad_ratio(got, wr, wm, plan_w)
+    r["wgrad_rw"] = worst_ratio(got, wr, wm, plan_w["n_add"])
+    if blk.i in st.keep_bwd:
+        st.stash[("wgrad", blk.i)] = dict(x=x.clone(), dz=dz.clone(), offs=offs, got=got.clone(), plan=plan_w,
+                                          want=wr, mag=wm)
+    del wr, wm
+    if blk.i == 0:
+        return
+    gbuf = blk.gsrc.buf
+    if blk.s2d:
+        dxs = interior(blk.dxs, 0, blk.cin_eff)
+        n = 4 * rup(blk.cout, 64) // 16
+        acc, bits = Acc(), True
+        for b0, b1 in chunks(B, ref_bytes(blk)["dgrad"], st.budget):
+            want, mag = s2d_dgrad_ref(dz[b0:b1], w64, blk.src.h, blk.src.w)
+            acc.add(dxs[b0:b1], want, n * 2.0 ** -23 * mag)
+            del want, mag
+            if not blk.dxs_direct:
+                v = d2s(dxs[b0:b1], blk.src.c)
+                want_bits = (snap["prior"][b0:b1].to(dev).float() + v.float()).to(BF16) if blk.gsrc_acc else v
+                bits = bits and bitwise(vint(blk.gsrc)[b0:b1], want_bits)
+        rd = acc.result()
+        r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
+        if not blk.dxs_direct:
+            r["d2s_bits"] = bits
+    else:
+        got = vint(blk.gsrc)
+        n = blk.k * blk.k * rup(blk.cout, 64) // 16
+        acc = Acc()
+        for b0, b1 in chunks(B, ref_bytes(blk)["dgrad"], st.budget):
+            want, mag = tapsum(dz[b0:b1], conv_taps(w64, mirror=True), blk.src.h, blk.src.w)
+            e, t = n * 2.0 ** -23 * mag, 0.0
+            if blk.gsrc_acc:
+                prior = snap["prior"][b0:b1].to(dev).double()
+                want = want + prior
+                t = U * (mag + prior.abs())
+                del prior
+            acc.add(got[b0:b1], want, e, t)
+            del want, mag, e, t
+        rd = acc.result()
+        r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
+    same = True
+    if len(snap["outside"]):
+        for b0, b1 in chunks(B, _img_bytes(gbuf), st.budget):
+            same = same and torch.equal(gbuf[b0:b1].index_select(3, snap["outside"]).cpu(), snap["gbuf_outside"][b0:b1])
+    r["outside_untouched"] = same and halo_zero(gbuf)
+
+
+def run_step_chunked(st, cot_seed, budget, prepare=None):
+    """run_step at a batch whose activations fill the card: forward_checks_chunked, lean_dense_loss and
+    check_block_bwd_chunked, every float64 working set within `budget` bytes"""
+    st.budget = budget
+    return run_step(st, cot_seed, prepare=prepare, loss=lambda s, ps: lean_dense_loss(s, ps, cot_seed),
+                    block_check=check_block_bwd_chunked, fwd_check=forward_checks_chunked)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# the training step's launch schedules, from the plan's geometry
+def plan_layout(model, batch, h, w, device="cpu", shared=None):
+    """a TrainPlan laid out without storage (every activation a stride-0 stand-in of its shape) and the activation-pool
+    bytes it needs: the geometry of every launch, on any machine"""
+    from rotate_yolov3_b200.pool import ActivationPool
+    from rotate_yolov3_b200.train_path import TrainPlan
+    pool = ActivationPool(device)
+    plan, need, _ = pool._layout(lambda: TrainPlan(model, batch, h, w, torch.device(device), pool,
+                                                   {} if shared is None else shared))
+    return plan, need
+
+
+def schedule_rows(plan, sms):
+    """per block of the training step, what its launches derive from the shape: the forward and dgrad conv (tiles, CTAs,
+    tiles per CTA against the staging ring), the split-K wgrad plan, the BN pieces of bn_stats / bn_act_bwd, the head-bias
+    blocks, and the largest element offset into any buffer the block's kernels address"""
+    B = plan.batch
+    rows = []
+    for blk in plan.blocks:
+        gh, gw = (blk.src.h // 2, blk.src.w // 2) if blk.s2d else (blk.src.h, blk.src.w)
+        np_ = B * (gh + 2) * (gw + 2)
+        r = dict(i=blk.i, kind="head" if blk.is_head else ("s2d" if blk.s2d else "k%d" % blk.k), grid=(blk.oh, blk.ow),
+                 fwd=conv_schedule(np_, blk.cout, False, sms))
+        if blk.i > 0:
+            r["dgrad"] = conv_schedule(np_, blk.cin_eff, bool(blk.gsrc_acc) and not blk.s2d, sms)
+        r["wgrad"] = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, B, gh, gw, sms)
+        if blk.is_head:
+            r["head_bias"] = head_bias_blocks(B, blk.oh)
+            bufs = [blk.src.buf, blk.dz, blk.out]
+        else:
+            rpp = 2 if getattr(blk, "dy_s2d", None) is not None and blk.cout // 8 * 2 <= 640 else 1
+            r["bn_fwd"] = bn_pieces(B, blk.oh, blk.ow, blk.cout, 1, sms)
+            r["bn_bwd"] = bn_pieces(B, blk.oh, blk.ow, blk.cout, rpp, sms)
+            bufs = [blk.src.buf, blk.z, blk.y.buf, blk.gy.buf]
+        bufs += [plan.col if blk.i == 0 else blk.gsrc.buf]
+        if blk.s2d:
+            bufs += [blk.xs, blk.dxs]
+        if getattr(blk, "dz_up", None) is not None:
+            bufs.append(blk.dz_up)
+        r["max_offset"] = max(b.numel() for b in bufs if b is not None) - 1
+        rows.append(r)
+    return rows
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -519,8 +938,10 @@ class Acc:
                 "bias": abs(self.es / self.n) / (BIAS_TOL * rms + TINY)}
 
 
-def chunks(batch, bytes_per_image):
-    per = max(1, min(batch, int(CHUNK_BYTES // bytes_per_image)))
+def chunks(batch, bytes_per_image, budget=None):
+    """[b0, b1) image ranges covering the batch, each within `budget` bytes (default CHUNK_BYTES) at bytes_per_image, or
+    one image when one image alone needs more"""
+    per = max(1, min(batch, int((budget or CHUNK_BYTES) // bytes_per_image)))
     return [(b, min(batch, b + per)) for b in range(0, batch, per)]
 
 

@@ -316,8 +316,9 @@ def bad_entries(d, skip=("dy_mode", "near_zero_u", "n_elems", "wgrad_rw", "mean_
 
 # ---------------------------------------------------------------------------------------------------------------
 # reduction chain lengths
-def bn_chain(batch, h, w, c, rows_per_piece=1):
-    """bn_stats / bn_act_bwd (mirror of mk_pieces in bnpipe.cuh)"""
+def bn_pieces(batch, h, w, c, rows_per_piece=1, sms=None):
+    """the piece schedule of bn_stats / bn_act_bwd (mirror of mk_pieces in bnpipe.cuh): pieces of `px` pixels of
+    `rows_per_piece` rows, `per_cta` of them per CTA of a `grid`-CTA launch"""
     cgs = c // 8
     max_px = 1280 // rows_per_piece // cgs
     if rows_per_piece == 2:
@@ -327,17 +328,38 @@ def bn_chain(batch, h, w, c, rows_per_piece=1):
     if rows_per_piece == 2 and px % 2:
         px += 1
     total = batch * (h // rows_per_piece) * ppr
-    per_cta = cdiv(total, 2 * gemm_sms())
-    grid = cdiv(total, per_cta)
-    per_thread = per_cta * cdiv(px * cgs, 256) * rows_per_piece
-    rows = cdiv(grid, 8) + 8
-    return dict(sums=per_thread + 256 // cgs + rows, slope=8 * per_thread + 5 + 8 + rows)
+    per_cta = cdiv(total, 2 * (sms or gemm_sms()))
+    return dict(px=px, total=total, per_cta=per_cta, grid=cdiv(total, per_cta), rows=rows_per_piece)
+
+
+def bn_chain(batch, h, w, c, rows_per_piece=1, sms=None):
+    """bn_stats / bn_act_bwd: the longest fp32 addition chains of the channel sums and of d slope"""
+    pg = bn_pieces(batch, h, w, c, rows_per_piece, sms)
+    per_thread = pg["per_cta"] * cdiv(pg["px"] * (c // 8), 256) * rows_per_piece
+    rows = cdiv(pg["grid"], 8) + 8
+    return dict(sums=per_thread + 256 // (c // 8) + rows, slope=8 * per_thread + 5 + 8 + rows)
+
+
+def head_bias_blocks(batch, ny):
+    """head_grad_nchw_kernel: (rows per block, blocks)"""
+    rpb = max(1, cdiv(ny * batch, 2048))
+    return rpb, cdiv(ny, rpb) * batch
 
 
 def head_bias_chain(batch, ny, nx):
-    rpb = max(1, cdiv(ny * batch, 2048))
-    blocks = cdiv(ny, rpb) * batch
+    rpb, blocks = head_bias_blocks(batch, ny)
     return 5 + rpb * cdiv(nx, 32) + cdiv(blocks, 8) + 8 + 1
+
+
+def conv_schedule(np_, cout, res, sms=None):
+    """the persistent implicit-GEMM launch (conv.cu conv_geom / launch_conv / ConvSmem) over np_ padded pixels: its
+    tiles, grid and tiles per CTA, the operand ring and the output staging tiles a CTA cycles through"""
+    bn = 256 if cout > 128 else (128 if cout > 64 else 64)
+    tiles = cdiv(np_, 128) * (rup(cout, bn) // bn)
+    grid = min(tiles, sms or gemm_sms())
+    return dict(bn=bn, tiles=tiles, grid=grid, per_cta=cdiv(tiles, grid),
+                stages=3 if bn == 256 else ((5 if res else 6) if bn == 128 else 8),
+                staging=2 if res and bn < 256 else 1, m_tail=np_ % 128)
 
 
 def se_chain(h, w, c):

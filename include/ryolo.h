@@ -606,7 +606,9 @@ int ryolo_augment_finish(const ryolo_finish_job* jobs_dev, int njobs, const uint
  * max_blocks >= blocks of any image (mcux * mcuy * bpm), max_out_h >= out rows of any image.
  * status[i] is set to a nonzero RYOLO_JPEG_ST_* mask when image i cannot be decoded on the device (a code not
  * in its table, a coefficient run past the block, data ending before the last block, a chunk that does not
- * synchronise); its output is then unspecified.  Every read stays inside its segment.
+ * synchronise, a block whose dequantised coefficients or samples leave the range where libjpeg-turbo's C and SIMD
+ * IDCTs agree); its output is then unspecified.  Every read stays inside its segment.  The pixel stage adds its
+ * bit to what the entropy stage left in status.
  * stages: RYOLO_JPEG_ENTROPY (status, coefficients), RYOLO_JPEG_PIXELS (IDCT, upsampling, colour, store) or both;
  * the second reads the coefficients the first left in the workspace.  image_bytes: the size of the image area
  * the images' coef_off / plane_off point into.  Allocates nothing; capturable in a CUDA graph; data < 4 GiB.
@@ -619,6 +621,7 @@ int ryolo_augment_finish(const ryolo_finish_job* jobs_dev, int njobs, const uint
 #define RYOLO_JPEG_ST_BAD_CODE 1  /* a code not in its table, or a run past coefficient 63          */
 #define RYOLO_JPEG_ST_TRUNCATED 2 /* the segment ends before its last block                         */
 #define RYOLO_JPEG_ST_NO_SYNC 4   /* a chunk on the decode path did not synchronise                 */
+#define RYOLO_JPEG_ST_RANGE 8     /* a block outside the range where every libjpeg-turbo IDCT agrees  */
 typedef struct ryolo_jpeg_image {
   int64_t out_off;      /* byte offset of the [out_h, out_w, 3] BGR image in out                              */
   int64_t coef_off;     /* byte offset in the image area of the int16 coefficient blocks, in decode order      */

@@ -14,7 +14,8 @@
 //   write     each chunk on the chain decodes its range again and stores the coefficients; every coefficient position
 //             of every block is written by exactly one thread.
 //   DC        one CTA per (segment, component) turns DC differences into values by a prefix sum.
-// Pixel stage: one thread per block dequantises and runs the ISLOW IDCT into the component planes; one CTA per output
+// Pixel stage: one thread per block dequantises and runs the ISLOW IDCT into the component planes, and flags a block
+// outside the range where libjpeg-turbo's IDCTs agree (RYOLO_JPEG_ST_RANGE); one CTA per output
 // row upsamples, converts the colour and stores B, G, R with the Exif orientation applied.
 #include "common.cuh"
 #include "jpeg.cuh"
@@ -184,7 +185,7 @@ __global__ void __launch_bounds__(kDcThreads)
 
 __global__ void __launch_bounds__(kIdctThreads)
     jpeg_idct_kernel(const ryolo_jpeg_image* __restrict__ images, const uint16_t* __restrict__ quant,
-                     uint8_t* __restrict__ area) {
+                     uint8_t* __restrict__ area, int32_t* __restrict__ status) {
   const ryolo_jpeg_image& im = images[blockIdx.y];
   const int64_t b = (int64_t)blockIdx.x * kIdctThreads + threadIdx.x;
   if (b >= (int64_t)im.mcux * im.mcuy * im.bpm) return;
@@ -198,7 +199,9 @@ __global__ void __launch_bounds__(kIdctThreads)
 #pragma unroll
   for (int i = 0; i < 8; i++) blk.v[i] = src[i];
   const int pitch = im.pitch[ci];
-  jpeg::idct_islow(blk.s, quant + im.qtab[ci], area + im.plane_off[ci] + (int64_t)row * pitch + col, pitch);
+  const int st =
+      jpeg::idct_islow(blk.s, quant + im.qtab[ci], area + im.plane_off[ci] + (int64_t)row * pitch + col, pitch);
+  if (st) atomicOr(status + blockIdx.y, st);
 }
 
 __global__ void __launch_bounds__(kPixThreads)
@@ -260,9 +263,9 @@ extern "C" int ryolo_jpeg_decode(const ryolo_jpeg_image* images, int nimages, co
     RYOLO_LAUNCH_CHECK();
   }
   if (stages & RYOLO_JPEG_PIXELS) {
-    RYOLO_ARG_CHECK(quant && out && max_blocks > 0 && max_out_h > 0);
+    RYOLO_ARG_CHECK(quant && out && status && max_blocks > 0 && max_out_h > 0);
     jpeg_idct_kernel<<<dim3((max_blocks + kIdctThreads - 1) / kIdctThreads, nimages), kIdctThreads, 0, stream>>>(
-        images, quant, area);
+        images, quant, area, status);
     RYOLO_LAUNCH_CHECK();
     jpeg_pixels_kernel<<<dim3(max_out_h, nimages), kPixThreads, 0, stream>>>(images, area, out);
     RYOLO_LAUNCH_CHECK();

@@ -5,9 +5,9 @@
 //   entropy    jdhuff.c decode_mcu: canonical Huffman codes (HUFF_DECODE), HUFF_EXTEND of the extra bits, (run, size)
 //              AC symbols with EOB and ZRL; 0xFF00 byte stuffing is skipped by the bit reader.  Reads past the end of
 //              a segment see zero bits, as libjpeg's fill_bit_buffer supplies them.
-//   IDCT       jidctint.c jpeg_idct_islow: 13-bit constants, PASS1_BITS 2, 64-bit products, rounding descale, and
-//              the output through IDCT_range_limit: index masked to 10 bits (RANGE_MASK), then the table, which is
-//              a saturation of the sign-wrapped index plus 128.
+//   IDCT       jidctint.c jpeg_idct_islow: 13-bit constants, PASS1_BITS 2, 64-bit products, rounding descale, the
+//              output plus 128 saturated; a block outside the range where that equals every libjpeg-turbo IDCT gets
+//              RYOLO_JPEG_ST_RANGE (idct_islow below).
 //   upsample   jdsample.c: h2v1 / h2v2 fancy (triangle) upsampling when the component is wider than 2 samples
 //              (box replication otherwise), h1v2 fancy, 4:1:1 box; first / last column replicated; context rows
 //              replicated at the top and at the last real row (jdmainct.c set_bottom_pointers).
@@ -286,33 +286,68 @@ RJ_HD int64_t dc_block(const ryolo_jpeg_image& im, const ryolo_jpeg_segment& sg,
 // Dequantisation and the ISLOW IDCT (jidctint.c)
 // ---------------------------------------------------------------------------------------------------------------------
 
-RJ_HD int range_limit(int64_t x, int shift) {
-  const int idx = (int)(int32_t)((x + ((int64_t)1 << (shift - 1))) >> shift) & 1023;
-  const int v = (idx < 512 ? idx : idx - 1024) + 128;
-  return v < 0 ? 0 : (v > 255 ? 255 : v);
+// Which IDCT cv2 runs depends on its libjpeg-turbo build: the C jidctint.c (64-bit products, and the output through a
+// range-limit table indexed with a 10-bit wrap) or, with SIMD, jidctint-sse2 / -avx2 (dequantisation and both passes'
+// inputs and outputs in 16-bit lanes with 32-bit products, the output saturated).  The two compute the same integers,
+// and this function computes them too, only while a block stays in the range real 8-bit pixels produce.  A block
+// whose dequantised coefficients or output leave it (a corrupt stream, an odd encoder) is decoded differently by the
+// two, so idct_islow returns RYOLO_JPEG_ST_RANGE for it and the image goes to the host decoder.  The predicate:
+//
+//   (a) every column c of dequantised coefficients F[u][c] = coef * q has  2 |F[0][c]| + 3 sum_{u>=1} |F[u][c]| <= 8192
+//   (b) every output value x (the pass-2 sum after its descale, before the + 128) lies in [-512, 511].
+//
+// Why it suffices.  Pass 1 is linear before its rounding: ws[n][c] = (sum_u M[n][u] F[u][c] + 2^10) >> 11, M the 8x8
+// integer matrix of the butterflies.  |M[n][0]| = 2^13 and |M[n][u]| <= 11387 = 1.39 * 2^13 for u >= 1 (sqrt 2
+// cos(pi / 16) = 1.387; tests/test_jpeg_syntax_cpu.py restates pass 1, builds M and checks both).  With 2 * 1.39 <= 3,
+// (a) gives |F[0][c]| + 1.39 sum_{u>=1} |F[u][c]| <= 4096, so
+//   |ws[n][c]| <= 4 * 4096 + 1 = 16385,  half of int16,  and every |F| <= 4096,  an eighth of it:
+// no 16-bit lane wraps or saturates in dequantisation or pass 1.  Pass 2's sums are at most 8 * 16385 * 11387 <
+// 1.5e9, inside int32, so every path holds the same x.  By (b), x + 128 through the 10-bit wrap is x + 128 itself, and
+// the table and the SIMD saturation give the same byte.  (b) is needed besides (a): a bound on the coefficients alone
+// that implies it (sum of |F| weighted by the IDCT's largest gains, or |F[0][0]| / 8 plus the AC energy) reaches past
+// 600 on the noisy q100 test pictures, whose outputs stay inside [-128, 127].
+constexpr int kIdctColumnLimit = 8192;
+constexpr int kIdctOutMin = -512, kIdctOutMax = 511;
+
+RJ_HD int min_abs(int v, int cap) {
+  const int a = v < 0 ? -v : v;
+  return a < cap ? a : cap;
 }
 
-// coef: 64 coefficients in natural order, q: the quantisation table in natural order; out: 8 rows of `pitch` bytes
-RJ_HD void idct_islow(const int16_t* coef, const uint16_t* q, uint8_t* out, int pitch) {
+// the rounding descale of a pass-2 sum; out of [kIdctOutMin, kIdctOutMax] sets *bad.  The descaled value is taken in
+// 32 bits: under (a) it is below 1.5e9 / 2^18 in magnitude, and a block breaking (a) is flagged whatever it wraps to.
+RJ_HD int descale_out(int64_t x, int shift, bool& bad) {
+  const int v = (int)((x + ((int64_t)1 << (shift - 1))) >> shift);
+  bad |= (unsigned)(v - kIdctOutMin) > (unsigned)(kIdctOutMax - kIdctOutMin);
+  return v < -128 ? 0 : (v > 127 ? 255 : v + 128);
+}
+
+// coef: 64 coefficients in natural order, q: the quantisation table in natural order; out: 8 rows of `pitch` bytes.
+// Returns 0, or RYOLO_JPEG_ST_RANGE when the block breaks the predicate above (out then holds saturated values).
+RJ_HD int idct_islow(const int16_t* coef, const uint16_t* q, uint8_t* out, int pitch) {
   constexpr int CB = 13, P1 = 2;
   int ws[64];
+  bool bad = false;
 #pragma unroll
   for (int c = 0; c < 8; c++) {
     int64_t z1, z2, z3, z4, z5, t0, t1, t2, t3, t10, t11, t12, t13;
-    z2 = (int64_t)((int)coef[16 + c] * (int)q[16 + c]);
-    z3 = (int64_t)((int)coef[48 + c] * (int)q[48 + c]);
+    int f[8];
+#pragma unroll
+    for (int u = 0; u < 8; u++) f[u] = (int)coef[8 * u + c] * (int)q[8 * u + c];
+    // in 32 bits: each |f| capped at the limit (a capped term alone breaks it) keeps the sum below 2^18
+    int col = 2 * min_abs(f[0], kIdctColumnLimit);
+#pragma unroll
+    for (int u = 1; u < 8; u++) col += 3 * min_abs(f[u], kIdctColumnLimit);
+    bad |= col > kIdctColumnLimit;
+    z2 = f[2], z3 = f[6];
     z1 = (z2 + z3) * 4433;
     t2 = z1 + z3 * -15137;
     t3 = z1 + z2 * 6270;
-    z2 = (int64_t)((int)coef[c] * (int)q[c]);
-    z3 = (int64_t)((int)coef[32 + c] * (int)q[32 + c]);
+    z2 = f[0], z3 = f[4];
     t0 = (z2 + z3) * ((int64_t)1 << CB);
     t1 = (z2 - z3) * ((int64_t)1 << CB);
     t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
-    t0 = (int64_t)((int)coef[56 + c] * (int)q[56 + c]);
-    t1 = (int64_t)((int)coef[40 + c] * (int)q[40 + c]);
-    t2 = (int64_t)((int)coef[24 + c] * (int)q[24 + c]);
-    t3 = (int64_t)((int)coef[8 + c] * (int)q[8 + c]);
+    t0 = f[7], t1 = f[5], t2 = f[3], t3 = f[1];
     z1 = t0 + t3, z2 = t1 + t2, z3 = t0 + t2, z4 = t1 + t3;
     z5 = (z3 + z4) * 9633;
     t0 *= 2446, t1 *= 16819, t2 *= 25172, t3 *= 12299;
@@ -350,15 +385,16 @@ RJ_HD void idct_islow(const int16_t* coef, const uint16_t* q, uint8_t* out, int 
     t0 += z1 + z3, t1 += z2 + z4, t2 += z2 + z3, t3 += z1 + z4;
     constexpr int sh = CB + P1 + 3;
     uint8_t* o = out + (int64_t)r * pitch;
-    o[0] = (uint8_t)range_limit(t10 + t3, sh);
-    o[7] = (uint8_t)range_limit(t10 - t3, sh);
-    o[1] = (uint8_t)range_limit(t11 + t2, sh);
-    o[6] = (uint8_t)range_limit(t11 - t2, sh);
-    o[2] = (uint8_t)range_limit(t12 + t1, sh);
-    o[5] = (uint8_t)range_limit(t12 - t1, sh);
-    o[3] = (uint8_t)range_limit(t13 + t0, sh);
-    o[4] = (uint8_t)range_limit(t13 - t0, sh);
+    o[0] = (uint8_t)descale_out(t10 + t3, sh, bad);
+    o[7] = (uint8_t)descale_out(t10 - t3, sh, bad);
+    o[1] = (uint8_t)descale_out(t11 + t2, sh, bad);
+    o[6] = (uint8_t)descale_out(t11 - t2, sh, bad);
+    o[2] = (uint8_t)descale_out(t12 + t1, sh, bad);
+    o[5] = (uint8_t)descale_out(t12 - t1, sh, bad);
+    o[3] = (uint8_t)descale_out(t13 + t0, sh, bad);
+    o[4] = (uint8_t)descale_out(t13 - t0, sh, bad);
   }
+  return bad ? RYOLO_JPEG_ST_RANGE : 0;
 }
 
 // plane position of block b (decode order) of an image: component, first row, first column

@@ -7,8 +7,9 @@ uploads them with the compressed bytes in one pinned staging copy.  The device d
 streams with one interleaved scan of 1 or 3 components, sampled 4:4:4, 4:2:2, 4:2:0, 4:4:0 or 4:1:1, with any restart
 interval (``ryolo_jpeg_decode``; the arithmetic is in ``csrc/jpeg.cuh``).  Every other stream -- progressive,
 arithmetic-coded, 12-bit, lossless, CMYK / YCCK, multi-scan, or one the parser does not accept -- is decoded on the
-host by ``cv2.imdecode`` and uploaded into the same output slot, and so is a stream the device finds corrupt.  The
-route each image took is returned with it."""
+host by ``cv2.imdecode`` and uploaded into the same output slot, and so is a stream the device finds corrupt or
+whose coefficients leave the range where libjpeg-turbo's C and SIMD IDCTs agree.  The route each image took is
+returned with it."""
 import functools
 
 import numpy as np
@@ -20,6 +21,7 @@ from .preprocess import _pinned, _staging
 DEFAULT_CHUNK_BYTES = 128
 DEVICE = "device"
 YCC, RGB, GRAY = 0, 1, 2                  # RYOLO_JPEG_YCC / RGB / GRAY
+ST_BAD_CODE, ST_TRUNCATED, ST_NO_SYNC, ST_RANGE = 1, 2, 4, 8      # RYOLO_JPEG_ST_*
 
 _NATURAL = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20,
                      13, 6, 7, 14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52,
@@ -448,8 +450,15 @@ class Batch:
                     raise ValueError("decode_images: image %d decodes to %s on the host, its header says %s"
                                      % (i, img.shape, tuple(self.images[i].shape)))
                 self.images[i].copy_(torch.from_numpy(img))
-                self.routes[i] = "host: corrupt entropy-coded data (status %d)" % int(status[j])
+                self.routes[i] = "host: %s (status %d)" % (status_reason(int(status[j])), int(status[j]))
         return self.images, self.routes
+
+
+def status_reason(st):
+    """why the device handed an image back, from its RYOLO_JPEG_ST_* mask"""
+    if st & (ST_BAD_CODE | ST_TRUNCATED | ST_NO_SYNC):
+        return "corrupt entropy-coded data"
+    return "coefficients outside the IDCT's exact range"
 
 
 def _align(n, a=16):

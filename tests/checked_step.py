@@ -11,20 +11,26 @@ batch whose activations fill the card (test_train_scale_f64_gpu.py): over image 
 block overwrites.  schedule_rows mirrors what each launch's schedule derives from the shape, from a plan built or only
 laid out (plan_layout).
 
-Eval forward (map_plan, check_first, check_conv, check_s2d_step, check_buffers): the steps of the eval plan mapped to the
-graph's layers and every conv launch checked on its own input buffers; the bounds are stated in
+Squeeze-excitation: forward_checks checks ryolo_se_fwd's m, p, s and u post hoc; plan._se_bwd is wrapped as well
+(check_se_bwd), because the SE backward runs inside its producing block's _backward_block, right before that block's
+bn_act_bwd reads gx: the wrapper checks the SE on its own inputs and hands check_block_bwd the gx the SE left.  The SE
+bounds are stated in test_se_f64_gpu.py.
+
+Eval forward (map_plan, check_first, check_conv, check_s2d_step, check_se_step, check_buffers): the steps of the eval
+plan mapped to the graph's layers and every conv launch checked on its own input buffers; the bounds are stated in
 test_detect_forward_f64_gpu.py."""
 import time
 import traceback
+import types
 
 import torch
 import torch.nn.functional as F
 
 from builders import ryolo_lib
-from f64_refs import (BF16, BIAS_TOL, F64, STAT_TOL, TINY, U, bf16_check, bitwise, bn_act_fwd_ref, bn_chain, bn_pieces,
-                      check_z, conv_schedule, conv_taps, d2s, f32_check, gemm_sms, halo_zero, head_bias_blocks,
-                      head_bias_chain, interior, rup, s2d, s2d_dgrad_ref, sum_check, tapsum, vint, wgrad_ratio, wgrad_ref,
-                      worst_ratio)
+from f64_refs import (BF16, BIAS_TOL, F64, HALF_BF16, STAT_TOL, TINY, U, bf16_check, bitwise, bn_act_fwd_ref, bn_chain,
+                      bn_pieces, check_z, conv_schedule, conv_taps, d2s, f32_check, gemm_sms, halo_zero, head_bias_blocks,
+                      head_bias_chain, interior, ratio, rup, s2d, s2d_dgrad_ref, se_block_s_ref, se_bwd_refs, se_fwd_ratios,
+                      sum_check, tapsum, vint, wgrad_ratio, wgrad_ref, worst_ratio)
 from helpers import wgrad_plan
 
 
@@ -41,7 +47,7 @@ class Step:
     def __init__(self, model, x):
         self.model, self.x = model, x
         self.batch, _, self.h, self.w = x.shape
-        self.stash, self.keep_fwd, self.keep_bwd = {}, set(), set()
+        self.stash, self.keep_fwd, self.keep_bwd, self.keep_se = {}, set(), set(), set()
 
 
 def _bn_of(model, blk):
@@ -287,6 +293,13 @@ def forward_checks(st):
     for blk in plan.blocks:
         if blk.s2d:
             out[blk.i]["xs"] = bitwise(interior(blk.xs, 0, 4 * blk.src.c), s2d(vint(blk.src)))
+    # squeeze-excitation (ryolo_se_fwd after the producing block's bn_act_fwd): m, p, s and u on the block's output x,
+    # recorded under the SE's layer index
+    for se in ses_of(plan):
+        fc = model.module_list[se.i].fc
+        out[se.i], _ = se_fwd_ratios(se, vint(se.x), vint(se.u), fc[0].weight.detach().double(),
+                                     fc[2].weight.detach().double())
+        out[se.i]["halo_u"] = halo_zero(se.u.buf)
     bufs = {}
     for blk in plan.blocks:
         for v in (blk.src, blk.y if not blk.is_head else None):
@@ -299,6 +312,11 @@ def forward_checks(st):
     st.fwd_halo = all(halo_zero(b) for b in bufs.values())
     st.fwd = out
     st.max_ratio = max(ratios)
+
+
+def ses_of(plan):
+    """the SE blocks of a training plan, each attached to the block that produces its input x"""
+    return [b.se for b in plan.blocks if getattr(b, "se", None) is not None]
 
 
 def check_block_bwd(st, blk, orig):
@@ -321,6 +339,12 @@ def check_block_bwd(st, blk, orig):
     orig(blk)
     if "error" in r:
         return r
+    if getattr(blk, "se", None) is not None and "se" in plan.sched.run[blk.i]:
+        # the block's SE ran inside orig, after the snapshot: bn_act_bwd read gx as the SE left it (check_se_bwd)
+        snap["dy"] = st.dy_after_se.pop(blk.i, None)
+        if snap["dy"] is None:
+            r["error"] = "no gradient recorded after the SE of block %d" % blk.i
+            return r
     try:
         _bwd_checks(st, blk, snap, r)
     except Exception:
@@ -393,6 +417,9 @@ def _bwd_checks(st, blk, snap, r):
     allowed[blk.gsrc.ch_off:blk.gsrc.ch_off + blk.gsrc.c] = True
     if blk.gres is not None and blk.gres.buf is gbuf:
         allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
+    se = getattr(blk, "se", None)
+    if se is not None and se.gx.buf is gbuf:            # the block's SE writes gx inside the block's backward
+        allowed[se.gx.ch_off:se.gx.ch_off + se.gx.c] = True
     prior = interior(snap["gbuf"], blk.gsrc.ch_off, blk.gsrc.c)
     if blk.s2d:
         want, mag = s2d_dgrad_ref(dz, w64, blk.src.h, blk.src.w)
@@ -443,12 +470,46 @@ def dense_loss(st, ps, seed):
     return sum((p * g).sum() for p, g in zip(ps, gs))
 
 
+def check_se_bwd(st, se, prod, orig, stream):
+    """gu, x and the prior gx snapshotted -> the production ryolo_se_bwd -> ds, dm, gW1, gW2 and gx checked (recorded
+    under the SE's layer index); then the gradient that the producing block's bn_act_bwd reads next, gx as the SE left
+    it, is kept for check_block_bwd"""
+    plan, model = st.plan, st.model
+    r, snap = {"acc": int(se.gx_acc)}, None
+    try:
+        snap = dict(gu=vint(se.gu).clone(), x=vint(se.x).clone(), gx_old=vint(se.gx).clone() if se.gx_acc else None)
+    except Exception:
+        r["error"] = traceback.format_exc()
+    orig(se, stream)
+    st.bwd[se.i] = r
+    if snap is None:
+        return
+    try:
+        assert prod.gy is se.gx and getattr(prod, "dy_s2d", None) is None and not prod.fuse_up
+        st.dy_after_se[prod.i] = dy_of(plan, prod)[0]
+        fc = model.module_list[se.i].fc
+        refs = se_bwd_refs(se, snap["gu"], snap["x"], snap["gx_old"], fc[0].weight.detach().double(),
+                           fc[2].weight.detach().double(), se.gw1, se.gw2)
+        B = st.batch
+        r["ds"] = ratio(se.ds.view(B, se.c), *refs["ds"])
+        r["dm"] = ratio(se.dm.view(B, se.c), *refs["dm"])
+        r["gw1"] = ratio(se.gw1.view(se.cr, se.c), *refs["gw1"])
+        r["gw2"] = ratio(se.gw2.view(se.c, se.cr), *refs["gw2"])
+        r.update({"gx_" + k: v for k, v in bf16_check(vint(se.gx), *refs["gx"]).items()})
+        r["halo_gu"], r["halo_gx"] = halo_zero(se.gu.buf), halo_zero(se.gx.buf)
+        if se.i in st.keep_se:
+            st.stash[("se", se.i)] = dict(snap, refs=refs, gx=vint(se.gx).clone())
+    except Exception:
+        r["error"] = traceback.format_exc()
+
+
 def backward(st, loss, block_check=check_block_bwd, head_grads=None):
     """loss.backward() with plan._backward_block wrapped: block_check(st, blk, orig) snapshots the block's inputs, runs
     orig(blk) and returns the block's results for st.bwd (None: nothing recorded).  head_grads(st, grads) sees the head
-    cotangents before the production _head_grads."""
+    cotangents before the production _head_grads.  A plan with SE blocks also has plan._se_bwd wrapped (check_se_bwd):
+    it runs inside the producing block's _backward_block, in production order."""
     plan = st.plan
-    st.bwd = {}
+    st.bwd, st.dy_after_se = {}, {}
     orig = plan._backward_block
 
     def wrapped(blk):
@@ -456,6 +517,13 @@ def backward(st, loss, block_check=check_block_bwd, head_grads=None):
         if r is not None:
             st.bwd[blk.i] = r
     patched = {"_backward_block": wrapped}
+    prod_of = {id(b.se): b for b in plan.blocks if getattr(b, "se", None) is not None}
+    if prod_of:
+        orig_se = plan._se_bwd
+
+        def se_bwd(se, stream):
+            check_se_bwd(st, se, prod_of[id(se)], orig_se, stream)
+        patched["_se_bwd"] = se_bwd
     if head_grads is not None:
         orig_hg = plan._head_grads
 
@@ -498,6 +566,11 @@ def gather_checks(st, gw_bits=True):
         else:
             want = blk.dw[:, :blk.cout, :blk.cin].reshape(blk.k, blk.k, blk.cout, blk.cin).permute(2, 3, 0, 1)
         r["gw_bits"] = torch.equal(blk.gw, want)
+    if gw_bits:
+        for se in ses_of(plan):
+            fc = st.model.module_list[se.i].fc
+            st.bwd.setdefault(se.i, {})["gw_bits"] = (torch.equal(fc[0].weight.grad, se.gw1.view(se.cr, se.c))
+                                                      and torch.equal(fc[2].weight.grad, se.gw2.view(se.c, se.cr)))
 
 
 def run_step(st, cot_seed=None, *, prepare=None, linear_fwd=None, loss=None, head_grads=None,
@@ -1023,7 +1096,7 @@ def map_plan(st):
     model, plan = st.model, st.plan
     defs = model.module_defs
     steps = plan["steps"]
-    outs, conv_of, s2d_of = {}, {}, {}
+    outs, conv_of, s2d_of, se_of, scaled = {}, {}, {}, {}, {}
     k = 0
     for i, d in enumerate(defs):
         t = d["type"]
@@ -1067,10 +1140,27 @@ def map_plan(st):
             assert i in outs, (t, i)                                # materialised by the fused conv
         elif t == "yolo":
             outs[i] = None
+        elif t == "se":
+            kind, a = steps[k]
+            se_of[i] = k
+            k += 1
+            src = outs[i - 1]
+            assert a["x"] == src.ptr and a["xcs"] == src.buf.shape[-1] and a["c"] == src.c, i
+            assert (a["h"], a["w"]) == tuple(src.interior().shape[1:3])
+            if kind == "se_fwd":
+                # out of place: u = x * s in a buffer of its own, x stays readable (from=-4 shortcuts, routes)
+                u = a["keep"][1]
+                outs[i] = View(u.buf, u.ch_off, u.c)
+                assert outs[i].ptr == a["u"] and a["ucs"] == u.buf.shape[-1] and u.c == src.c
+            else:
+                # in place: layer i - 1's output is scaled after its conv wrote it; nothing reads the unscaled tensor
+                assert kind == "se", (i, kind)
+                outs[i] = src
+                scaled[i - 1] = a["scale"]
         else:
             raise AssertionError("layer type %s in the detect graph" % t)
     assert k == len(steps)
-    st.outs, st.conv_of, st.s2d_of = outs, conv_of, s2d_of
+    st.outs, st.conv_of, st.s2d_of, st.se_of, st.scaled = outs, conv_of, s2d_of, se_of, scaled
 
 
 def check_s2d_step(st, i):
@@ -1103,6 +1193,37 @@ def check_first(st):
     if st.stash is not None:
         st.stash["first"] = dict(x=st.x[:2].clone(), got=interior(xs, 0, 4 * cout)[:2].clone(), w=a["w"], b=bias,
                                  slope=slope(model, 0))
+    return r
+
+
+def scaled_want(want, e, t, s):
+    """a bf16 conv output that an in-place SE then multiplied by its fp32 scale s [B, c]: the conv's own rounding (half a
+    bf16 ulp of |want| + e + t, plus e + t) carried through the multiply, whose fp32 rounding adds U |want s|; the SE's
+    bf16 rounding is the half ulp bf16_check allows"""
+    s = s.double().view(s.shape[0], 1, 1, -1)
+    w = want * s
+    return w, (HALF_BF16 * (want.abs() + e + t) + e + t) * s, U * w.abs()
+
+
+def check_se_step(st, i):
+    """an eval SE step on its own buffers.  se_fwd: m, p, s and u against float64 of x (the SE bounds of the training
+    step), u's halo zero.  se (in place, x overwritten): s against float64 of the kernel's own channel sums"""
+    kind, a = st.plan["steps"][st.se_of[i]]
+    fc = st.model.module_list[i].fc
+    w1, w2 = a["w1"].double(), a["w2"].double()
+    r = dict(kind=kind, w_bits=torch.equal(a["w1"], fc[0].weight.detach().float())
+             and torch.equal(a["w2"], fc[2].weight.detach().float()))
+    if kind == "se":
+        b = a["sums"].numel() // a["c"]
+        r["s"] = ratio(a["scale"].view(b, a["c"]), *se_block_s_ref(a["sums"].view(b, a["c"]), w1, w2, a["h"] * a["w"]))
+        return r
+    se = types.SimpleNamespace(h=a["h"], w=a["w"], c=a["c"], cr=a["cr"], m=a["m"], p=a["p"], s=a["s"])
+    x, u = st.outs[i - 1].interior(), st.outs[i].interior()
+    rr, refs = se_fwd_ratios(se, x, u, w1, w2)
+    r.update(rr)
+    r["halo_u"] = halo_zero(st.outs[i].buf)
+    if st.stash is not None and i in st.keep:
+        st.stash[("se", i)] = dict(x=x.clone(), s=a["s"].clone(), u=u.clone(), refs=refs)
     return r
 
 
@@ -1159,7 +1280,12 @@ def check_conv(st, i):
         assert a["r"] is None
     head = desc.out_dtype == L.DT_F32
     up = bool(desc.upsample2x)
-    out = st.outs[i] if not up and not desc.has_residual else st.outs[i + 1]
+    oi = i if not up and not desc.has_residual else i + 1
+    out = st.outs[oi]
+    sc = getattr(st, "scaled", {}).get(oi)         # an in-place SE scaled this output after the conv wrote it
+    if sc is not None:
+        assert not head and not up
+        sc = sc.view(desc.batch, cout)
     n = taps * cin_pad // 16
     mats = [(dy, dx, pk[t, :cout, :desc.cin].double().t().contiguous())
             for t, (dy, dx) in enumerate(conv_offsets(k, taps))]
@@ -1179,6 +1305,8 @@ def check_conv(st, i):
             heads.append(f32_check(got, s + b64, e)["max"])
         else:
             want, t = conv_want(s, b64, slope_, res[b0:b1] if res is not None else None)
+            if sc is not None:
+                want, e, t = scaled_want(want, e, t, sc[b0:b1])
             y = out.interior()[b0:b1]
             if up:
                 base = y[:, ::2, ::2]

@@ -371,6 +371,91 @@ def se_chain(h, w, c):
     return -(-span // lanes) + lanes + nsplit
 
 
+def se_block_chain(h, w, c):
+    """longest fp32 addition chain of the in-place eval SE's channel sums (csrc/se.cu se_pool_kernel): the pixels one
+    thread adds over its rows, then one atomicAdd per thread and row block in any order"""
+    rpb = -(-h // 64) if h > 64 else 1
+    pstep = 256 // (c // 8)
+    return rpb * -(-w // pstep) + pstep * -(-h // rpb)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# squeeze-excitation: float64 references of ryolo_se_fwd / ryolo_se_bwd on the kernels' own inputs.  se carries h, w, c,
+# cr and the kernels' fp32 outputs m, p, s (ds, dm for the backward) as flat [B * c] / [B * cr] tensors.
+def ratio(got, want, bound):
+    return float(((got.double() - want).abs() / (bound + TINY)).max())
+
+
+def se_fwd_refs(se, x, w1, w2):
+    """float64 references of the forward outputs from the kernels' own inputs; returns {name: (ref, bound)}"""
+    B, hw = x.shape[0], se.h * se.w
+    c, cr = se.c, se.cr
+    m, p, s = se.m.view(B, c).double(), se.p.view(B, cr).double(), se.s.view(B, c).double()
+    xd = x.double()
+    m64 = xd.sum((1, 2)) / hw
+    m_b = se_chain(se.h, se.w, c) * U * xd.abs().sum((1, 2)) / hw + U * m64.abs()
+    p64 = m @ w1.t()
+    p_b = (c + 1) * U * (m.abs() @ w1.abs().t())
+    hid = p.clamp(min=0)
+    a64 = hid @ w2.t()
+    s64 = torch.sigmoid(a64)
+    s_b = s64 * (1 - s64) * (cr + 1) * U * (hid @ w2.abs().t()) + 4 * U * s64
+    u64 = xd * s.view(B, 1, 1, c)
+    return dict(m=(m64, m_b), p=(p64, p_b), s=(s64, s_b), u=(u64, 3 * U * u64.abs()))
+
+
+def se_bwd_refs(se, gu, x, gx_old, w1, w2, gw1, gw2):
+    """float64 references of ryolo_se_bwd's outputs from its own inputs (gx_old: the prior gx it accumulates onto, None
+    when it writes first); returns {name: (ref, bound)}"""
+    B, hw = x.shape[0], se.h * se.w
+    c, cr = se.c, se.cr
+    m, p, s = se.m.view(B, c).double(), se.p.view(B, cr).double(), se.s.view(B, c).double()
+    ds, dm = se.ds.view(B, c).double(), se.dm.view(B, c).double()
+    prod = gu.double() * x.double()
+    ds64 = prod.sum((1, 2))
+    ds_b = se_chain(se.h, se.w, c) * U * prod.abs().sum((1, 2))
+    da = ds * s * (1 - s)
+    mask = (p > 0).double()
+    dh_mag = da.abs() @ w2.abs()
+    dhid = (da @ w2) * mask
+    dh_err = (c + 4) * U * dh_mag * mask
+    dm64 = dhid @ w1
+    dm_b = (cr + 1) * U * (dhid.abs() @ w1.abs()) + dh_err @ w1.abs()
+    hid = p.clamp(min=0)
+    gw2_64 = da.t() @ hid
+    gw2_b = (B + 4) * U * (da.abs().t() @ hid)
+    gw1_64 = dhid.t() @ m
+    gw1_b = (B + 1) * U * (dhid.abs().t() @ m.abs()) + dh_err.t() @ m.abs()
+    gus = gu.double() * s.view(B, 1, 1, c)
+    dmh = (dm / hw).view(B, 1, 1, c)
+    gx64 = gus + dmh + (gx_old.double() if gx_old is not None else 0.0)
+    gx_e = 3 * U * (gus.abs() + dmh.abs() + (gx_old.double().abs() if gx_old is not None else 0.0))
+    return dict(ds=(ds64, ds_b), dm=(dm64, dm_b), gw1=(gw1_64, gw1_b), gw2=(gw2_64, gw2_b), gx=(gx64, gx_e))
+
+
+def se_fwd_ratios(se, x, u, w1, w2):
+    """ryolo_se_fwd's m, p, s and u against se_fwd_refs: {name: worst ratio}, u with its rounding-bias ratio"""
+    B = x.shape[0]
+    refs = se_fwd_refs(se, x, w1, w2)
+    r = dict(m=ratio(se.m.view(B, se.c), *refs["m"]), p=ratio(se.p.view(B, se.cr), *refs["p"]),
+             s=ratio(se.s.view(B, se.c), *refs["s"]))
+    r.update({"u_" + k: v for k, v in bf16_check(u, *refs["u"]).items()})
+    return r, refs
+
+
+def se_block_s_ref(sums, w1, w2, hw):
+    """ryolo_se_block's scale from its own fp32 channel sums [B, c]: mean = sums * fp32(1 / hw) (2 U), p = W1 mean
+    ((c + 1) U |W1| |mean|, carried through W2 with the mean's 2 U), s = sigmoid(W2 relu(p)) as in the SE bounds;
+    returns (s, bound)"""
+    c, cr = w1.shape[1], w1.shape[0]
+    m = sums.double() / hw
+    p_err = (c + 3) * U * (m.abs() @ w1.abs().t())
+    hid = (m @ w1.t()).clamp(min=0)
+    s64 = torch.sigmoid(hid @ w2.t())
+    s_b = s64 * (1 - s64) * ((cr + 1) * U * ((hid + p_err) @ w2.abs().t()) + p_err @ w2.abs().t()) + 4 * U * s64
+    return s64, s_b
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # the bf16 weight gradient (csrc/wgrad.cu) on one set of operands
 def wgrad(dzb, zcs, cout_pad, xb, xcs, cin_pad, b, h, w, k, dw, stream=None):

@@ -1,20 +1,22 @@
 """TEST INFRASTRUCTURE: one checked bf16 training step and the per-launch checks of the eval forward, against float64 of
 the inputs each kernel actually received.  The only module of the suite that wraps plan methods: the float64 tests
-(test_train_step_f64_gpu.py, test_dilated_train_f64_gpu.py, test_multiclass_f64_gpu.py, test_se_f64_gpu.py,
-test_detect_forward_f64_gpu.py) bring their model, shape and extra checks and read the results this module records.
+(test_train_step_f64_gpu.py, test_train_scale_f64_gpu.py, test_dilated_train_f64_gpu.py, test_multiclass_f64_gpu.py,
+test_se_f64_gpu.py, test_detect_forward_f64_gpu.py) bring their model, shape and extra checks and read the results this
+module records.
 
 Training step (run_step): after model(x) every buffer a forward kernel wrote is still there, so forward_checks checks
-each launch post hoc on the plan's own input buffers; plan._backward_block is wrapped (instance attribute) so that each
-block's inputs are snapshotted, the production code runs unchanged and its outputs are checked right after
-(check_block_bwd).  The bounds are stated in test_train_step_f64_gpu.py.  run_step_chunked runs the same checks at a
-batch whose activations fill the card (test_train_scale_f64_gpu.py): over image chunks, with host copies of only what a
-block overwrites.  schedule_rows mirrors what each launch's schedule derives from the shape, from a plan built or only
-laid out (plan_layout).
+each launch post hoc on the plan's own input buffers; plan._backward_block is wrapped (instance attribute) so that what
+each block overwrites is snapshotted, the production code runs unchanged and its outputs are checked right after
+(check_block_bwd).  The bounds are stated in test_train_step_f64_gpu.py.  Every check runs over image chunks of at most
+`budget` float64 bytes, so that the same checks hold at a batch whose activations fill the card
+(test_train_scale_f64_gpu.py): the snapshot copies only what a block overwrites to host memory, and every full
+reduction is summed in float64 over the chunks.  schedule_rows mirrors what each launch's schedule derives from the
+shape, from a plan built or only laid out (plan_layout).
 
 Squeeze-excitation: forward_checks checks ryolo_se_fwd's m, p, s and u post hoc; plan._se_bwd is wrapped as well
 (check_se_bwd), because the SE backward runs inside its producing block's _backward_block, right before that block's
-bn_act_bwd reads gx: the wrapper checks the SE on its own inputs and hands check_block_bwd the gx the SE left.  The SE
-bounds are stated in test_se_f64_gpu.py.
+bn_act_bwd reads gx: the wrapper checks the SE on its own inputs, and check_block_bwd reads dy after the block, which is
+the gx the SE left.  The SE bounds are stated in test_se_f64_gpu.py.
 
 Eval forward (map_plan, check_first, check_conv, check_s2d_step, check_se_step, check_buffers): the steps of the eval
 plan mapped to the graph's layers and every conv launch checked on its own input buffers; the bounds are stated in
@@ -28,7 +30,7 @@ import torch.nn.functional as F
 
 from builders import ryolo_lib
 from f64_refs import (BF16, BIAS_TOL, F64, HALF_BF16, STAT_TOL, TINY, U, bf16_check, bitwise, bn_act_fwd_ref, bn_chain,
-                      bn_pieces, check_z, conv_schedule, conv_taps, d2s, f32_check, gemm_sms, halo_zero, head_bias_blocks,
+                      bn_pieces, conv_schedule, conv_taps, d2s, f32_check, gemm_sms, halo_zero, head_bias_blocks,
                       head_bias_chain, interior, ratio, rup, s2d, s2d_dgrad_ref, se_block_s_ref, se_bwd_refs, se_fwd_ratios,
                       sum_check, tapsum, vint, wgrad_ratio, wgrad_ref, worst_ratio)
 from helpers import wgrad_plan
@@ -62,32 +64,55 @@ def _weight(model, blk):
     return model.module_list[blk.i].Conv2d.weight.detach()
 
 
-def fwd_ref(plan, blk, w):
-    """float64 raw conv of the block on its actual input buffer, and its magnitude"""
-    w64 = w.detach().to(BF16).double()
-    if blk.i == 0:
-        x = interior(plan.col, 0, 27)
-        return tapsum(x, [(0, 0, w64.reshape(blk.cout, 27).t())], blk.oh, blk.ow)
-    return tapsum(vint(blk.src), conv_taps(w64), blk.oh, blk.ow, blk.stride)
-
-
 def conv_updates(blk):
     return blk.k_eff * blk.k_eff * blk.cin_pad // 16
 
 
-def stats_check(z, c, sums, mean, invstd, scale, shift, rm0, rv0, rm, rv, gamma, beta, eps, mom, l, unbiased=True):
-    """batch statistics: the kernel's sums against float64 (reduction bound), mean / invstd against the two-pass float64
-    statistics (target 2^-12), the finalisation and the running statistics against both the float64 statistics and the
-    fp32 arithmetic of bn_finalize_channel applied to the kernel's own sums"""
-    z64 = z.double().reshape(-1, c)
-    m64 = z64.mean(0)
-    ref = dict(n=z64.shape[0], m64=m64, v64=(z64 - m64).pow(2).mean(0), s1=z64.sum(0), a1=z64.abs().sum(0),
-               s2=z64.pow(2).sum(0))
-    return stats_ratios(ref, z.device, c, sums, mean, invstd, scale, shift, rm0, rv0, rm, rv, gamma, beta, eps, mom, l,
-                        unbiased)
+def f64_bytes(c_in, c_out, hw_in, hw_out):
+    """float64 working set per image of a tap-sum reference and its check: the padded operand, its |.|, one shifted
+    copy; value, magnitude and about eight temporaries of the result"""
+    return 8 * (3 * c_in * hw_in + 10 * c_out * hw_out)
 
 
-def stats_ref_chunked(z, c, chunk_list):
+def ref_bytes(blk):
+    """float64 bytes per image of the block's conv, wgrad and dgrad references and their checks"""
+    gh, gw = (blk.src.h // 2, blk.src.w // 2) if blk.s2d else (blk.src.h, blk.src.w)
+    cin = 27 if blk.i == 0 else blk.cin_eff
+    hw = blk.src.h * blk.src.w
+    out = dict(fwd=f64_bytes(cin, blk.cout, (gh + 2) * (gw + 2), blk.oh * blk.ow),
+               wgrad=f64_bytes(cin, blk.cout, (gh + 2) * (gw + 2), gh * gw))
+    if blk.s2d:        # dz zero-inserted on the input grid, then the mirrored 3x3 taps
+        out["dgrad"] = f64_bytes(blk.cout, blk.src.c, hw, hw) + 8 * hw * blk.cout
+    elif blk.i > 0:
+        out["dgrad"] = f64_bytes(blk.cout, blk.cin, hw, hw)
+    return out
+
+
+def _img_bytes(t):
+    return t[0].numel() * t.element_size()
+
+
+def _host(t, chunk_list):
+    """t (an image-major device view) copied to host memory chunk by chunk"""
+    return torch.cat([t[b0:b1].cpu() for b0, b1 in chunk_list])
+
+
+def _channels_host(buf, ch, b0, b1):
+    """channels ch of images [b0, b1) of buf, copied to host memory (no device copy when ch is every channel)"""
+    v = buf[b0:b1]
+    return (v if len(ch) == v.shape[-1] else v.index_select(3, ch)).cpu()
+
+
+def _max_offset(v, buf):
+    """largest element offset into the buffer buf that its view v addresses"""
+    return v.storage_offset() - buf.storage_offset() + sum((s - 1) * d for s, d in zip(v.shape, v.stride()))
+
+
+def _overlap(a, b):
+    return a is not None and b is not None and a.buf is b.buf and a.ch_off < b.ch_off + b.c and b.ch_off < a.ch_off + a.c
+
+
+def stats_ref(z, c, chunk_list):
     """the float64 reductions stats_ratios needs, over image chunks of z [B, h, w, c] (two passes)"""
     s1 = torch.zeros(c, dtype=F64, device=z.device)
     a1, s2, q = s1.clone(), s1.clone(), s1.clone()
@@ -106,6 +131,9 @@ def stats_ref_chunked(z, c, chunk_list):
 
 def stats_ratios(ref, device, c, sums, mean, invstd, scale, shift, rm0, rv0, rm, rv, gamma, beta, eps, mom, l,
                  unbiased=True):
+    """batch statistics: the kernel's sums against float64 (reduction bound), mean / invstd against the two-pass float64
+    statistics of ref (target 2^-12), the finalisation and the running statistics against both the float64 statistics and
+    the fp32 arithmetic of bn_finalize_channel applied to the kernel's own sums"""
     n, m64, v64 = ref["n"], ref["m64"], ref["v64"]
     std = (v64 + eps).sqrt()
     s1, s2 = sums[:c].double(), sums[c:2 * c].double()
@@ -219,13 +247,21 @@ def dy_of(plan, blk, shift=0, imgs=slice(None)):
 
 
 def forward_checks(st):
+    """every forward launch post hoc on the plan's buffers, over image chunks of at most st.budget float64 bytes"""
     plan, model = st.plan, st.model
     L = _layout()
+    B = st.batch
     out = {}
-    # im2col of the image: bit for bit, columns 27..63 and the halo zero
-    want_col = F.unfold(st.x, 3, padding=1).view(st.batch, 27, st.h, st.w).permute(0, 2, 3, 1).to(BF16)
-    st.im2col = dict(bits=bitwise(interior(plan.col, 0, 27), want_col),
-                     pad_zero=bool((interior(plan.col, 27, 37) == 0).all()), halo=halo_zero(plan.col))
+    # im2col of the image: bit for bit, columns 27..63 and the halo zero; the largest element offset checked
+    col = plan.col
+    bits = pad = True
+    for b0, b1 in chunks(B, 8 * 27 * st.h * st.w, st.budget):
+        want = F.unfold(st.x[b0:b1], 3, padding=1).view(b1 - b0, 27, st.h, st.w).permute(0, 2, 3, 1).to(BF16)
+        bits = bits and bitwise(interior(col, 0, 27)[b0:b1], want)
+        pad = pad and bool((interior(col, 27, 37)[b0:b1] == 0).all())
+        del want
+    st.checked_offsets = {"col": (col.numel(), _max_offset(interior(col, 27, 37), col))}
+    st.im2col = dict(bits=bits, pad_zero=pad, halo=halo_zero(col))
     # the multi-tensor pack against the single-operand pack into fresh buffers
     packs = []
     for blk in plan.blocks:
@@ -243,56 +279,81 @@ def forward_checks(st):
         if blk.owner is not None:          # weight_from blocks: their own launches (test_dilated_train_f64_gpu.py)
             continue
         r = {}
-        w = _weight(model, blk)
-        want, mag = fwd_ref(plan, blk, w)
+        w64 = _weight(model, blk).to(BF16).double()
+        if blk.i == 0:
+            x, taps, s = interior(plan.col, 0, 27), [(0, 0, w64.reshape(blk.cout, 27).t())], 1
+        else:
+            x, taps, s = vint(blk.src), conv_taps(w64), blk.stride
         n = conv_updates(blk)
+        cl = chunks(B, ref_bytes(blk)["fwd"], st.budget)
         if blk.is_head:
             bias = model.module_list[blk.i].Conv2d.bias.detach().double()
             got = blk.out.detach().permute(0, 2, 3, 1)
-            r["z"] = f32_check(got, want + bias, n * 2.0 ** -23 * mag)["max"]
+            worst = []
+            for b0, b1 in cl:
+                want, mag = tapsum(x[b0:b1], taps, blk.oh, blk.ow, s)
+                worst.append(f32_check(got[b0:b1], want + bias, n * 2.0 ** -23 * mag)["max"])
+                del want, mag
+            r["z"] = float(torch.tensor(worst, dtype=F64).max())
             out[blk.i] = r
             continue
         z = interior(blk.z, 0, blk.cout)
-        rz = check_z(z, want, mag, n)
+        acc, kept = Acc(), []
+        for b0, b1 in cl:
+            want, mag = tapsum(x[b0:b1], taps, blk.oh, blk.ow, s)
+            acc.add(z[b0:b1], want, n * 2.0 ** -23 * mag)
+            if blk.i in st.keep_fwd:
+                kept.append((want, mag))
+            del want, mag
+        rz = acc.result()
         r["z"], r["z_bias"] = rz["max"], rz["bias"]
         if blk.i in st.keep_fwd:
-            st.stash[("z", blk.i)] = dict(want=want.clone(), mag=mag.clone(), n=n, got=z.clone())
-        del want, mag
+            st.stash[("z", blk.i)] = dict(want=torch.cat([k[0] for k in kept]), mag=torch.cat([k[1] for k in kept]),
+                                          n=n, got=z.clone())
+        del kept
+        cz = chunks(B, 8 * 6 * _img_bytes(z), st.budget)
         if blk.has_bn:
             bn = _bn_of(model, blk)
-            rs, ratio = stats_check(z, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale, blk.shift, st.rm0[blk.i],
-                                    st.rv0[blk.i], bn.running_mean, bn.running_var, bn.weight.detach(), bn.bias.detach(),
-                                    bn.eps, bn.momentum, bn_chain(st.batch, blk.oh, blk.ow, blk.cout)["sums"])
+            args = (stats_ref(z, blk.cout, cz), z.device, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale,
+                    blk.shift, st.rm0[blk.i], st.rv0[blk.i], bn.running_mean, bn.running_var, bn.weight.detach(),
+                    bn.bias.detach(), bn.eps, bn.momentum, bn_chain(B, blk.oh, blk.ow, blk.cout)["sums"])
+            rs, mos = stats_ratios(*args)
             r.update(rs)
-            r["mean_over_std"] = ratio
+            r["mean_over_std"] = mos
+            ratios.append(mos)
             # the same check with the running variance taken as biased (n instead of n - 1): kept for the bound self-test
-            rb_, _ = stats_check(z, blk.cout, blk.sums, blk.mean, blk.invstd, blk.scale, blk.shift, st.rm0[blk.i],
-                                 st.rv0[blk.i], bn.running_mean, bn.running_var, bn.weight.detach(), bn.bias.detach(),
-                                 bn.eps, bn.momentum, bn_chain(st.batch, blk.oh, blk.ow, blk.cout)["sums"], unbiased=False)
-            st.rv_biased[blk.i] = max(rb_["running"], rb_["finalize"])
-            ratios.append(ratio)
+            rb, _ = stats_ratios(*args, unbiased=False)
+            st.rv_biased[blk.i] = max(rb["running"], rb["finalize"])
         else:
             # a bias (+ PReLU) conv without BatchNorm: fixed statistics, scale 1 and shift = the conv bias, bit for bit
             bias = model.module_list[blk.i].Conv2d.bias.detach()
             r["fixed_stats"] = bool((blk.scale == 1).all()) and torch.equal(blk.shift, bias)
-        # bn_act_fwd
+        # bn_act_fwd; an up-sampling block writes each pixel four times
         res = vint(blk.res) if blk.res is not None else None
-        want_y, t = bn_act_fwd_ref(z, blk.scale, blk.shift, slope_of(model, blk), res)
         y = interior(blk.y.buf, blk.y.ch_off, blk.cout)
-        if blk.fuse_up:
-            base = y[:, ::2, ::2]
-            r["up_copies"] = all(bitwise(y[:, ry::2, rx::2], base) for ry in range(2) for rx in range(2))
-            y = base
-        ry_ = bf16_check(y, want_y, 0.0, t)
+        yv = y[:, ::2, ::2] if blk.fuse_up else y
+        acc, copies = Acc(), True
+        for b0, b1 in cz:
+            want_y, t = bn_act_fwd_ref(z[b0:b1], blk.scale, blk.shift, slope_of(model, blk),
+                                       res[b0:b1] if res is not None else None)
+            if blk.fuse_up:
+                copies = copies and all(bitwise(y[b0:b1, ry::2, rx::2], yv[b0:b1]) for ry in range(2) for rx in range(2))
+            acc.add(yv[b0:b1], want_y, 0.0, t)
+            del want_y, t
+        ry_ = acc.result()
         r["y"], r["y_bias"] = ry_["max"], ry_["bias"]
+        if blk.fuse_up:
+            r["up_copies"] = copies
         if blk.i in st.keep_fwd and res is not None:
-            st.stash[("y", blk.i)] = dict(z=z.clone(), res=res.clone(), got=y.clone(), sc=blk.scale.clone(),
+            st.stash[("y", blk.i)] = dict(z=z.clone(), res=res.clone(), got=yv.clone(), sc=blk.scale.clone(),
                                           sh=blk.shift.clone(), slope=slope_of(model, blk))
         out[blk.i] = r
     # space-to-depth copies (bn_act_fwd_s2d or ryolo_space_to_depth) bit for bit; every halo zero
     for blk in plan.blocks:
         if blk.s2d:
-            out[blk.i]["xs"] = bitwise(interior(blk.xs, 0, 4 * blk.src.c), s2d(vint(blk.src)))
+            src = vint(blk.src)
+            xs = interior(blk.xs, 0, 4 * blk.src.c)
+            out[blk.i]["xs"] = all(bitwise(xs[b0:b1], s2d(src[b0:b1])) for b0, b1 in chunks(B, 4 * _img_bytes(xs), st.budget))
     # squeeze-excitation (ryolo_se_fwd after the producing block's bn_act_fwd): m, p, s and u on the block's output x,
     # recorded under the SE's layer index
     for se in ses_of(plan):
@@ -319,32 +380,61 @@ def ses_of(plan):
     return [b.se for b in plan.blocks if getattr(b, "se", None) is not None]
 
 
+def snapshot(st, blk):
+    """before the block's backward, what it overwrites and its checks read, copied to host memory over image chunks: z
+    (which becomes dz in place), the prior of an accumulated gradient view, the channels of the shared gradient buffer
+    outside the views the block (and its SE) write; for the blocks in st.keep_bwd, dy read 32 channels off.  dy itself
+    is read after the block, from buffers the block does not write."""
+    B = st.batch
+    snap = {}
+
+    def host(t):
+        return _host(t, chunks(B, _img_bytes(t), st.budget))
+    if not blk.is_head:
+        snap["z"] = host(interior(blk.z, 0, blk.cout))
+        assert not _overlap(blk.gy, blk.gsrc) and not _overlap(blk.gy, blk.gres) and blk.gy.buf is not blk.z
+        if blk.gres is not None and blk.gres_acc:
+            snap["gres_prior"] = host(vint(blk.gres))
+        if blk.i in st.keep_bwd and blk.fuse_up:
+            snap["dy_shift"], _ = dy_of(st.plan, blk, shift=32)
+    if blk.gsrc is not None:
+        gbuf = blk.gsrc.buf
+        if blk.gsrc_acc:
+            snap["prior"] = host(vint(blk.gsrc))
+        # a space-to-depth block whose producer reads its dgrad output in place writes no gradient view of its own
+        se = getattr(blk, "se", None)
+        views = [blk.gres, se.gx if se is not None else None, None if blk.s2d and blk.dxs_direct else blk.gsrc]
+        allowed = torch.zeros(gbuf.shape[-1], dtype=torch.bool)
+        for v in views:
+            if v is not None and v.buf is gbuf:
+                allowed[v.ch_off:v.ch_off + v.c] = True
+        snap["outside"] = (~allowed).nonzero().flatten().to(gbuf.device)
+        if len(snap["outside"]):
+            snap["gbuf_outside"] = torch.cat([_channels_host(gbuf, snap["outside"], b0, b1)
+                                              for b0, b1 in chunks(B, _img_bytes(gbuf), st.budget)])
+    return snap
+
+
+def outside_untouched(st, blk, snap):
+    """the channels of the block's gradient buffer outside the views it writes are as snapshot() left them, and the halo
+    is zero"""
+    gbuf = blk.gsrc.buf
+    same = not len(snap["outside"]) or all(
+        torch.equal(_channels_host(gbuf, snap["outside"], b0, b1), snap["gbuf_outside"][b0:b1])
+        for b0, b1 in chunks(st.batch, _img_bytes(gbuf), st.budget))
+    return same and halo_zero(gbuf)
+
+
 def check_block_bwd(st, blk, orig):
     """snapshot -> the production _backward_block -> checks; returns the results (never raises into autograd)"""
-    plan = st.plan
-    r = {}
-    snap = {}
+    r, snap = {}, {}
     try:
-        if not blk.is_head:
-            snap["z"] = interior(blk.z, 0, blk.cout).clone()
-            snap["dy"], r["dy_mode"] = dy_of(plan, blk)
-            if blk.i in st.keep_bwd and blk.fuse_up:
-                snap["dy_shift"], _ = dy_of(plan, blk, shift=32)
-            if blk.gres is not None:
-                snap["gres_prior"] = vint(blk.gres).clone()
-        if blk.gsrc is not None:
-            snap["gbuf"] = blk.gsrc.buf.clone()
+        snap = snapshot(st, blk)
     except Exception:
         r["error"] = traceback.format_exc()
     orig(blk)
     if "error" in r:
         return r
-    if getattr(blk, "se", None) is not None and "se" in plan.sched.run[blk.i]:
-        # the block's SE ran inside orig, after the snapshot: bn_act_bwd read gx as the SE left it (check_se_bwd)
-        snap["dy"] = st.dy_after_se.pop(blk.i, None)
-        if snap["dy"] is None:
-            r["error"] = "no gradient recorded after the SE of block %d" % blk.i
-            return r
     try:
         _bwd_checks(st, blk, snap, r)
     except Exception:
@@ -354,41 +444,55 @@ def check_block_bwd(st, blk, orig):
 
 def dz_checks(st, blk, snap, r):
     """the head cotangent's dz bit for bit, or bn_act_bwd of a BatchNorm block (dz, d beta, d gamma, d slope, the shortcut
-    gradient); returns dz"""
-    model = st.model
+    gradient) on the dy it read; returns dz"""
+    plan, model = st.plan, st.model
+    B = st.batch
+    dev = st.x.device
     if blk.is_head:
         dz = interior(blk.dz, 0, blk.cout)
-        r["dz_bits"] = bitwise(dz, st.g_nhwc[blk.i].to(BF16))
+        g = st.g_nhwc[blk.i]
+        r["dz_bits"] = all(bitwise(dz[b0:b1], g[b0:b1].to(BF16)) for b0, b1 in chunks(B, 4 * _img_bytes(dz), st.budget))
         r["dz_pad_zero"] = bool((blk.dz[..., blk.cout:] == 0).all()) and halo_zero(blk.dz)
-    else:
-        dz = interior(blk.z, 0, blk.cout)
-        chain = bn_chain(st.batch, blk.oh, blk.ow, blk.cout, 2 if r["dy_mode"] == 2 and blk.cout // 8 * 2 <= 640 else 1)
-        rb, near = bn_bwd_check(snap["z"], snap["dy"], dz, blk.bsums, blk.mean, blk.invstd, blk.scale, blk.shift,
-                                slope_of(model, blk), chain)
-        r["dz"], r["dz_bias"] = rb["max"], rb["bias"]
-        for k in ("dbeta", "dgamma", "dslope"):
-            r[k] = rb[k]
-        r["near_zero_u"] = near
-        r["n_elems"] = snap["z"].numel()
-        if blk.i in st.keep_bwd:
-            st.stash[("bn", blk.i)] = dict(z=snap["z"], dy=snap["dy"], dy_shift=snap.get("dy_shift"), dz=dz.clone(),
-                                           sums=blk.bsums.clone(), mean=blk.mean.clone(), invstd=blk.invstd.clone(),
-                                           sc=blk.scale.clone(), sh=blk.shift.clone(), slope=slope_of(model, blk),
-                                           chain=chain)
-        if blk.gres is not None:
-            d = snap["dy"]
-            want = (snap["gres_prior"].float() + d).to(BF16) if blk.gres_acc else d.to(BF16)
-            r["gres_bits"] = bitwise(vint(blk.gres), want)
-        r["dz_halo"] = halo_zero(blk.z)
+        return dz
+    dz = interior(blk.z, 0, blk.cout)
+    _, r["dy_mode"] = dy_of(plan, blk, imgs=slice(0, 1))
+    chain = bn_chain(B, blk.oh, blk.ow, blk.cout, 2 if r["dy_mode"] == 2 and blk.cout // 8 * 2 <= 640 else 1)
+    cl = chunks(B, 8 * 12 * blk.oh * blk.ow * blk.cout, st.budget)
+
+    def parts():
+        for b0, b1 in cl:
+            yield snap["z"][b0:b1].to(dev), dy_of(plan, blk, imgs=slice(b0, b1))[0], dz[b0:b1]
+    rb, near = bn_bwd_check_chunked(parts, blk.cout, blk.bsums, blk.mean, blk.invstd, blk.scale, blk.shift,
+                                    slope_of(model, blk), chain)
+    r["dz"], r["dz_bias"] = rb["max"], rb["bias"]
+    for k in ("dbeta", "dgamma", "dslope", "finite"):
+        r[k] = rb[k]
+    r["near_zero_u"] = near
+    r["n_elems"] = dz.numel()
+    if blk.i in st.keep_bwd:
+        st.stash[("bn", blk.i)] = dict(z=snap["z"].to(dev), dy=dy_of(plan, blk)[0], dy_shift=snap.get("dy_shift"),
+                                       dz=dz.clone(), sums=blk.bsums.clone(), mean=blk.mean.clone(),
+                                       invstd=blk.invstd.clone(), sc=blk.scale.clone(), sh=blk.shift.clone(),
+                                       slope=slope_of(model, blk), chain=chain)
+    if blk.gres is not None:
+        gres = vint(blk.gres)
+        ok = True
+        for b0, b1 in cl:
+            d = dy_of(plan, blk, imgs=slice(b0, b1))[0]
+            want = (snap["gres_prior"][b0:b1].to(dev).float() + d).to(BF16) if blk.gres_acc else d.to(BF16)
+            ok = ok and bitwise(gres[b0:b1], want)
+        r["gres_bits"] = ok
+    r["dz_halo"] = halo_zero(blk.z)
     return dz
 
 
 def _bwd_checks(st, blk, snap, r):
     plan, model = st.plan, st.model
-    w = _weight(model, blk)
-    w64 = w.to(BF16).double()
+    B = st.batch
+    dev = st.x.device
+    w64 = _weight(model, blk).to(BF16).double()
     dz = dz_checks(st, blk, snap, r)
-    # weight gradient (split-K layout) and its gather
+    # weight gradient (split-K layout): the float64 reference summed over image chunks
     if blk.i == 0:
         x, offs, cin = interior(plan.col, 0, 27), [(0, 0)], 27
     elif blk.s2d:
@@ -399,82 +503,102 @@ def _bwd_checks(st, blk, snap, r):
         p = (blk.k - 1) // 2
         offs = [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)]
     gh, gw_ = x.shape[1], x.shape[2]
-    wr, wm = wgrad_ref(x, dz, offs)
-    plan_w = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, st.batch, gh, gw_, gemm_sms())
+    wr = wm = 0.0
+    for b0, b1 in chunks(B, ref_bytes(blk)["wgrad"], st.budget):
+        a, m = wgrad_ref(x[b0:b1], dz[b0:b1], offs)
+        wr, wm = wr + a, wm + m
+        del a, m
+    plan_w = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, B, gh, gw_, gemm_sms())
     got = blk.dw[:, :blk.cout, :cin]
     # test_wgrad's random-walk bound (KAPPA sqrt(n_add) 2^-24 A) is reported, not required: on the step's operands the
     # accumulator's truncations do not cancel
     r["wgrad"] = wgrad_ratio(got, wr, wm, plan_w)
     r["wgrad_rw"] = worst_ratio(got, wr, wm, plan_w["n_add"])
-    if blk.i in st.keep_bwd and blk.k == 3 and not blk.s2d:
+    if blk.i in st.keep_bwd:
         st.stash[("wgrad", blk.i)] = dict(x=x.clone(), dz=dz.clone(), offs=offs, got=got.clone(), plan=plan_w)
     del wr, wm
     if blk.i == 0:
         return
     # input gradient
     gbuf = blk.gsrc.buf
-    allowed = torch.zeros(gbuf.shape[-1], dtype=torch.bool, device=gbuf.device)
-    allowed[blk.gsrc.ch_off:blk.gsrc.ch_off + blk.gsrc.c] = True
-    if blk.gres is not None and blk.gres.buf is gbuf:
-        allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
-    se = getattr(blk, "se", None)
-    if se is not None and se.gx.buf is gbuf:            # the block's SE writes gx inside the block's backward
-        allowed[se.gx.ch_off:se.gx.ch_off + se.gx.c] = True
-    prior = interior(snap["gbuf"], blk.gsrc.ch_off, blk.gsrc.c)
     if blk.s2d:
-        want, mag = s2d_dgrad_ref(dz, w64, blk.src.h, blk.src.w)
+        dxs = interior(blk.dxs, 0, blk.cin_eff)
         n = 4 * rup(blk.cout, 64) // 16
-        rd = check_z(interior(blk.dxs, 0, blk.cin_eff), want, mag, n)
+        acc, bits = Acc(), True
+        for b0, b1 in chunks(B, ref_bytes(blk)["dgrad"], st.budget):
+            want, mag = s2d_dgrad_ref(dz[b0:b1], w64, blk.src.h, blk.src.w)
+            acc.add(dxs[b0:b1], want, n * 2.0 ** -23 * mag)
+            del want, mag
+            if not blk.dxs_direct:
+                v = d2s(dxs[b0:b1], blk.src.c)
+                want_bits = (snap["prior"][b0:b1].to(dev).float() + v.float()).to(BF16) if blk.gsrc_acc else v
+                bits = bits and bitwise(vint(blk.gsrc)[b0:b1], want_bits)
+        rd = acc.result()
         r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
-        del want, mag
-        if blk.dxs_direct:
-            allowed[:] = False
-            if blk.gres is not None and blk.gres.buf is gbuf:
-                allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
-        else:
-            v = d2s(interior(blk.dxs, 0, blk.cin_eff), blk.src.c)
-            want_bits = (prior.float() + v.float()).to(BF16) if blk.gsrc_acc else v
-            r["d2s_bits"] = bitwise(vint(blk.gsrc), want_bits)
+        if not blk.dxs_direct:
+            r["d2s_bits"] = bits
     else:
-        want, mag = tapsum(dz, conv_taps(w64, mirror=True), blk.src.h, blk.src.w)
-        n = blk.k * blk.k * rup(blk.cout, 64) // 16
-        e = n * 2.0 ** -23 * mag
-        t = 0.0
-        if blk.gsrc_acc:
-            want = want + prior.double()
-            t = U * (mag + prior.double().abs())
         got = vint(blk.gsrc)
-        rd = bf16_check(got, want, e, t)
+        n = blk.k * blk.k * rup(blk.cout, 64) // 16
+        acc = Acc()
+        for b0, b1 in chunks(B, ref_bytes(blk)["dgrad"], st.budget):
+            want, mag = tapsum(dz[b0:b1], conv_taps(w64, mirror=True), blk.src.h, blk.src.w)
+            e, t = n * 2.0 ** -23 * mag, 0.0
+            if blk.gsrc_acc:
+                prior = snap["prior"][b0:b1].to(dev).double()
+                want = want + prior
+                t = U * (mag + prior.abs())
+                del prior
+            acc.add(got[b0:b1], want, e, t)
+            del want, mag, e, t
+        rd = acc.result()
         r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
         if blk.i in st.keep_bwd:
-            st.stash[("dgrad", blk.i)] = dict(dz=dz.clone(), w64=w64, got=got.clone(), prior=prior.clone(),
+            st.stash[("dgrad", blk.i)] = dict(dz=dz.clone(), w64=w64, got=got.clone(),
+                                              prior=snap["prior"].to(dev) if blk.gsrc_acc else None,
                                               acc=blk.gsrc_acc, h=blk.src.h, w=blk.src.w, n=n,
                                               shifted=(interior(gbuf, blk.gsrc.ch_off - 32, blk.gsrc.c).clone()
                                                        if blk.gsrc.ch_off >= 32 else None))
-        del want, mag
-    outside = ~allowed
-    r["outside_untouched"] = torch.equal(gbuf[..., outside], snap["gbuf"][..., outside]) and halo_zero(gbuf)
+    r["outside_untouched"] = outside_untouched(st, blk, snap)
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # the training step: the run
+class _LeanDot(torch.autograd.Function):
+    """sum(p * G) whose gradient is G itself: no cotangent-sized temporaries"""
+
+    @staticmethod
+    def forward(ctx, p, g):
+        ctx.g = g
+        return sum((p[b] * g[b]).sum() for b in range(p.shape[0]))
+
+    @staticmethod
+    def backward(ctx, go):
+        assert float(go) == 1.0
+        return ctx.g, None
+
+
 def dense_loss(st, ps, seed):
-    """loss = sum (p * G) with a dense random cotangent G per head (it reaches every head channel); keeps G in the
-    layout of the head's dz as st.g_nhwc"""
+    """loss = sum (p * G) with a dense random cotangent G per head (it reaches every head channel), drawn in the shape of
+    p and permuted on the host into the layout of the fp32 head buffer, so that the cotangent the plan receives is G
+    itself (one copy of G on the device, no product or transpose of it); st.g_nhwc views G in the layout of the head's
+    dz"""
     gen = torch.Generator().manual_seed(seed)
-    gs = [torch.randn(p.shape, generator=gen).to(p.device) for p in ps]
     st.g_nhwc = {}
-    for blk, g in zip(st.plan.heads, gs):
-        b, na, ny, nx, no = g.shape
-        st.g_nhwc[blk.i] = g.permute(0, 2, 3, 1, 4).reshape(b, ny, nx, na * no)     # channel a * no + k
-    return sum((p * g).sum() for p, g in zip(ps, gs))
+    loss = 0.0
+    for blk, p in zip(st.plan.heads, ps):
+        b, na, ny, nx, no = p.shape
+        g = torch.randn(p.shape, generator=gen).permute(0, 1, 4, 2, 3).reshape(b, na * no, ny, nx).to(p.device)
+        st.g_nhwc[blk.i] = g.permute(0, 2, 3, 1)                              # channel a * no + k
+        loss = loss + _LeanDot.apply(p, g.view(b, na, no, ny, nx).permute(0, 1, 3, 4, 2))
+    return loss
 
 
 def check_se_bwd(st, se, prod, orig, stream):
     """gu, x and the prior gx snapshotted -> the production ryolo_se_bwd -> ds, dm, gW1, gW2 and gx checked (recorded
-    under the SE's layer index); then the gradient that the producing block's bn_act_bwd reads next, gx as the SE left
-    it, is kept for check_block_bwd"""
-    plan, model = st.plan, st.model
+    under the SE's layer index).  The producing block's bn_act_bwd reads gx next, as the SE left it: check_block_bwd reads
+    it after the block."""
+    model = st.model
     r, snap = {"acc": int(se.gx_acc)}, None
     try:
         snap = dict(gu=vint(se.gu).clone(), x=vint(se.x).clone(), gx_old=vint(se.gx).clone() if se.gx_acc else None)
@@ -486,7 +610,6 @@ def check_se_bwd(st, se, prod, orig, stream):
         return
     try:
         assert prod.gy is se.gx and getattr(prod, "dy_s2d", None) is None and not prod.fuse_up
-        st.dy_after_se[prod.i] = dy_of(plan, prod)[0]
         fc = model.module_list[se.i].fc
         refs = se_bwd_refs(se, snap["gu"], snap["x"], snap["gx_old"], fc[0].weight.detach().double(),
                            fc[2].weight.detach().double(), se.gw1, se.gw2)
@@ -504,12 +627,12 @@ def check_se_bwd(st, se, prod, orig, stream):
 
 
 def backward(st, loss, block_check=check_block_bwd, head_grads=None):
-    """loss.backward() with plan._backward_block wrapped: block_check(st, blk, orig) snapshots the block's inputs, runs
-    orig(blk) and returns the block's results for st.bwd (None: nothing recorded).  head_grads(st, grads) sees the head
-    cotangents before the production _head_grads.  A plan with SE blocks also has plan._se_bwd wrapped (check_se_bwd):
-    it runs inside the producing block's _backward_block, in production order."""
+    """loss.backward() with plan._backward_block wrapped: block_check(st, blk, orig) snapshots what the block overwrites,
+    runs orig(blk) and returns the block's results for st.bwd (None: nothing recorded).  head_grads(st, grads) sees the
+    head cotangents before the production _head_grads.  A plan with SE blocks also has plan._se_bwd wrapped
+    (check_se_bwd): it runs inside the producing block's _backward_block, in production order."""
     plan = st.plan
-    st.bwd, st.dy_after_se = {}, {}
+    st.bwd = {}
     orig = plan._backward_block
 
     def wrapped(blk):
@@ -550,7 +673,7 @@ def gather_checks(st, gw_bits=True):
         if blk.is_head and blk.owner is None:
             g = st.g_nhwc[blk.i]
             s = a = 0.0
-            for b0, b1 in chunks(st.batch, 8 * 3 * g[0].numel(), getattr(st, "budget", None)):
+            for b0, b1 in chunks(st.batch, 8 * 3 * g[0].numel(), st.budget):
                 g64 = g[b0:b1].double()
                 s, a = s + g64.sum((0, 1, 2)), a + g64.abs().sum((0, 1, 2))
             gb = plan.garena[blk.gb_off:blk.gb_off + blk.cout]
@@ -573,15 +696,17 @@ def gather_checks(st, gw_bits=True):
                                                       and torch.equal(fc[2].weight.grad, se.gw2.view(se.c, se.cr)))
 
 
-def run_step(st, cot_seed=None, *, prepare=None, linear_fwd=None, loss=None, head_grads=None,
-             block_check=check_block_bwd, gw_bits=True, fwd_check=forward_checks):
+def run_step(st, cot_seed=None, *, budget=None, prepare=None, linear_fwd=None, loss=None, head_grads=None,
+             block_check=check_block_bwd, gw_bits=True):
     """one checked training step of st.model on st.x.
 
-    prepare(st) runs once the checked forward has built st.plan, before any check.  linear_fwd(st, blk) runs right after
-    each plan._linear_fwd launch; the plan must exist to be wrapped, so with linear_fwd the checked step follows one
-    warm-up step that builds it.  loss(st, ps) gives the loss (default: dense_loss with cot_seed); head_grads and
-    block_check as in backward(); gw_bits as in gather_checks(); fwd_check(st) checks the forward."""
+    budget: the float64 bytes of one chunk of images in every check (default CHUNK_BYTES).  prepare(st) runs once the
+    checked forward has built st.plan, before any check.  linear_fwd(st, blk) runs right after each plan._linear_fwd
+    launch; the plan must exist to be wrapped, so with linear_fwd the checked step follows one warm-up step that builds
+    it.  loss(st, ps) gives the loss (default: dense_loss with cot_seed); head_grads and block_check as in backward();
+    gw_bits as in gather_checks()."""
     model = st.model
+    st.budget = CHUNK_BYTES if budget is None else budget
     t0 = time.time()
     plan = None
     if linear_fwd is not None:
@@ -615,332 +740,13 @@ def run_step(st, cot_seed=None, *, prepare=None, linear_fwd=None, loss=None, hea
     by = {b.i: b for b in plan.blocks}
     st.nbt_ok = all(i in by and int(model.module_list[i].BatchNorm2d.num_batches_tracked)
                     == nbt0[i] + (by[i].owner is None and by[i].has_bn) for i in nbt0)
-    fwd_check(st)
+    forward_checks(st)
     torch.cuda.synchronize()
     st.t_fwd = time.time() - t0
     backward(st, loss(st, ps) if loss is not None else dense_loss(st, ps, cot_seed), block_check, head_grads)
     gather_checks(st, gw_bits)
     st.t_total = time.time() - t0
     return st
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# the training step at full batch: the same checks over image chunks, nothing of activation size cloned on the device
-def f64_bytes(c_in, c_out, hw_in, hw_out):
-    """float64 working set per image of a tap-sum reference and its check: the padded operand, its |.|, one shifted
-    copy; value, magnitude and about eight temporaries of the result"""
-    return 8 * (3 * c_in * hw_in + 10 * c_out * hw_out)
-
-
-def ref_bytes(blk):
-    """float64 bytes per image of the block's conv, wgrad and dgrad references and their checks"""
-    gh, gw = (blk.src.h // 2, blk.src.w // 2) if blk.s2d else (blk.src.h, blk.src.w)
-    cin = 27 if blk.i == 0 else blk.cin_eff
-    hw = blk.src.h * blk.src.w
-    out = dict(fwd=f64_bytes(cin, blk.cout, (gh + 2) * (gw + 2), blk.oh * blk.ow),
-               wgrad=f64_bytes(cin, blk.cout, (gh + 2) * (gw + 2), gh * gw))
-    if blk.s2d:        # dz zero-inserted on the input grid, then the mirrored 3x3 taps
-        out["dgrad"] = f64_bytes(blk.cout, blk.src.c, hw, hw) + 8 * hw * blk.cout
-    elif blk.i > 0:
-        out["dgrad"] = f64_bytes(blk.cout, blk.cin, hw, hw)
-    return out
-
-
-def _img_bytes(t):
-    return t[0].numel() * t.element_size()
-
-
-class _LeanDot(torch.autograd.Function):
-    """sum(p * G) whose gradient is G itself: no cotangent-sized temporaries"""
-
-    @staticmethod
-    def forward(ctx, p, g):
-        ctx.g = g
-        return sum((p[b] * g[b]).sum() for b in range(p.shape[0]))
-
-    @staticmethod
-    def backward(ctx, go):
-        assert float(go) == 1.0
-        return ctx.g, None
-
-
-def lean_dense_loss(st, ps, seed):
-    """dense_loss with G drawn in the layout of the fp32 head buffers, so that the cotangent the plan receives is G
-    itself (one copy of G on the device, no product or transpose of it)"""
-    gen = torch.Generator().manual_seed(seed)
-    st.g_nhwc = {}
-    loss = 0.0
-    for blk, p in zip(st.plan.heads, ps):
-        b, na, ny, nx, no = p.shape
-        g = torch.randn((b, na * no, ny, nx), generator=gen).to(p.device)
-        st.g_nhwc[blk.i] = g.permute(0, 2, 3, 1)                              # channel a * no + k
-        loss = loss + _LeanDot.apply(p, g.view(b, na, no, ny, nx).permute(0, 1, 3, 4, 2))
-    return loss
-
-
-def _host(t, chunk_list):
-    """t (an image-major device view) copied to host memory chunk by chunk"""
-    return torch.cat([t[b0:b1].cpu() for b0, b1 in chunk_list])
-
-
-def _max_offset(v, buf):
-    """largest element offset into the buffer buf that its view v addresses"""
-    return v.storage_offset() - buf.storage_offset() + sum((s - 1) * d for s, d in zip(v.shape, v.stride()))
-
-
-def forward_checks_chunked(st):
-    """forward_checks over image chunks of at most st.budget float64 bytes: post hoc on the plan's buffers"""
-    plan, model = st.plan, st.model
-    L = _layout()
-    B = st.batch
-    out = {}
-    st.checked_offsets = {}
-    bits = pad = True
-    col = plan.col
-    for b0, b1 in chunks(B, 8 * 27 * st.h * st.w, st.budget):
-        want = F.unfold(st.x[b0:b1], 3, padding=1).view(b1 - b0, 27, st.h, st.w).permute(0, 2, 3, 1).to(BF16)
-        bits = bits and bitwise(interior(col, 0, 27)[b0:b1], want)
-        pad = pad and bool((interior(col, 27, 37)[b0:b1] == 0).all())
-        del want
-    st.checked_offsets["col"] = (col.numel(), _max_offset(interior(col, 27, 37), col))
-    st.im2col = dict(bits=bits, pad_zero=pad, halo=halo_zero(col))
-    packs = []
-    for blk in plan.blocks:
-        w = _weight(model, blk)
-        wf = w.reshape(blk.cout, 27, 1, 1).contiguous() if blk.i == 0 else w
-        packs.append((blk.i, "fwd", torch.equal(blk.pw, L.pack_weights(blk.fdesc, wf, mode=2 if blk.s2d else 0))))
-        if blk.i > 0:
-            packs.append((blk.i, "dgrad", torch.equal(blk.pwd, L.pack_weights(blk.ddesc, w, mode=3 if blk.s2d else 1))))
-    st.packs = packs
-    ratios = []
-    for blk in plan.blocks:
-        assert blk.owner is None
-        r = {}
-        w64 = _weight(model, blk).to(BF16).double()
-        if blk.i == 0:
-            x, taps, s = interior(plan.col, 0, 27), [(0, 0, w64.reshape(blk.cout, 27).t())], 1
-        else:
-            x, taps, s = vint(blk.src), conv_taps(w64), blk.stride
-        n = conv_updates(blk)
-        cl = chunks(B, ref_bytes(blk)["fwd"], st.budget)
-        if blk.is_head:
-            bias = model.module_list[blk.i].Conv2d.bias.detach().double()
-            got = blk.out.detach().permute(0, 2, 3, 1)
-            worst = []
-            for b0, b1 in cl:
-                want, mag = tapsum(x[b0:b1], taps, blk.oh, blk.ow, s)
-                worst.append(f32_check(got[b0:b1], want + bias, n * 2.0 ** -23 * mag)["max"])
-                del want, mag
-            r["z"] = float(torch.tensor(worst, dtype=F64).max())
-            out[blk.i] = r
-            continue
-        z = interior(blk.z, 0, blk.cout)
-        acc = Acc()
-        for b0, b1 in cl:
-            want, mag = tapsum(x[b0:b1], taps, blk.oh, blk.ow, s)
-            acc.add(z[b0:b1], want, n * 2.0 ** -23 * mag)
-            del want, mag
-        rz = acc.result()
-        r["z"], r["z_bias"] = rz["max"], rz["bias"]
-        cz = chunks(B, 8 * 6 * _img_bytes(z), st.budget)
-        if blk.has_bn:
-            bn = _bn_of(model, blk)
-            rs, ratio = stats_ratios(stats_ref_chunked(z, blk.cout, cz), z.device, blk.cout, blk.sums, blk.mean,
-                                     blk.invstd, blk.scale, blk.shift, st.rm0[blk.i], st.rv0[blk.i], bn.running_mean,
-                                     bn.running_var, bn.weight.detach(), bn.bias.detach(), bn.eps, bn.momentum,
-                                     bn_chain(B, blk.oh, blk.ow, blk.cout)["sums"])
-            r.update(rs)
-            r["mean_over_std"] = ratio
-            ratios.append(ratio)
-        else:
-            bias = model.module_list[blk.i].Conv2d.bias.detach()
-            r["fixed_stats"] = bool((blk.scale == 1).all()) and torch.equal(blk.shift, bias)
-        res = vint(blk.res) if blk.res is not None else None
-        y = interior(blk.y.buf, blk.y.ch_off, blk.cout)
-        acc, copies = Acc(), True
-        for b0, b1 in cz:
-            want_y, t = bn_act_fwd_ref(z[b0:b1], blk.scale, blk.shift, slope_of(model, blk),
-                                       res[b0:b1] if res is not None else None)
-            yc = y[b0:b1]
-            if blk.fuse_up:
-                base = yc[:, ::2, ::2]
-                copies = copies and all(bitwise(yc[:, ry::2, rx::2], base) for ry in range(2) for rx in range(2))
-                yc = base
-            acc.add(yc, want_y, 0.0, t)
-            del want_y, t
-        ry_ = acc.result()
-        r["y"], r["y_bias"] = ry_["max"], ry_["bias"]
-        if blk.fuse_up:
-            r["up_copies"] = copies
-        out[blk.i] = r
-    for blk in plan.blocks:
-        if blk.s2d:
-            src = vint(blk.src)
-            xs = interior(blk.xs, 0, 4 * blk.src.c)
-            out[blk.i]["xs"] = all(bitwise(xs[b0:b1], s2d(src[b0:b1])) for b0, b1 in chunks(B, 4 * _img_bytes(xs), st.budget))
-    bufs = {}
-    for blk in plan.blocks:
-        for v in (blk.src, blk.y if not blk.is_head else None):
-            if v is not None and v.buf is not None:
-                bufs[id(v.buf)] = v.buf
-        if not blk.is_head:
-            bufs[id(blk.z)] = blk.z
-        if blk.s2d:
-            bufs[id(blk.xs)] = blk.xs
-    st.fwd_halo = all(halo_zero(b) for b in bufs.values())
-    st.fwd = out
-    st.max_ratio = max(ratios)
-
-
-def _overlap(a, b):
-    return a is not None and b is not None and a.buf is b.buf and a.ch_off < b.ch_off + b.c and b.ch_off < a.ch_off + a.c
-
-
-def check_block_bwd_chunked(st, blk, orig):
-    """check_block_bwd over image chunks: before the block, only what it overwrites and later checks read goes to host
-    memory (z, which becomes dz in place; the prior of an accumulated gradient view; the channels of a shared gradient
-    buffer outside the block's views); dy is read after the block from buffers the block does not write"""
-    B = st.batch
-    r, snap = {}, {}
-    try:
-        if not blk.is_head:
-            z = interior(blk.z, 0, blk.cout)
-            snap["z"] = _host(z, chunks(B, _img_bytes(z), st.budget))
-            assert not _overlap(blk.gy, blk.gsrc) and not _overlap(blk.gy, blk.gres) and blk.gy.buf is not blk.z
-            if blk.gres is not None and blk.gres_acc:
-                snap["gres_prior"] = _host(vint(blk.gres), chunks(B, _img_bytes(vint(blk.gres)), st.budget))
-        if blk.gsrc is not None:
-            gbuf = blk.gsrc.buf
-            if blk.gsrc_acc:
-                snap["prior"] = _host(vint(blk.gsrc), chunks(B, _img_bytes(vint(blk.gsrc)), st.budget))
-            allowed = torch.zeros(gbuf.shape[-1], dtype=torch.bool)
-            allowed[blk.gsrc.ch_off:blk.gsrc.ch_off + blk.gsrc.c] = True
-            if blk.gres is not None and blk.gres.buf is gbuf:
-                allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
-            snap["outside"] = (~allowed).nonzero().flatten().to(gbuf.device)
-            if len(snap["outside"]):
-                snap["gbuf_outside"] = torch.cat([gbuf[b0:b1].index_select(3, snap["outside"]).cpu()
-                                                  for b0, b1 in chunks(B, _img_bytes(gbuf), st.budget)])
-    except Exception:
-        r["error"] = traceback.format_exc()
-    orig(blk)
-    if "error" in r:
-        return r
-    try:
-        _bwd_checks_chunked(st, blk, snap, r)
-    except Exception:
-        r["error"] = traceback.format_exc()
-    return r
-
-
-def _bwd_checks_chunked(st, blk, snap, r):
-    plan, model = st.plan, st.model
-    B = st.batch
-    dev = st.x.device
-    w64 = _weight(model, blk).to(BF16).double()
-    if blk.is_head:
-        dz = interior(blk.dz, 0, blk.cout)
-        g = st.g_nhwc[blk.i]
-        r["dz_bits"] = all(bitwise(dz[b0:b1], g[b0:b1].to(BF16)) for b0, b1 in chunks(B, 4 * _img_bytes(dz), st.budget))
-        r["dz_pad_zero"] = bool((blk.dz[..., blk.cout:] == 0).all()) and halo_zero(blk.dz)
-    else:
-        dz = interior(blk.z, 0, blk.cout)
-        _, r["dy_mode"] = dy_of(plan, blk, imgs=slice(0, 1))
-        rpp = 2 if r["dy_mode"] == 2 and blk.cout // 8 * 2 <= 640 else 1
-        chain = bn_chain(B, blk.oh, blk.ow, blk.cout, rpp)
-        cl = chunks(B, 8 * 12 * blk.oh * blk.ow * blk.cout, st.budget)
-
-        def parts():
-            for b0, b1 in cl:
-                yield snap["z"][b0:b1].to(dev), dy_of(plan, blk, imgs=slice(b0, b1))[0], dz[b0:b1]
-        rb, near = bn_bwd_check_chunked(parts, blk.cout, blk.bsums, blk.mean, blk.invstd, blk.scale, blk.shift,
-                                        slope_of(model, blk), chain)
-        r["dz"], r["dz_bias"] = rb["max"], rb["bias"]
-        for k in ("dbeta", "dgamma", "dslope", "finite"):
-            r[k] = rb[k]
-        r["near_zero_u"] = near
-        r["n_elems"] = dz.numel()
-        if blk.gres is not None:
-            gres = vint(blk.gres)
-            ok = True
-            for b0, b1 in cl:
-                d = dy_of(plan, blk, imgs=slice(b0, b1))[0]
-                want = (snap["gres_prior"][b0:b1].to(dev).float() + d).to(BF16) if blk.gres_acc else d.to(BF16)
-                ok = ok and bitwise(gres[b0:b1], want)
-            r["gres_bits"] = ok
-        r["dz_halo"] = halo_zero(blk.z)
-    # weight gradient: the float64 reference summed over image chunks
-    if blk.i == 0:
-        x, offs, cin = interior(plan.col, 0, 27), [(0, 0)], 27
-    elif blk.s2d:
-        x, cin = interior(blk.xs, 0, blk.cin_eff), blk.cin_eff
-        offs = [(qy - 1, qx - 1) for qy in range(2) for qx in range(2)]
-    else:
-        x, cin = vint(blk.src), blk.cin
-        p = (blk.k - 1) // 2
-        offs = [(kh - p, kw - p) for kh in range(blk.k) for kw in range(blk.k)]
-    gh, gw_ = x.shape[1], x.shape[2]
-    wr = wm = 0.0
-    for b0, b1 in chunks(B, ref_bytes(blk)["wgrad"], st.budget):
-        a, m = wgrad_ref(x[b0:b1], dz[b0:b1], offs)
-        wr, wm = wr + a, wm + m
-        del a, m
-    plan_w = wgrad_plan(blk.k_eff, blk.cin_pad, blk.cout_pad, B, gh, gw_, gemm_sms())
-    got = blk.dw[:, :blk.cout, :cin]
-    r["wgrad"] = wgrad_ratio(got, wr, wm, plan_w)
-    r["wgrad_rw"] = worst_ratio(got, wr, wm, plan_w["n_add"])
-    if blk.i in st.keep_bwd:
-        st.stash[("wgrad", blk.i)] = dict(x=x.clone(), dz=dz.clone(), offs=offs, got=got.clone(), plan=plan_w,
-                                          want=wr, mag=wm)
-    del wr, wm
-    if blk.i == 0:
-        return
-    gbuf = blk.gsrc.buf
-    if blk.s2d:
-        dxs = interior(blk.dxs, 0, blk.cin_eff)
-        n = 4 * rup(blk.cout, 64) // 16
-        acc, bits = Acc(), True
-        for b0, b1 in chunks(B, ref_bytes(blk)["dgrad"], st.budget):
-            want, mag = s2d_dgrad_ref(dz[b0:b1], w64, blk.src.h, blk.src.w)
-            acc.add(dxs[b0:b1], want, n * 2.0 ** -23 * mag)
-            del want, mag
-            if not blk.dxs_direct:
-                v = d2s(dxs[b0:b1], blk.src.c)
-                want_bits = (snap["prior"][b0:b1].to(dev).float() + v.float()).to(BF16) if blk.gsrc_acc else v
-                bits = bits and bitwise(vint(blk.gsrc)[b0:b1], want_bits)
-        rd = acc.result()
-        r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
-        if not blk.dxs_direct:
-            r["d2s_bits"] = bits
-    else:
-        got = vint(blk.gsrc)
-        n = blk.k * blk.k * rup(blk.cout, 64) // 16
-        acc = Acc()
-        for b0, b1 in chunks(B, ref_bytes(blk)["dgrad"], st.budget):
-            want, mag = tapsum(dz[b0:b1], conv_taps(w64, mirror=True), blk.src.h, blk.src.w)
-            e, t = n * 2.0 ** -23 * mag, 0.0
-            if blk.gsrc_acc:
-                prior = snap["prior"][b0:b1].to(dev).double()
-                want = want + prior
-                t = U * (mag + prior.abs())
-                del prior
-            acc.add(got[b0:b1], want, e, t)
-            del want, mag, e, t
-        rd = acc.result()
-        r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
-    same = True
-    if len(snap["outside"]):
-        for b0, b1 in chunks(B, _img_bytes(gbuf), st.budget):
-            same = same and torch.equal(gbuf[b0:b1].index_select(3, snap["outside"]).cpu(), snap["gbuf_outside"][b0:b1])
-    r["outside_untouched"] = same and halo_zero(gbuf)
-
-
-def run_step_chunked(st, cot_seed, budget, prepare=None):
-    """run_step at a batch whose activations fill the card: forward_checks_chunked, lean_dense_loss and
-    check_block_bwd_chunked, every float64 working set within `budget` bytes"""
-    st.budget = budget
-    return run_step(st, cot_seed, prepare=prepare, loss=lambda s, ps: lean_dense_loss(s, ps, cot_seed),
-                    block_check=check_block_bwd_chunked, fwd_check=forward_checks_chunked)
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -36,7 +36,8 @@ reductions).  What this graph adds, checked here:
                         exact sum, so no element is ambiguous), d bias = sum dz and d slope under the bn_chain bound.
 
 No dilated dgrad of this cfg accumulates (each dilated conv's source gradient has that merge as its only writer), so the
-bound self-test also runs ryolo_dilate_merge with accumulate = 1 on the step's own phase gradient and prior buffer.
+bound self-test also runs ryolo_dilate_merge with accumulate = 1 on the step's own phase gradient and source gradient
+buffer.
 
 Measured on an H100 80GB HBM3 (132 SMs, power limit 700 W, 1980 MHz max SM clock), seeds as below.  `pytest -s` prints
 one line per block (each kernel's worst |err| / bound); the worst per launch kind over the three shapes (block):
@@ -57,7 +58,8 @@ import pytest
 import torch
 
 from builders import m_model, phase_merge, phase_split, ryolo_lib
-from checked_step import Step, check_block_bwd, conv_updates, dy_of, dz_checks, run_step, slope_of
+from checked_step import (Step, check_block_bwd, conv_updates, dy_of, dz_checks, outside_untouched, run_step, slope_of,
+                          snapshot)
 from f64_refs import (BF16, F64, TINY, U, bad_entries, bf16_check, bitwise, bn_chain, check_z, conv_taps, dil_conv,
                       dil_wgrad_ref, f32_check, gemm_sms, halo_zero, interior, nchw, nhwc, passed, rup, s2_refs,
                       sum_check, tapsum, vint, wgrad_ratio, wgrad_ref)
@@ -182,13 +184,7 @@ def check_bwd(st, blk, orig):
         return check_block_bwd(st, blk, orig)
     r, snap = {}, {}
     try:
-        if not blk.is_head:
-            snap["z"] = interior(blk.z, 0, blk.cout).clone()
-            snap["dy"], r["dy_mode"] = dy_of(st.plan, blk)
-            if blk.gres is not None:
-                snap["gres_prior"] = vint(blk.gres).clone()
-        if blk.gsrc is not None:
-            snap["gbuf"] = blk.gsrc.buf.clone()
+        snap = snapshot(st, blk)
         if blk.owner is not None or blk.i in st.owner_of_users:
             snap["dw"] = blk.dw.clone()
     except Exception:
@@ -203,38 +199,32 @@ def check_bwd(st, blk, orig):
     return r
 
 
-def _outside(blk, gbuf, prior_buf):
-    allowed = torch.zeros(gbuf.shape[-1], dtype=torch.bool, device=gbuf.device)
-    allowed[blk.gsrc.ch_off:blk.gsrc.ch_off + blk.gsrc.c] = True
-    if blk.gres is not None and blk.gres.buf is gbuf:
-        allowed[blk.gres.ch_off:blk.gres.ch_off + blk.gres.c] = True
-    return torch.equal(gbuf[..., ~allowed], prior_buf[..., ~allowed]) and halo_zero(gbuf)
-
-
 def _own_bwd_checks(st, blk, snap, r):
     model = st.model
+    dev = st.x.device
     w64 = _w64(st, blk)
     if blk.is_head or blk.has_bn:
         dz = dz_checks(st, blk, snap, r)
     else:
         dz = interior(blk.z, 0, blk.cout)
+        dy, r["dy_mode"] = dy_of(st.plan, blk)          # read after the block, which does not write it
         if blk.owner is not None:        # linear: dz = dy, the shortcut gradient (+)= dy
-            r["dz_bits"] = bitwise(dz, snap["dy"].to(BF16))
+            r["dz_bits"] = bitwise(dz, dy.to(BF16))
         else:                            # block 109: bias + PReLU
             chain = bn_chain(st.batch, blk.oh, blk.ow, blk.cout)
             slope = slope_of(model, blk)
             bias = model.module_list[blk.i].Conv2d.bias.detach()
-            rb = bias_act_bwd_check(snap["z"], snap["dy"], dz, blk.bsums, bias, slope, chain)
+            z = snap["z"].to(dev)
+            rb = bias_act_bwd_check(z, dy, dz, blk.bsums, bias, slope, chain)
             r["dz"], r["dz_bias"], r["dbeta"], r["dslope"] = rb["max"], rb["bias"], rb["dbias"], rb["dslope"]
-            st.stash["b109"] = dict(z=snap["z"], dy=snap["dy"], dz=dz.clone(), sums=blk.bsums.clone(), bias=bias,
-                                    slope=slope, chain=chain)
+            st.stash["b109"] = dict(z=z, dy=dy, dz=dz.clone(), sums=blk.bsums.clone(), bias=bias, slope=slope,
+                                    chain=chain)
         if blk.gres is not None:
-            d = snap["dy"]
-            r["gres_bits"] = bitwise(vint(blk.gres), (snap["gres_prior"].float() + d).to(BF16) if blk.gres_acc
-                                       else d.to(BF16))
+            r["gres_bits"] = bitwise(vint(blk.gres), (snap["gres_prior"].to(dev).float() + dy).to(BF16) if blk.gres_acc
+                                       else dy.to(BF16))
         r["dz_halo"] = halo_zero(blk.z)
     x = vint(blk.src)
-    prior = interior(snap["gbuf"], blk.gsrc.ch_off, blk.gsrc.c)
+    prior = snap["prior"].to(dev) if blk.gsrc_acc else None
     got_dw = blk.dw[:, :blk.cout, :blk.cin]
     sms = gemm_sms()
     if blk.dil is not None:
@@ -254,7 +244,7 @@ def _own_bwd_checks(st, blk, snap, r):
             st.stash["dil_d"] = max(dh, dw)
             st.stash["dil"] = dict(i=blk.i, x=x.clone(), dz=dz.clone(), dh=dh, dw=dw, got=got_dw.clone(),
                                    before=snap["dw"][:, :blk.cout, :blk.cin].clone(), plan=plan_w, v=v.clone(),
-                                   dxp=blk.dxp.clone(), w64=w64, n=n, prior_buf=snap["gbuf"], gsrc=blk.gsrc)
+                                   dxp=blk.dxp.clone(), w64=w64, n=n, gbuf=blk.gsrc.buf.clone(), gsrc=blk.gsrc)
     elif blk.stride == 2:
         # zero-insert path: dz on the even pixels of the input grid, zeros elsewhere
         up = interior(blk.dz_up, 0, blk.cout)
@@ -285,7 +275,7 @@ def _own_bwd_checks(st, blk, snap, r):
             t = U * (mag + prior.double().abs())
         rd = bf16_check(vint(blk.gsrc), want, n * 2.0 ** -23 * mag, t)
         r["dgrad"], r["dgrad_bias"] = rd["max"], rd["bias"]
-    r["outside_untouched"] = _outside(blk, blk.gsrc.buf, snap["gbuf"])
+    r["outside_untouched"] = outside_untouched(st, blk, snap)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -491,7 +481,7 @@ def test_bounds_reject_plausible_bugs(step):
     # (which holds the step's final gradient there): correct against bf16(prior + merge), fails against an overwrite
     L = ryolo_lib()
     g = d["gsrc"]
-    buf = d["prior_buf"].clone()
+    buf = d["gbuf"].clone()
     buf[:, 1:-1, 1:-1, g.ch_off:g.ch_off + g.c] = torch.randn(buf.shape[0], buf.shape[1] - 2, buf.shape[2] - 2, g.c,
                                                               device=buf.device, generator=torch.Generator(
                                                                   device=buf.device).manual_seed(9)).to(BF16)

@@ -7,10 +7,10 @@ outputs with the rounding-bias test, L 2^-24 sum |terms| for reductions, every r
 and L from each launch's own schedule at its batch and grid (wgrad_plan, bn_chain, head_bias_chain).
 
 Batch 3 runs checked_step.run_step as the 608 test does, and the eval forward at the same sizes the per-launch checks of
-test_detect_forward_f64_gpu.py.  Batch 64 fills the card (at 768^2 the activation pool alone is 69.4 GB), so
-run_step_chunked checks the same launches over image chunks of at most BUDGET float64 bytes: the forward post hoc, the
-backward inside the _backward_block wrapper on the live buffers, with only what a block overwrites copied to host memory
-first, and every full reduction (wgrad, BN sums, d gamma / d beta / d slope, head bias) summed in float64 over chunks.
+test_detect_forward_f64_gpu.py.  Batch 64 fills the card (at 768^2 the activation pool alone is 69.4 GB); run_step checks
+the same launches there, over image chunks of at most BUDGET float64 bytes: the forward post hoc, the backward inside the
+_backward_block wrapper on the live buffers, with only what a block overwrites copied to host memory first, and every
+full reduction (wgrad, BN sums, d gamma / d beta / d slope, head bias) summed in float64 over chunks.
 
 bn_act_bwd's dz bound leaves out the elements whose PReLU branch is ambiguous (u within four fp32 ulps of 0); z is bf16,
 so in a channel every z equal to the bf16 value nearest -shift / scale drops out together: up to 0.01 % of a block's
@@ -27,8 +27,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from checked_step import Step, chunks, plan_layout, ref_bytes, run_step, run_step_chunked, schedule_rows
-from f64_refs import (BF16, F64, bitwise, bn_chain, check_z, gemm_sms, interior, passed, sum_check, wgrad_ratio,
+from checked_step import Step, check_block_bwd, chunks, plan_layout, ref_bytes, run_step, schedule_rows
+from f64_refs import (BF16, F64, bitwise, bn_chain, check_z, gemm_sms, interior, passed, sum_check, vint, wgrad_ratio,
                       wgrad_ref)
 from helpers import init_darknet_weights, wgrad_plan
 
@@ -197,7 +197,7 @@ def _big_step(size):
         sms = gemm_sms()
         plans = {b.i: wgrad_plan(3, b.cin_pad, b.cout_pad, BIG_BATCH, b.src.h, b.src.w, sms) for b in k3}
         pick = min(k3, key=lambda b: (plans[b.i]["ksplit"] == 1, not plans[b.i]["short_last"], b.src.h))
-        st.keep_bwd = {pick.i}
+        st.pick, st.pick_plan = pick, plans[pick.i]
         st.stash["bn"] = dict(z=interior(pick.z, 0, pick.cout).clone(), sums=pick.sums.clone(),
                               l=bn_chain(BIG_BATCH, pick.oh, pick.ow, pick.cout)["sums"])
         # the first interior element of the im2col past index 2^31 (its image kept on the host)
@@ -216,8 +216,16 @@ def _big_step(size):
                 b, y, x_ = b + 1, 1, 1
             st.stash["col"] = dict(b=b, y=y, x=x_, c=0, col=col[b].cpu(), img=st.x[b].cpu(),
                                    index=b * per + (y * col.shape[2] + x_) * col.shape[3])
+
+    def block_check(st, blk, orig):
+        r = check_block_bwd(st, blk, orig)
+        if blk is st.pick:      # the picked wgrad's operands and result (st.keep_bwd would keep its other launches' too)
+            st.stash["wgrad"] = dict(x=vint(blk.src).clone(), dz=interior(blk.z, 0, blk.cout).clone(),
+                                     offs=[(kh - 1, kw - 1) for kh in range(3) for kw in range(3)],
+                                     got=blk.dw[:, :blk.cout, :blk.cin].clone(), plan=st.pick_plan)
+        return r
     t0 = time.time()
-    st = run_step_chunked(Step(model, x), 3, BUDGET, prepare=prepare)
+    st = run_step(Step(model, x), 3, budget=BUDGET, prepare=prepare, block_check=block_check)
     res = _keep_step(st, torch.cuda.get_device_properties(0).multi_processor_count)
     res.checked_offsets = st.checked_offsets
     res.seconds = time.time() - t0
@@ -410,10 +418,10 @@ def test_schedule_coverage(sweep, big608, big768):
 def test_bounds_reject_bugs_at_the_new_shapes(sweep, big608, big768):
     found = {}
     # split-K weight gradient at batch 64: the last (shorter) split's partial lost, the last image left out
-    wg = next(v for k, v in big768.stash.items() if k[0] == "wgrad")
+    wg = big768.stash["wgrad"]
     pw = wg["plan"]
     assert pw["ksplit"] > 1, pw
-    want, mag = wg["want"], wg["mag"]
+    want, mag = wgrad_ref(wg["x"], wg["dz"], wg["offs"])
     assert wgrad_ratio(wg["got"], want, mag, pw) <= 1.0
     b, h, w = wg["dz"].shape[:3]
     flat = torch.zeros(b * (h + 2) * (w + 2), dtype=F64, device=want.device)

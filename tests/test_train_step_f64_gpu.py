@@ -8,11 +8,11 @@ Forward: after model(x) every buffer a forward kernel wrote is still there, so e
 plan's own input buffers (the im2col columns, a view, a concat slice, the space-to-depth copy): im2col bit for bit, the
 multi-tensor weight pack bit for bit against ryolo_conv_pack_weights_ex, the raw conv z, the fp32 heads, the batch
 statistics (two-pass float64) with the running-statistics update, and bn_act_fwd / bn_act_fwd_s2d.  Backward:
-plan._backward_block is wrapped (instance attribute) so that each block's inputs are snapshotted, the production code runs
-unchanged, and its outputs are checked right after: bn_act_bwd (dz, d beta, d gamma, d slope, the shortcut gradient), the
-split-K weight gradient and its gather, the dgrad (mode-1 operands; mode-3 operands with ksize -2 and the depth_to_space
-pass) including the accumulate flag and the channels outside the gradient view.  No graph sits between a kernel and its
-reference, so no PReLU kink crossing blurs a check and the bounds are the single-kernel ones:
+plan._backward_block is wrapped (instance attribute) so that what each block overwrites is snapshotted, the production
+code runs unchanged, and its outputs are checked right after: bn_act_bwd (dz, d beta, d gamma, d slope, the shortcut
+gradient), the split-K weight gradient and its gather, the dgrad (mode-1 operands; mode-3 operands with ksize -2 and the
+depth_to_space pass) including the accumulate flag and the channels outside the gradient view.  No graph sits between a
+kernel and its reference, so no PReLU kink crossing blurs a check and the bounds are the single-kernel ones:
 
   A = the same operation in float64 on |operands|,  n = sequential accumulator updates (taps * cin_pad / 16 for the conv
   kernel; for the split-K wgrad the longest chain, wgrad_plan's updates of one split + the ksplit partials added in split

@@ -476,6 +476,9 @@ class Darknet(nn.Module):
             with torch.cuda.device(x.device):
                 pkey = key + (self.training,)
                 if self._pplan is None or self._pplan_key != pkey:
+                    # drop the old plan first: at batch 16 x 608^2 the training plan and the next one (eval, or another
+                    # multi-scale size) do not fit one 80 GB card together
+                    self._pplan = self._pplan_key = None
                     self._pplan = ParityPlan(self, b, h, w, x.device, self.training)
                     self._pplan_key = pkey
                 if self.training:

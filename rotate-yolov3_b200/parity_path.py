@@ -13,6 +13,7 @@ d beta, d slope, split dz, shortcut gradient) -> wgrad (px_wgrad: the wgmma wgra
 planes of dz and x: nine plane blocks, summed by px_unpack_wgrad) -> dgrad (px_conv with mirrored / transposed split weights, fp32 accumulate
 into the source's gradient buffer)."""
 import ctypes
+import weakref
 
 import torch
 
@@ -272,7 +273,9 @@ class ParityPlan:
 class DarknetParityFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, plan, x, names, *params):
-        ctx.plan, ctx.names = plan, names
+        # weak, as in DarknetTrainFn: a caller that keeps this step's heads (whose grad_fn is this node) must not keep the
+        # plan alive after the model has replaced it
+        ctx.plan, ctx.names = weakref.ref(plan), names
         outs = plan.forward(x)
         ctx.gen = plan.gen
         m = plan.model
@@ -286,7 +289,10 @@ class DarknetParityFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        plan = ctx.plan
+        plan = ctx.plan()
+        if plan is None:
+            raise RuntimeError("Darknet parity plan: the plan of this forward was dropped (the model ran another shape or "
+                               "mode, or moved) before its backward")
         check_activations(plan, ctx.gen)
         m = plan.model
         gl = []

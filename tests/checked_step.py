@@ -807,7 +807,11 @@ class Acc:
 
     def add(self, got, want, e, t=0.0):
         self.maxes.append(bf16_check(got, want, e, t)["max"])
-        self.es += float(((got.double() - want) * want.sign()).sum())
+        self.moments(got.double() - want, want)
+
+    def moments(self, err, want):
+        """the whole-tensor sums of the bias ratio: signed error along want, want^2, element count"""
+        self.es += float((err * want.sign()).sum())
         self.w2 += float(want.pow(2).sum())
         self.n += want.numel()
 

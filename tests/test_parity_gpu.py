@@ -258,3 +258,35 @@ def test_parity_plan_rejects_stale_backward():
     with pytest.raises(RuntimeError):
         sum(t.sum() for t in a).backward()
     sum(t.sum() for t in b).backward()
+
+
+def test_parity_plan_does_not_outlive_its_replacement():
+    """a new parity plan is built only after the previous one is gone, even while the caller keeps the last training
+    step's heads (whose grad_fn is the step's autograd node): at batch 16 x 608^2 the training plan and its successor do
+    not fit one 80 GB card together"""
+    import weakref
+
+    from rotate_yolov3_b200 import parity_path as PP
+    m = _parity_model(mini_cfg(64, 48), 5, train=True)
+    plans, alive_at_init = [], []
+    init = PP.ParityPlan.__init__
+
+    def recording_init(self, *a, **k):
+        alive_at_init.append([p() is not None for p in plans])
+        init(self, *a, **k)
+        plans.append(weakref.ref(self))
+
+    with pytest.MonkeyPatch.context() as mp:
+        mp.setattr(PP.ParityPlan, "__init__", recording_init)
+        pred = m(torch.rand(2, 3, 48, 64, device="cuda"))
+        m.eval()
+        with torch.no_grad():
+            m(torch.rand(2, 3, 48, 64, device="cuda"))
+            m(torch.rand(2, 3, 32, 96, device="cuda"))
+        m.train()
+        stale = pred
+        pred = m(torch.rand(1, 3, 48, 64, device="cuda"))
+    assert alive_at_init == [[], [False], [False, False], [False, False, False]], alive_at_init
+    with pytest.raises(RuntimeError, match="dropped"):
+        sum(t.sum() for t in stale).backward()
+    sum(t.sum() for t in pred).backward()

@@ -162,6 +162,35 @@ int ryolo_match_detections(const float* iou, int p, int t, int iou_stride, const
                            const float* tcls, float iou_thres, unsigned char* claimed_scratch,
                            unsigned char* correct, void* stream);
 
+/* The same assignment for every image of a batch, straight from ryolo_detect_select_classes + ryolo_rnms_batched_classes
+ * and with nothing read back to the host (reference test.py:80-151 after non_max_suppression).
+ * dets8 [batch, cap, 8], keep [batch, cap], num_keep [batch]: their output (image b keeps rows keep[b, :num_keep[b]]).
+ * targets [nt, 7] = (image, class, x, y, w, h, theta), x / w normalised by width and y / h by height (letterbox_labels);
+ * image b's targets are the rows with image == b, in row order (rows of other image values belong to no image), scaled to
+ * pixels as test.py:131-133 does.  Each image's kept rows are ordered by confidence descending, class ascending, then row
+ * (a stable segmented sort: the order of nms.detections_per_image), its IoU matrix against its targets is computed with
+ * ryolo_riou_pairwise's arithmetic, bit for bit, and walked as ryolo_match_detections does.
+ * Output: image b's rows go to correct / conf / pcls [*count + sum of the earlier images' num_keep, ...) in that order
+ * (correct uint8, conf = column 5, pcls = column 7), and *count (device int32) is advanced by the batch's kept rows.
+ * class_hist (NULL = none) [nc + 1] int32: += the number of targets (of images 0..batch-1) per class, the last entry
+ * counting classes that are not integers in [0, nc).  iou_scratch [cap * nt] fp32: image b's matrix, row stride t_b (its
+ * target count), starts at cap * (targets of the images before b).  batch <= 4096; class ids < 2^24.
+ * workspace == NULL: writes the workspace size to *workspace_bytes and returns (needs the device, which sizes the sort). */
+int ryolo_match_batched(const float* dets8, const int64_t* keep, const int32_t* num_keep, int batch, int cap,
+                        const float* targets, int nt, int height, int width, float iou_thres, unsigned char* correct,
+                        float* conf, float* pcls, int32_t* count, int32_t* class_hist, int nc, float* iou_scratch,
+                        void* workspace, size_t* workspace_bytes, void* stream);
+
+/* ap_per_class (reference utils/utils.py:200-286) over the first *n_rows of n_cap rows (correct, conf, pcls as
+ * ryolo_match_batched writes them), with n_gt [nc] targets per class.  out [nc, 4] float64 = (p, r, ap, f1) of each class;
+ * a class with n_gt == 0 is not one of the reference's classes and gets zeros.  Rows are ordered by a stable sort on
+ * confidence, descending: ties keep their row order (the reference's np.argsort(-conf) leaves it unspecified).  p, r and
+ * f1 are the reference's float64 values; AP sums its terms in row order (the reference's np.sum is pairwise).  No float
+ * atomics: the results repeat bit for bit.  workspace == NULL: writes the size to *workspace_bytes and returns. */
+int ryolo_ap_per_class(const unsigned char* correct, const float* conf, const float* pcls, const int32_t* n_rows,
+                       int n_cap, const int32_t* n_gt, int nc, double* out, void* workspace, size_t* workspace_bytes,
+                       void* stream);
+
 /* ------------------------------------------------------------------------------------------ *
  * non_max_suppression candidate filter (reference: utils/nms/nms.py:34-40, 55)
  *

@@ -120,6 +120,9 @@ SIGNATURES = {
     "ryolo_riou_pairwise": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _vp, _vp]),
     "ryolo_riou_paired_grad": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "ryolo_match_detections": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _f, _vp, _vp, _vp]),
+    "ryolo_match_batched": (_i, [_vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
+                                 ctypes.POINTER(_sz), _vp]),
+    "ryolo_ap_per_class": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, ctypes.POINTER(_sz), _vp]),
     "ryolo_nms_filter_workspace_bytes": (_sz, [_i]),
     "ryolo_nms_filter": (_i, [_vp, _i, _i, _f, _f, _vp, _i, _vp, _vp, _sz, _vp]),
     "ryolo_yolo_decode": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _f, _f, _i, _vp, _i, _i, _vp, _vp]),

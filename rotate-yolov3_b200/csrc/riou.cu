@@ -196,6 +196,47 @@ __device__ __forceinline__ void derive_box(const float* __restrict__ p, bool in_
   }
 }
 
+// stage A1 for one pair, lane for lane the packed arithmetic of the pairwise kernel: true when the bounding circles of row
+// box r and column box c may overlap (sign of d^2 - R^2)
+__device__ __forceinline__ bool circle_overlap(const float4& r0, const float4& c0) {
+  const float dx = __fadd_rn(c0.x, -r0.x), dy = __fadd_rn(c0.y, -r0.y);
+  const float R = __fadd_rn(c0.z, r0.z), Rn = __fadd_rn(-c0.z, -r0.z);
+  float s = __fmul_rn(dy, dy);
+  s = __fmaf_rn(dx, dx, s);
+  s = __fmaf_rn(R, Rn, s);
+  return (__float_as_uint(s) >> 31) != 0u;
+}
+
+// stage A2 for one pair: false when some box axis separates the boxes (branch-free, one comparison)
+__device__ __forceinline__ bool sat_overlap(const float4& a0, const float4& a1, const float4& b0, const float4& b1) {
+  const float dx = b0.x - a0.x, dy = b0.y - a0.y;
+  const float rx = fmaf(dx, a1.x, dy * a1.y), ry = fmaf(dy, a1.x, -dx * a1.y);      // offset in a's frame
+  const float cd = fmaf(a1.x, b1.x, a1.y * b1.y), sd = fmaf(a1.x, b1.y, -a1.y * b1.x);
+  const float px = fmaf(rx, cd, ry * sd), py = fmaf(ry, cd, -rx * sd);              // offset in b's frame
+  const float C = fabsf(cd), S = fabsf(sd);
+  const float k = -1.0001f;      // tiny relative slack: touching boxes go on to the integral
+  const float m1 = fmaf(k, fmaf(b1.w, S, fmaf(b1.z, C, a1.z)), fabsf(rx));
+  const float m2 = fmaf(k, fmaf(b1.w, C, fmaf(b1.z, S, a1.w)), fabsf(ry));
+  const float m3 = fmaf(k, fmaf(a1.w, S, fmaf(a1.z, C, b1.z)), fabsf(px));
+  const float m4 = fmaf(k, fmaf(a1.w, C, fmaf(a1.z, S, b1.w)), fabsf(py));
+  const float worst = fmaxf(fmaxf(m1, m2), fmaxf(m3, m4));      // > 0: separated on some axis
+  return !(worst > 0.f);
+}
+
+// stage B for one pair that passed A1 and A2: the clamp integral (riou_area.cuh) and the IoU
+__device__ __forceinline__ float pair_iou(const float4& a0, const float4& a1, const float4& b0, const float4& b1, int mode) {
+  float inter = clamp_integral_area2(a0.x, a0.y, a1.x, a1.y, a1.z, a1.w, b0.x, b0.y, b1.x, b1.y, b1.z, b1.w);
+  inter = fminf(inter, fminf(a0.w, b0.w));
+  float uni = a0.w + b0.w - inter;
+  if (mode == RYOLO_IOU_MODE_GIOU) {
+    RBox ra, rb;
+    ra.cx = a0.x; ra.cy = a0.y; ra.c = a1.x; ra.s = a1.y; ra.hw = a1.z; ra.hh = a1.w;
+    rb.cx = b0.x; rb.cy = b0.y; rb.c = b1.x; rb.s = b1.y; rb.hw = b1.z; rb.hh = b1.w;
+    uni = envelope_area(ra, rb);
+  }
+  return uni == 0.f ? 0.f : inter / uni;   // union == 0 -> 0 (utils/utils.py:693-694)
+}
+
 __device__ __forceinline__ void store_row(RiouSmem& sm, int t, const float4& d0, const float4& d1) {
   sm.row0[t] = d0;
   sm.row1[t] = d1;
@@ -293,18 +334,7 @@ __global__ void __launch_bounds__(RIOU_THREADS, 4) riou_pairwise_kernel(const fl
       for (int q = tid, round = 0; q < cnt1; q += RIOU_THREADS, round++) {
         const int e = sm.q1[q];
         const float4 a0 = sm.row0[e >> 7], a1 = sm.row1[e >> 7], b0 = sm.col0[e & (CT - 1)], b1 = sm.col1[e & (CT - 1)];
-        const float dx = b0.x - a0.x, dy = b0.y - a0.y;
-        const float rx = fmaf(dx, a1.x, dy * a1.y), ry = fmaf(dy, a1.x, -dx * a1.y);      // offset in a's frame
-        const float cd = fmaf(a1.x, b1.x, a1.y * b1.y), sd = fmaf(a1.x, b1.y, -a1.y * b1.x);
-        const float px = fmaf(rx, cd, ry * sd), py = fmaf(ry, cd, -rx * sd);              // offset in b's frame
-        const float C = fabsf(cd), S = fabsf(sd);
-        const float k = -1.0001f;      // tiny relative slack: touching boxes go on to the integral
-        const float m1 = fmaf(k, fmaf(b1.w, S, fmaf(b1.z, C, a1.z)), fabsf(rx));
-        const float m2 = fmaf(k, fmaf(b1.w, C, fmaf(b1.z, S, a1.w)), fabsf(ry));
-        const float m3 = fmaf(k, fmaf(a1.w, S, fmaf(a1.z, C, b1.z)), fabsf(px));
-        const float m4 = fmaf(k, fmaf(a1.w, C, fmaf(a1.z, S, b1.w)), fabsf(py));
-        const float worst = fmaxf(fmaxf(m1, m2), fmaxf(m3, m4));      // > 0: separated on some axis
-        kept |= (worst > 0.f ? 0u : 1u) << round;
+        kept |= (sat_overlap(a0, a1, b0, b1) ? 1u : 0u) << round;
       }
       const int cnt = __popc(kept);
       int incl = cnt;
@@ -330,17 +360,7 @@ __global__ void __launch_bounds__(RIOU_THREADS, 4) riou_pairwise_kernel(const fl
       for (int q = tid; q < cnt2; q += RIOU_THREADS) {
         const int e = sm.q2[q];
         const int r = e >> 7, c = e & (CT - 1);
-        const float4 a0 = sm.row0[r], a1 = sm.row1[r], b0 = sm.col0[c], b1 = sm.col1[c];
-        float inter = clamp_integral_area2(a0.x, a0.y, a1.x, a1.y, a1.z, a1.w, b0.x, b0.y, b1.x, b1.y, b1.z, b1.w);
-        inter = fminf(inter, fminf(a0.w, b0.w));
-        float uni = a0.w + b0.w - inter;
-        if (mode == RYOLO_IOU_MODE_GIOU) {
-          RBox ra, rb;
-          ra.cx = a0.x; ra.cy = a0.y; ra.c = a1.x; ra.s = a1.y; ra.hw = a1.z; ra.hh = a1.w;
-          rb.cx = b0.x; rb.cy = b0.y; rb.c = b1.x; rb.s = b1.y; rb.hw = b1.z; rb.hh = b1.w;
-          uni = envelope_area(ra, rb);
-        }
-        sm.out[r * CT + c] = uni == 0.f ? 0.f : inter / uni;   // union == 0 -> 0 (utils/utils.py:693-694)
+        sm.out[r * CT + c] = pair_iou(sm.row0[r], sm.row1[r], sm.col0[c], sm.col1[c], mode);
       }
     }
     __syncthreads();
@@ -376,6 +396,43 @@ __global__ void __launch_bounds__(RIOU_THREADS, 4) riou_pairwise_kernel(const fl
     }
     __syncthreads();
   }
+}
+
+// The same-image (prediction, target) pairs of an evaluation batch in one launch (ryolo_match_batched).  pbox [batch*cap, 5]:
+// image b's num_keep[b] predictions from row b*cap; tbox [*, 5]: the targets grouped by image, image b's from row
+// tstart[b] to tstart[b+1], timg = image of each grouped row.  Image b's matrix is written row-major at
+// iou + cap * tstart[b] (row stride t_b), so the buffer holds cap * nt values whatever the split of the targets.  Each
+// value is the pairwise kernel's for the same boxes, bit for bit: the same derived boxes and the same three stages.
+__global__ void __launch_bounds__(256) riou_image_pairs_kernel(const float* __restrict__ pbox, int cap,
+                                                               const int* __restrict__ num_keep,
+                                                               const float* __restrict__ tbox,
+                                                               const int* __restrict__ timg,
+                                                               const int* __restrict__ tstart, int batch,
+                                                               float* __restrict__ iou) {
+  const long long total = (long long)cap * tstart[batch];
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int b = timg[e / cap];
+    const int t0 = tstart[b], t = tstart[b + 1] - t0;
+    const long long local = e - (long long)cap * t0;
+    const int i = (int)(local / t), j = (int)(local - (long long)i * t);
+    if (i >= num_keep[b]) continue;
+    float4 r0, r1, c0, c1;
+    derive_box(pbox + ((size_t)b * cap + i) * 5, true, FAR_AWAY, r0, r1);
+    derive_box(tbox + (size_t)(t0 + j) * 5, true, -FAR_AWAY, c0, c1);
+    float v = 0.f;
+    if (circle_overlap(r0, c0) && sat_overlap(r0, r1, c0, c1)) v = pair_iou(r0, r1, c0, c1, RYOLO_IOU_MODE_IOU);
+    iou[e] = v;
+  }
+}
+
+int launch_riou_image_pairs(const float* pbox, int cap, const int* num_keep, const float* tbox, const int* timg,
+                            const int* tstart, int batch, int nt, float* iou, cudaStream_t stream) {
+  const long long blocks = ((long long)cap * nt + 255) / 256, limit = (long long)device_sm_count() * 16;
+  if (blocks == 0) return RYOLO_OK;
+  riou_image_pairs_kernel<<<(unsigned)(blocks < limit ? blocks : limit), 256, 0, stream>>>(pbox, cap, num_keep, tbox, timg,
+                                                                                         tstart, batch, iou);
+  RYOLO_LAUNCH_CHECK();
+  return RYOLO_OK;
 }
 
 }  // namespace ryolo

@@ -118,6 +118,21 @@ int ryolo_rnms_batched_classes(const float* dets8, int segments, int cap, const 
                                int64_t* keep_out, int32_t* num_keep, void* workspace, size_t workspace_bytes,
                                void* stream);
 
+/* Cross-scale merge of multi-scale detection (reference: multi_detect, detect.py:81-101): the kept rows of `scales`
+ * results of ryolo_detect_select_classes + ryolo_rnms_batched_classes, mapped back to original-image pixels and
+ * concatenated per image.  dets_host / keep_host / num_keep_host: host arrays of `scales` device pointers, result s
+ * being dets [batch, cap, 8], keep [batch, cap] int64 and num_keep [batch] int32.  table [scales, batch, 3] fp32 =
+ * (padx, pady, gain) of each scale and image (the reference's scale_coords).  out [batch, scales * cap, 8]: image b's
+ * rows are result 0's kept rows dets[b, keep[b, i]] for i < num_keep[b], then result 1's, ... (the offsets are prefix
+ * sums of num_keep on the device), each with x = rint((x - padx) / gain), y = rint((y - pady) / gain),
+ * w = rint(w / gain), h = rint(h / gain) in fp32 (rint: half to even) and theta, conf, class_conf, class copied; the
+ * rest of the image's rows are zero (conf 0: no conf_thres >= 0 selects them).  1 <= scales <= RYOLO_MERGE_MAX_SCALES,
+ * batch <= 65535.  Allocates nothing; capturable in a CUDA graph. */
+#define RYOLO_MERGE_MAX_SCALES 16
+int ryolo_merge_scales(const float* const* dets_host, const int64_t* const* keep_host,
+                       const int32_t* const* num_keep_host, int scales, int batch, int cap, const float* table,
+                       float* out, void* stream);
+
 /* Introspection of the last ryolo_rnms_full_mask call that used `workspace` (valid until the workspace is
  * reused): device pointers to the score-sorted boxes [n,6], the sort permutation order[n]
  * (int32, sorted position -> original index) and the suppression mask [n, ceil(n/64)] uint64 in the

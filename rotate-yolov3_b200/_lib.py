@@ -16,6 +16,7 @@ DT_BF16 = 0
 DT_F32 = 1
 DT_F16 = 2
 DT_U8 = 3
+MERGE_MAX_SCALES = 16          # RYOLO_MERGE_MAX_SCALES
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
@@ -115,6 +116,7 @@ SIGNATURES = {
     "ryolo_detect_select_classes": (_i, [_vp, _i, _i, _i, _f, _f, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "ryolo_rnms_batched_classes_workspace_bytes": (_sz, [_i, _i]),
     "ryolo_rnms_batched_classes": (_i, [_vp, _i, _i, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
+    "ryolo_merge_scales": (_i, [ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp), _i, _i, _i, _vp, _vp, _vp]),
     "ryolo_rnms_debug_views": (_i, [_vp, _i, ctypes.POINTER(_vp), ctypes.POINTER(_vp), ctypes.POINTER(_vp)]),
     "ryolo_riou_paired": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "ryolo_riou_pairwise": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _vp, _vp]),

@@ -63,14 +63,16 @@ class YOLOLayer(nn.Module):
         self.img_size = max(img_size)
         self.stride = self.img_size / max(ng)
         yv, xv = torch.meshgrid([torch.arange(ny), torch.arange(nx)], indexing="ij")
-        self.grid_xy = torch.stack((xv, yv), 2).to(device).type(dtype).view((1, 1, ny, nx, 2))
-        self.anchor_vec = self.anchors.clone().to(device)
+        # non-blocking uploads: an eval loop that alternates sizes (detect.py --multi-scale) re-makes the grids at every
+        # change of size and must not wait for the device each time
+        self.grid_xy = torch.stack((xv, yv), 2).to(device, non_blocking=True).type(dtype).view((1, 1, ny, nx, 2))
+        self.anchor_vec = self.anchors.clone().to(device, non_blocking=True)
         self.anchor_vec[:, :2] /= self.stride
         self.anchor_wh = self.anchor_vec.view(1, self.na, 1, 1, 3).to(device).type(dtype)
-        self.ng = torch.Tensor(ng).to(device)
+        self.ng = torch.Tensor(ng).to(device, non_blocking=True)
         self.nx = nx
         self.ny = ny
-        a = self.anchors.to(device=device, dtype=torch.float32).contiguous()
+        a = self.anchors.to(device=device, dtype=torch.float32, non_blocking=True).contiguous()
         old = getattr(self, "_anchors_dev", None)
         if old is not None and old.device == a.device and old.shape == a.shape:
             # in place: the CUDA graphs of the eval plans of other shapes hold this address in their decode launches
@@ -260,7 +262,7 @@ class Darknet(nn.Module):
         """the eval plans (with their CUDA graphs) of one batch size, or all; the packed weights stay"""
         for key in [k for k in self._plans if batch is None or k[0] == batch]:
             del self._plans[key]
-        if self._plan_cur is not None and self._plan_cur not in self._plans.values():
+        if self._plan_cur is not None and not any(p is self._plan_cur for p in self._plans.values()):
             self._plan_cur = None
             self._graph = self._x_static = self._graph_out = self._graph_kernels = None
 

@@ -6,10 +6,12 @@
 Everything below the tensor plumbing happens in libryolo.so (ryolo_rnms / ryolo_nms_filter)."""
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
 
+_vp = ctypes.c_void_p
 
 def _workspace(nbytes, device):
     # torch's caching allocator is stream-aware; 256-B alignment is guaranteed (512-B blocks)
@@ -206,6 +208,72 @@ def detect_postprocess_classes(io, conf_thres, nms_thres, cap, min_wh=2.0):
                                                  _lib.ptr(keep), _lib.ptr(num), _lib.ptr(ws), ws_bytes, stream)
         _lib.check(st, "ryolo_rnms_batched_classes")
     return {"dets": dets, "counts": counts, "keep": keep, "num_keep": num}
+
+
+def multiscale_sizes(img_size, rng=np.random):
+    """The two sizes detect.py --multi-scale draws for base size img_size (detect.py:54-59): multiples of 32 between
+    about img_size / 1.5 and img_size * 1.3, two distinct, from rng.choice (numpy's global RNG by default, so a seeded
+    numpy draws the reference's sizes).  Returns a list of two ints in the drawn order."""
+    img_sz_min = round(img_size / 32 / 1.5) + 1
+    img_sz_max = round(img_size / 32 * 1.3) - 1
+    return [int(x) for x in rng.choice(range(img_sz_min * 32, (img_sz_max + 1) * 32, 32), 2, False)]
+
+
+STAGE1_NMS_THRES = 0.95      # multi_detect's per-scale NMS threshold (detect.py:90)
+
+
+def detect_multiscale(model, images, sizes, conf_thres, nms_thres, cap):
+    """detect.py --multi-scale (multi_detect, detect.py:16-119) for a whole batch, without host round trips.
+
+    images: list of uint8 [H, W, 3] BGR images (cv2.imread / decode_images; host or CUDA), uploaded once.  For every
+    size s of `sizes` (multiples of 32, square letterbox), largest first: letterbox(images, s), the eval forward of
+    `model`, and the per-scale detection detect_postprocess_classes(io, conf_thres, 0.95, cap) before the next forward
+    overwrites io.  Then, per image, the kept rows of every scale mapped to original-image pixels as
+    scale_coords(...).round() maps them, concatenated in the order of `sizes` (kept rows ascending within a scale), and
+    the second detection detect_postprocess_classes(merged, conf_thres, nms_thres, len(sizes) * cap) on those 8-column
+    rows: as in the reference, its class maximum runs over (class_conf, class index), so a row of class c >= 1 has its
+    conf multiplied by c and comes out as class 1 (INTEGRATION.md §4).  `cap` bounds the candidates per image and scale;
+    the second stage never truncates.
+
+    Returns detect_postprocess_classes' dict (dets, counts, keep, num_keep) in original-image pixels:
+    detections_per_image of it is multi_detect's final_dets per image."""
+    from . import preprocess
+    if model.training:
+        raise ValueError("detect_multiscale runs the eval forward: call model.eval() first")
+    sizes = [int(s) for s in sizes]
+    if not sizes:
+        raise ValueError("detect_multiscale: sizes is empty")
+    if len(sizes) > _lib.MERGE_MAX_SCALES:
+        raise ValueError("detect_multiscale: at most %d sizes, got %d" % (_lib.MERGE_MAX_SCALES, len(sizes)))
+    bad = [s for s in sizes if s <= 0 or s % 32]
+    if bad:
+        raise ValueError("detect_multiscale: every size must be a positive multiple of 32, got %s" % (bad,))
+    if not conf_thres >= 0:
+        raise ValueError("detect_multiscale: conf_thres must be >= 0, got %r" % (conf_thres,))
+    cap = int(cap)
+    if cap < 1:
+        raise ValueError("detect_multiscale: cap must be >= 1, got %d" % cap)
+    device = next(model.parameters()).device
+    srcs = preprocess.upload_images(images, device)
+    bsz, scales = len(srcs), len(sizes)
+    shapes = [tuple(s.shape[:2]) for s in srcs]
+    table = np.empty((scales, bsz, 3), np.float32)     # (padx, pady, gain), each rounded to float32 as scale_coords does
+    for k, s in enumerate(sizes):
+        table[k] = np.array(preprocess.scale_coords_terms((s, s), shapes), np.float64).T
+    stage1 = [None] * scales
+    with torch.cuda.device(device), torch.no_grad():
+        table_dev = preprocess.upload_table(table, device)
+        # largest first: the eval pool of this batch size grows at most once and keeps every size's plan
+        for k in sorted(range(scales), key=lambda k: -sizes[k]):
+            img, _ = preprocess.letterbox(srcs, sizes[k], device=device)
+            io, _ = model(img)
+            stage1[k] = detect_postprocess_classes(io, conf_thres, STAGE1_NMS_THRES, cap)
+        merged = torch.empty((bsz, scales * cap, 8), dtype=torch.float32, device=device)
+        arr = lambda key: (_vp * scales)(*[r[key].data_ptr() for r in stage1])
+        st = _lib.lib.ryolo_merge_scales(arr("dets"), arr("keep"), arr("num_keep"), scales, bsz, cap, _lib.ptr(table_dev),
+                                         _lib.ptr(merged), _lib.stream_ptr(device))
+        _lib.check(st, "ryolo_merge_scales")
+        return detect_postprocess_classes(merged, conf_thres, nms_thres, scales * cap)
 
 
 def detections_per_image(res):

@@ -199,6 +199,76 @@ def _check_image(img, i):
         raise ValueError("letterbox: image %d is empty (%s)" % (i, tuple(img.shape)))
 
 
+def _sources(images, device):
+    """the checked images: CUDA tensors on `device` with rows of packed pixels, host images as C-contiguous numpy"""
+    srcs = []
+    for i, im in enumerate(images):
+        if isinstance(im, torch.Tensor):
+            if im.dtype != torch.uint8:
+                raise ValueError("letterbox: image %d must be uint8, got %s" % (i, im.dtype))
+            _check_image(im, i)
+            if im.is_cuda:
+                if im.device != device:
+                    raise ValueError("letterbox: image %d is on %s, not %s" % (i, im.device, device))
+                if im.stride(2) != 1 or im.stride(1) != 3:
+                    im = im.contiguous()
+                srcs.append(im)
+                continue
+            im = im.numpy()
+        im = np.asarray(im)
+        if im.dtype != np.uint8:
+            raise ValueError("letterbox: image %d must be uint8, got %s" % (i, im.dtype))
+        _check_image(im, i)
+        srcs.append(np.ascontiguousarray(im))
+    return srcs
+
+
+def upload_images(images, device):
+    """The images as uint8 [H, W, 3] CUDA tensors on `device`, for callers that letterbox the same images at several
+    sizes: host images are staged in the pinned buffer and uploaded with one copy on the current stream, CUDA images
+    are returned as they are.  images: as ``letterbox`` takes them."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError("upload_images needs a CUDA device, got %s" % (device,))
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    if not isinstance(images, (list, tuple)) or len(images) == 0:
+        raise ValueError("letterbox: images must be a non-empty list of [H, W, 3] uint8 images")
+    srcs = _sources(images, device)
+    offs, total = [], 0
+    for s in srcs:
+        offs.append(total)
+        total += s.nbytes if isinstance(s, np.ndarray) else 0
+    if total == 0:
+        return srcs
+    with torch.cuda.device(device):
+        pinned = _pinned(device, total)
+        stage = pinned[:total].numpy()
+        for s, o in zip(srcs, offs):
+            if isinstance(s, np.ndarray):
+                stage[o:o + s.nbytes] = s.reshape(-1)
+        dev = _send(pinned, torch.empty(total, dtype=torch.uint8, device=device), device)
+    return [dev[o:o + s.nbytes].view(s.shape) if isinstance(s, np.ndarray) else s for s, o in zip(srcs, offs)]
+
+
+def upload_table(arr, device):
+    """a small host array (a job or coefficient table) as a uint8 device buffer, through the pinned staging buffer"""
+    raw = np.ascontiguousarray(arr).view(np.uint8).reshape(-1)
+    pinned = _pinned(device, raw.size)
+    pinned[:raw.size].numpy()[:] = raw
+    return _send(pinned, torch.empty(raw.size, dtype=torch.uint8, device=device), device)
+
+
+def _send(pinned, dev, device):
+    """one H2D copy of the first dev.numel() staged bytes into dev on the current stream; the staging buffer is free
+    again once the event recorded after the copy has completed (_pinned waits for it)"""
+    dev.copy_(pinned[:dev.numel()], non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record()
+    _staging[device.index] = (pinned, ev)
+    return dev
+
+
 def letterbox(images, new_shape=608, mode="square", dtype=torch.float32, device=None, out=None):
     """The reference's ``letterbox`` + network-input normalisation for a batch of images, on the device.
 
@@ -232,25 +302,7 @@ def letterbox(images, new_shape=608, mode="square", dtype=torch.float32, device=
         out_hw = tuple(int(v) for v in new_shape) if not isinstance(new_shape, int) and len(new_shape) == 2 else None
     if out_hw is None:
         geometry((1, 1), new_shape, mode)                   # raises the ValueError for the bad new_shape / mode
-    srcs = []
-    for i, im in enumerate(images):
-        if isinstance(im, torch.Tensor):
-            if im.dtype != torch.uint8:
-                raise ValueError("letterbox: image %d must be uint8, got %s" % (i, im.dtype))
-            _check_image(im, i)
-            if im.is_cuda:
-                if im.device != device:
-                    raise ValueError("letterbox: image %d is on %s, not %s" % (i, im.device, device))
-                if im.stride(2) != 1 or im.stride(1) != 3:
-                    im = im.contiguous()
-                srcs.append(im)
-                continue
-            im = im.numpy()
-        im = np.asarray(im)
-        if im.dtype != np.uint8:
-            raise ValueError("letterbox: image %d must be uint8, got %s" % (i, im.dtype))
-        _check_image(im, i)
-        srcs.append(np.ascontiguousarray(im))
+    srcs = _sources(images, device)
     bsz = len(srcs)
     meta = torch.empty((bsz, 4), dtype=torch.float64)
     geo = []
@@ -316,11 +368,16 @@ def _upload(srcs, geo, device):
                                     word, word + xt.size, 0)
         word += xt.size + yt.size
     stage[:bsz * _JOB_BYTES] = np.frombuffer(bytes(jobs), np.uint8)
-    dev.copy_(pinned[:total], non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record()
-    _staging[device.index] = (pinned, ev)
-    return dev
+    return _send(pinned, dev, device)
+
+
+def scale_coords_terms(img1_shape, shapes):
+    """the reference's scale_coords terms per original shape, in Python floats: (padx, pady, gain) lists; the
+    transform is x = (x - padx) / gain, y = (y - pady) / gain, w = w / gain, h = h / gain with each term in float32"""
+    gains = [max(img1_shape) / max(s[:2]) for s in shapes]
+    padx = [(img1_shape[1] - s[1] * g) / 2 for s, g in zip(shapes, gains)]
+    pady = [(img1_shape[0] - s[0] * g) / 2 for s, g in zip(shapes, gains)]
+    return padx, pady, gains
 
 
 def scale_coords(img1_shape, coords, img0_shape):
@@ -333,9 +390,7 @@ def scale_coords(img1_shape, coords, img0_shape):
     if (batched and len(shapes) != coords.shape[0]) or coords.dim() not in (2, 3) or coords.shape[-1] < 4:
         raise ValueError("scale_coords: coords [n, >=4] with one shape or [B, n, >=4] with B shapes, got %s and %d "
                          "shapes" % (tuple(coords.shape), len(shapes)))
-    gains = [max(img1_shape) / max(s[:2]) for s in shapes]
-    padx = [(img1_shape[1] - s[1] * g) / 2 for s, g in zip(shapes, gains)]
-    pady = [(img1_shape[0] - s[0] * g) / 2 for s, g in zip(shapes, gains)]
+    padx, pady, gains = scale_coords_terms(img1_shape, shapes)
     view = coords if batched else coords.unsqueeze(0)
     col = lambda v: torch.tensor(v, dtype=coords.dtype).view(-1, 1).to(coords.device, non_blocking=True)
     view[..., 0] -= col(padx)
